@@ -10,7 +10,7 @@ One "step" = one pass of the hot path over one batch of 16 frames:
 `e2e`    : the same metric through the C ABI with HOST buffers: pinned PCM -> H2D -> mel -> forward -> paste -> D2H of the 16
            composited frames, every step (ltb_w2l_step_e2e_async, copies pipelined on a second stream).
 Extra keys on the same JSON line (all measured in this run):
-  roofline          dominant kernels (tcgen05 convs) against the MEASURED burst tensor peak; `sustained` inside it = a >= 2 s
+  roofline          dominant kernels (wgmma convs) against the burst tensor peak; `sustained` inside it = a >= 2 s
                     forward-only loop against the measured sustained peak
   sustained         the same step loop run for >= 3 s with the clock / power trace
   e2e_plugin        fps through the reference-facing hooks exactly as avatars/base_avatar.py calls them:
@@ -20,8 +20,8 @@ Extra keys on the same JSON line (all measured in this run):
   cross_session     the batching scheduler's engine call: 16 slots from 8 different sessions in one forward + paste launch
   musetalk          BASELINE configs[2] (MuseTalk 256x256 batch 8, fp16): value / e2e / roofline of its own
   musetalk512       BASELINE configs[4] (512x512 = 64x64 latents, batch 8) + 8 CONCURRENT sessions per GPU; every rank at N > 1
-  torch_eager_b200  the reference network in stock PyTorch on THIS GPU (fp32 = TF32 cuDNN as the reference runs it, and fp16
-                    channels_last): the existing Blackwell path to beat
+  torch_eager       the reference network in stock PyTorch on THIS GPU (fp32 = TF32 cuDNN as the reference runs it, and fp16
+                    channels_last): the existing GPU path to beat
   cpu_baseline      the oracle port on the host cores (N = 1 only)
 Under torchrun (N > 1) every rank drives its own GPU with its own session (sessions are independent: weak scaling);
 weights are packed on rank 0 and broadcast once with NCCL (the only collective of the design); each rank pins itself to
@@ -51,7 +51,7 @@ BATCH = 16
 SL, SR, FPS = 10, 10, 25   # opt.l, opt.r (20 ms chunks), opt.fps
 FRAME_H, FRAME_W = 720, 1280
 BBOX = (200, 520, 480, 800)
-WORKLOAD = ("wav2lip256 batch 16, 256x256, 1xB200 per rank, 60 s synthetic 16 kHz sine audio, "
+WORKLOAD = ("wav2lip256 batch 16, 256x256, 1xH100 per rank, 60 s synthetic 16 kHz sine audio, "
             "mel + U-Net fwd + paste-back into 720p frames (BASELINE.json configs[1])")
 
 
@@ -59,10 +59,10 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        burst = float(d.get("bf16_tflops", 1661.3))
+        burst = float(d.get("bf16_tflops", 989.0))
         return {"burst": burst, "sustained": float(d.get("bf16_tflops_sustained", burst)), "hbm": float(d["hbm_gbs"]),
                 "src": "MEASURED_PEAKS.json (cuBLAS bf16: best-of-10 burst / 4 s sustained)"}
-    return {"burst": 1650.0, "sustained": 1400.0, "hbm": 6650.0, "src": "fallback (B200_PROFILING.md)"}
+    return {"burst": 989.0, "sustained": 989.0, "hbm": 3350.0, "src": "H100 SXM data sheet (dense fp16, 700 W card; not measured)"}
 
 
 # ------------------------------------------------------------------------------------------------ clocks / placement
@@ -281,7 +281,7 @@ def timed_steps(torch, stream, gate, enqueue, steps, extra_streams=()):
     return ev0.elapsed_time(ev1)
 
 
-def torch_eager_b200(torch, steps=10):
+def torch_eager(torch, steps=10):
     """The reference network (oracle restatement, bit-pinned to the unmodified module) in stock PyTorch on this GPU.
     A baseline leg, like cpu_baseline: nothing of the product path goes through it."""
     from livetalking_b200 import synth
@@ -580,7 +580,7 @@ class MuseTalkBench:
         res = {
             "metric": "lip-sync frames/sec (MuseTalk %dx%d, batch %d, fp16: whisper + PE + UNet + VAE decode + blend paste-back)" % (S, S, B),
             "value": round(world * 1000.0 * B / ms, 2), "unit": "frames/s", "n_gpus": world, "ms_per_step": round(ms, 3), "steps": steps, "warmup": warm,
-            "config": {"workload": "MuseTalk %dx%d batch %d, 1xB200 per rank, fp16 (BASELINE.json configs[%d]); online path of "
+            "config": {"workload": "MuseTalk %dx%d batch %d, 1xH100 per rank, fp16 (BASELINE.json configs[%d]); online path of "
                                    "avatars/musetalk_avatar.py:130-164, latents pre-encoded" % (S, S, B, 2 if hw == 32 else 4),
                        "weights": "synthetic; rank 0 -> all ranks by one NCCL broadcast (%.1f s)" % self.bcast_s if world > 1 else "synthetic"},
             "e2e": {"value": round(world * 1000.0 * B / e2e_ms, 2), "unit": "frames/s", "h2d_bytes_per_step": int(wf2.n * 4 + B * 50 * 384 * 2),
@@ -596,10 +596,10 @@ class MuseTalkBench:
         if batch_sessions > 0:
             res["cross_session"] = self._cross_session(args, hw, batch_sessions, B)
             if self.world == 1:                        # single-GPU probe only (a one-sided failure must not strand other ranks in a collective)
-                try:                                   # eight sessions per launch (batch 64): how far the batch-size lever goes
-                    res["cross_session_x8"] = self._cross_session(args, hw, 2 * batch_sessions, B)
+                try:                                   # six sessions per launch (batch 48, what 80 GB holds next to the other legs)
+                    res["cross_session_x6"] = self._cross_session(args, hw, batch_sessions + batch_sessions // 2, B)
                 except Exception as e:
-                    res["cross_session_x8"] = {"error": repr(e)[:200]}
+                    res["cross_session_x6"] = {"error": repr(e)[:200]}
         return res
 
     def _cross_session(self, args, hw, G, Bs):
@@ -747,6 +747,17 @@ def ultralight_leg(torch, args):
 
 
 # ------------------------------------------------------------------------------------------------ our arm
+def dump_outputs(out_dir: str, frames: np.ndarray) -> None:
+    """The composited frames [B, H, W, 3] u8 of the last timed step, as float32: the mouth box in full (where the network
+    output lands) and a fixed seeded sample of 4 Mi values over the whole batch (all 16 frames would be 177 MB)."""
+    os.makedirs(out_dir, exist_ok=True)
+    y0, y1, x0, x1 = BBOX
+    np.save(os.path.join(out_dir, "frames_bbox.npy"), frames[:, y0:y1, x0:x1].astype(np.float32))
+    pick = np.random.default_rng(0).choice(frames.size, size=1 << 22, replace=False)
+    pick.sort()
+    np.save(os.path.join(out_dir, "frames_sample.npy"), frames.reshape(-1)[pick].astype(np.float32))
+
+
 def run_ours(args):
     import torch
     from livetalking_b200 import engine, synth
@@ -811,6 +822,7 @@ def run_ours(args):
         if idx[0] % (64 * BATCH) == 0:
             torch.cuda.synchronize()
     torch.cuda.synchronize()
+    idx[0] = 0   # the ramp's step count depends on the clock: the warm-up and timed steps start from the same frame index every run
     for k in range(args.warmup):
         step_all(k)
     barrier()
@@ -819,6 +831,8 @@ def run_ours(args):
     sampler.start()
     ms = timed_steps(torch, stream, gate, step_all, args.steps, xstreams)
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, sess.paste_batch(idx[0] - BATCH))
     launches = (sess.launch_count - l0) * args.sessions
     clocks = sampler.stop()
     t = torch.tensor([ms], dtype=torch.float64, device="cuda")
@@ -877,7 +891,7 @@ def run_ours(args):
     if not np.array_equal(chk, pin_out[(e2e_step.n - 1) & 1].array):
         raise RuntimeError("pipelined e2e frames differ from the synchronous path")
 
-    # ---- roofline of the dominant kernels (tcgen05 implicit-GEMM convs)
+    # ---- roofline of the dominant kernels (wgmma implicit-GEMM convs)
     roof = None
     if rank == 0:
         ms_ops, flops, kinds = sess.profile_ops(idx[0])
@@ -896,17 +910,10 @@ def run_ours(args):
             fwd_sus = timed_steps(torch, stream, gate, lambda k: sess.forward_async(idx[0] + k * BATCH), n_f) / n_f
             frac_sus = {"forward_ms_per_step": round(fwd_sus, 4), "achieved": round(algo_flops / fwd_sus / 1e9, 2), "peak": peaks["sustained"],
                         "frac": round(algo_flops / fwd_sus / 1e9 / peaks["sustained"], 4), "seconds": round(n_f * fwd_sus / 1000.0, 2)}
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "conv_traffic.json")
-        if os.path.exists(tp):
-            try:
-                traffic = json.load(open(tp)).get("dram_bytes_per_step")
-            except Exception:
-                traffic = None
         roof = {"bound": "tensor", "achieved": round(achieved, 2), "peak": peaks["burst"], "unit": "TFLOP/s",
-                "frac": round(achieved / peaks["burst"], 4), "traffic": traffic,
+                "frac": round(achieved / peaks["burst"], 4), "traffic": None,
                 "peak_source": peaks["src"] + "; burst peak for this tens-of-ms window, sustained peak for `sustained`",
-                "kernel": "conv_halo_umma + conv_ystack_umma + conv_gather_umma + stem_umma (tcgen05 implicit-GEMM convs): all conv launches of "
+                "kernel": "conv_halo_wgmma + conv_gather_wgmma + stem_umma (wgmma implicit-GEMM convs): all conv launches of "
                           "one step, timed live as %d back-to-back forward-graph replays (CUDA events, session stream, gated)" % K,
                 "forward_ms_per_step": round(fwd_ms, 4), "sustained": frac_sus,
                 "conv_ms_per_step_eager_events": round(float(med[conv].sum()), 4),
@@ -931,7 +938,7 @@ def run_ours(args):
         guarded("e2e_plugin_threads", lambda: plugin_threads(engine, model, (list(frames), list(faces), [tuple(c) for c in coords])))
         guarded("sessions32", lambda: sessions_leg(torch, engine, model, av, audio, 32, max(5, min(args.steps, 20))))
         guarded("cross_session", lambda: cross_session_leg(engine, model, max(5, min(args.steps, 20))))
-        guarded("torch_eager_b200", lambda: torch_eager_b200(torch))
+        guarded("torch_eager", lambda: torch_eager(torch))
     if rank == 0 and world == 1 and not args.quick and not args.no_ultralight:
         guarded("ultralight", lambda: ultralight_leg(torch, args))
     if world > 1 and not args.quick:            # configs[3] at N > 1: 32 sessions on EVERY GPU (aggregate over ranks)
@@ -1008,6 +1015,8 @@ def main():
     ap.add_argument("--quick", action="store_true", help="contract line only (value / e2e / roofline), no extra legs")
     ap.add_argument("--sessions", type=int, default=1, help="concurrent avatar sessions per GPU in the `value` leg (each batch 16, own stream)")
     ap.add_argument("--dump-ops", default=None, help="write per-op timings (json)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the frames the last timed step composited as DIR/<name>.npy (float32, same inputs every run)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Secondary benchmark: MuseTalk 256x256, batch 8 (BASELINE.json configs[2]) on one B200.
+"""Secondary benchmark: MuseTalk 256x256, batch 8 (BASELINE.json configs[2]) on one H100.
 
     python bench_musetalk.py [--steps K] [--warmup W] [--batch 8]
 
@@ -112,7 +112,7 @@ def main():
         "breakdown_ms": {"whisper": round(ms_whisper, 3), "unet_plus_vae_decode": round(ms_unet_vae, 3), "blend_paste": round(ms_paste, 3),
                          "vae_encode_x2": round(ms_enc, 3)},
         "gpu_launches_per_step": int(launches), "model_load_s": round(load_s, 1), "peak_tflops": peak,
-        "config": {"workload": "MuseTalk 256x256 batch %d, VAE enc -> UNet -> VAE dec, 1xB200, fp16 (BASELINE.json configs[2])" % B},
+        "config": {"workload": "MuseTalk 256x256 batch %d, VAE enc -> UNet -> VAE dec, 1xH100, fp16 (BASELINE.json configs[2])" % B},
     }
     print(json.dumps(out))
     ctx.close()

@@ -1,5 +1,5 @@
 /*
- * libltb200 — C ABI of the B200-native lip-sync engine (sm_100a only, no CPU fallback).
+ * libltb200 — C ABI of the H100-native lip-sync engine (sm_90a only, no CPU fallback).
  *
  * This is the drop-in boundary behind LiveTalking's avatar plugin surface.  Every entry point names the
  * reference interface it replaces (paths relative to the lipku/LiveTalking tree).  Conventions:
@@ -183,7 +183,7 @@ int ltb_capture_end(ltb_ctx* c, ltb_graph** out);
 int ltb_graph_launch(ltb_ctx* c, ltb_graph* g);
 int ltb_graph_destroy(ltb_graph* g);
 
-/* conv / linear / batched GEMM on the tcgen05 kernels (nn.Conv2d, nn.Linear, attention Q.K^T and P.V):
+/* conv / linear / batched GEMM on the wgmma kernels (nn.Conv2d, nn.Linear, attention Q.K^T and P.V):
  * out[pix, co] = act(sum_{tap,ci} in[pix*s + tap - pad, ic_off+ci] * w[co, w_koff + tap*Cin + ci] + bias[co] (+ res[pix, co]))
  * w: fp16 [Cout][Ktot] (K-major rows); w_tap: optional tap-major copy [9][Cout][Cin] enabling the TMA halo kernel for
  * 3x3 s1 p1; bias may be NULL (zero).  zbatch > 1 runs zbatch independent GEMMs (z = zo*zdiv + zi) with element
@@ -224,7 +224,7 @@ int ltb_op_eltwise(ltb_ctx* c, const void* x, const void* y, long long n, long l
 int ltb_op_upsample2x(ltb_ctx* c, const void* x, int N, int H, int W, int C, void* out);
 int ltb_op_copy_channels(ltb_ctx* c, const void* src, long long rows, int C, int SCtot, int sc_off, void* dst, int DCtot, int dc_off);
 int ltb_op_transpose_heads(ltb_ctx* c, const void* v, int B, int n_keys, int Ctot, int c_off, int heads, int d, int n_pad, void* vt);
-/* Fused multi-head attention out = softmax(scale * Q K^T) V on tcgen05 (scores stay in TMEM / shared memory): the diffusers Attention
+/* Fused multi-head attention out = softmax(scale * Q K^T) V on wgmma (scores stay in registers): the diffusers Attention
  * blocks of the UNet (avatars/musetalk/models/unet.py:29-48) and the Whisper encoder layers (whisper/audio2feature.py:106-117).
  * q [B][nq] rows of q_pitch halves, k [B][kv_rows] rows of kv_pitch halves, head h at columns [h*d, (h+1)*d); vt = the
  * ltb_op_transpose_heads output [B*heads][d][n_pad]; keys >= valid get probability 0; out [B*nq][out_pitch], head h at columns

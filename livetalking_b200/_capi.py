@@ -136,12 +136,6 @@ _SIGS = {
                                        C.POINTER(C.c_float)]),
 }
 
-# hardware probes: only in lib/libltb200_diag.so (include/ltb200_diag.h)
-DIAG_SIGS = {
-    "ltb_umma_probe": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
-    "ltb_umma_probe_noswz": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
-}
-
 EXPORTED_SYMBOLS = tuple(_SIGS)
 
 _lib = None
@@ -153,17 +147,12 @@ def lib() -> C.CDLL:
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise LtbError(f"{LIB_PATH} not found: build it with `python -m livetalking_b200.build` "
-                           "(sm_100a CUDA library; there is no CPU fallback)")
+                           "(sm_90a CUDA library; there is no CPU fallback)")
         l = C.CDLL(LIB_PATH)
         for name, (res, args) in _SIGS.items():
             fn = getattr(l, name)
             fn.restype = res
             fn.argtypes = args
-        for name, (res, args) in DIAG_SIGS.items():      # present in the diagnostic build only
-            fn = getattr(l, name, None)
-            if fn is not None:
-                fn.restype = res
-                fn.argtypes = args
         _lib = l
     return _lib
 

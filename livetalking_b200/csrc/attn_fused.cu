@@ -1,28 +1,25 @@
-// Fused multi-head attention on tcgen05 (sm_100a): softmax(scale * Q K^T) V with the score matrix S living only in TMEM and
-// shared memory — replaces the three-kernel path (batched QK^T GEMM -> fp16 S in HBM -> softmax kernel -> batched PV GEMM)
+// Fused multi-head attention on Hopper wgmma (sm_90a): softmax(scale * Q K^T) V with the score matrix S living only in
+// registers — replaces the three-kernel path (batched QK^T GEMM -> fp16 S in HBM -> softmax kernel -> batched PV GEMM)
 // of the diffusers Attention blocks (UNet self / cross attention, avatars/musetalk/models/unet.py:29-48 -> diffusers
-// BasicTransformerBlock) and the Whisper encoder layers (avatars/musetalk/whisper/audio2feature.py:106-117).
+// BasicTransformerBlock) and the Whisper / HuBERT encoder layers (avatars/musetalk/whisper/audio2feature.py:106-117).
 //
-// One CTA = 128 queries of one (batch, head).  TWO passes over the keys instead of an online rescale of O:
-//   pass 1: S_t = Q K_t^T (tcgen05.mma, M=128 queries, N=128 keys, K = head dim) -> TMEM; the softmax warps read their row
-//           (one query per thread, one TMEM lane) and keep the running maximum m and the sum l = sum exp(scale*(s - m));
-//   pass 2: S_t is recomputed (the head dim is 48..160: re-running 3..10 K steps is cheaper than keeping or rescaling
-//           anything), P_t = exp(scale*(s - m)) / l is written as fp16 into shared memory in the canonical K-major 128B-swizzled
-//           layout and consumed as the A operand of O += P_t V_t (M=128, N = head dim, K=128 keys) — O accumulates in TMEM.
+// One CTA = 128 queries of one (batch, head); each of the two consumer warpgroups owns 64 of them.  TWO passes over the keys
+// instead of an online rescale of O:
+//   pass 1: S_t = Q K_t^T (wgmma, M=64 queries per warpgroup, N=128 keys, K = head dim) in registers; every thread keeps the
+//           running maximum m and the sum l = sum exp(scale*(s - m)) of its two query rows (merged over the four lanes of a row);
+//   pass 2: S_t is recomputed (the head dim is 16..160: re-running 1..10 K steps is cheaper than keeping or rescaling
+//           anything), P_t = exp(scale*(s - m)) / l is packed to fp16 straight into the A-operand register fragments of
+//           O += P_t V_t (M=64, N = head dim, K=128 keys) — O accumulates in registers.
 // Q / K tiles come by TMA straight out of the fused qkv (or q / kv) projection buffers (4-D maps (d, token, head, batch); the
 // box is 64 channels wide and the tensor's channel extent is the head dim, so the padding up to 64 is zero-filled); V^T tiles from
-// the [B*H][d][keys] buffer transpose_heads writes.  TMEM: 128 columns of S + d columns of O (<= 256 for d <= 128: two CTAs per SM
-// overlap each other's MMA / softmax phases, so the per-CTA pipeline is kept simple and serial).
-// Roles (320 threads): warp 0 TMA producer, warp 1 MMA issuer, warps 2-9 softmax + epilogue: TMEM lane quarter = warp % 4, and the two
-// warps of a quarter split the 128 key columns of a tile (ncu r02q: with four softmax warps the kernel sat at 32 % of the SFU pipe and
-// 37 % issue utilisation — latency bound on one warp per scheduler); their row statistics are merged once, after pass 1.
+// the [B*H][d][keys] buffer transpose_heads writes.  Roles (288 threads): warps 0-7 consumers, warp 8 TMA producer.
 #include <cuda.h>
 
 #include <mutex>
 
 #include "ltb_internal.h"
 #include "ops.h"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace ltb {
 
@@ -35,7 +32,7 @@ struct alignas(64) AttnParams {
   float scale_log2e;   // scale * log2(e): probabilities are exp2((s - m) * scale_log2e)
 };
 
-constexpr int kAttnThreads = 320;
+constexpr int kAttnThreads = 288;
 constexpr int kTileBytes = 128 * 128;   // 128 rows x 64 fp16
 
 __device__ __forceinline__ float ex2f(float x) {
@@ -44,56 +41,39 @@ __device__ __forceinline__ float ex2f(float x) {
   return y;
 }
 
-__global__ void __launch_bounds__(kAttnThreads) attn_fused_kernel(const __grid_constant__ AttnParams p) {
+template <int D>
+__global__ void __launch_bounds__(kAttnThreads, 1) attn_fused_kernel(const __grid_constant__ AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t q_full, k_full[2], k_empty[2], v_full, v_empty, s_full, s_empty, p_full, p_empty, o_full;
-  __shared__ uint32_t tmem_slot;
-  __shared__ float2 row_stat[2][128];      // (max, sum) of each query row over one half of the key columns
+  __shared__ __align__(8) uint64_t q_full, k_full[2], k_empty[2], v_full, v_empty;
 
   pdl_launch_dependents();   // the output projection (a PDL-launched conv kernel) may start its prologue under this kernel's tail
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int q0 = blockIdx.x * 128, bh = blockIdx.y, b = bh / p.H, h = bh - b * p.H;
-  const int chunks = (p.d + 63) / 64;                 // 64-channel K chunks of the QK^T contraction
+  constexpr int chunks = (D + 63) / 64;               // 64-channel K chunks of the QK^T contraction
   const int nkt = (p.valid + 127) / 128;              // key tiles (keys >= valid are masked; rows beyond the tensor come back as zeros)
   const uint32_t KS = (uint32_t)p.kstages;            // K ring depth (1 when the head dim needs three chunks: shared memory)
   const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t q_smem = smem0;                                       // chunks x [128 x 128 B]
-  const uint32_t k_smem = q_smem + chunks * kTileBytes;                // 2 stages x chunks x [128 x 128 B]
+  const uint32_t k_smem = q_smem + chunks * kTileBytes;                // KS stages x chunks x [128 x 128 B]
   const uint32_t v_smem = k_smem + KS * chunks * kTileBytes;           // 2 key blocks x [d rows x 128 B]
-  const uint32_t v_blk = ((uint32_t)p.d * 128u + 1023u) & ~1023u;
-  const uint32_t p_smem = v_smem + 2 * v_blk;                          // 2 key blocks x [128 x 128 B]
-  uint8_t* const p_ptr = smem_raw + (p_smem - smem_u32(smem_raw));
-  const uint32_t tcols = (128 + p.d <= 256) ? 256u : 512u;
+  constexpr uint32_t v_blk = ((uint32_t)D * 128u + 1023u) & ~1023u;
 
   if (tid == 0) {
     mbar_init(smem_u32(&q_full), 1);
     for (int s = 0; s < 2; ++s) {
       mbar_init(smem_u32(&k_full[s]), 1);
-      mbar_init(smem_u32(&k_empty[s]), 1);
+      mbar_init(smem_u32(&k_empty[s]), 8);   // one arrival per consumer warp
     }
     mbar_init(smem_u32(&v_full), 1);
-    mbar_init(smem_u32(&v_empty), 1);
-    mbar_init(smem_u32(&s_full), 1);
-    mbar_init(smem_u32(&s_empty), 8);     // the eight softmax warps
-    mbar_init(smem_u32(&p_full), 8);
-    mbar_init(smem_u32(&p_empty), 1);
-    mbar_init(smem_u32(&o_full), 1);
+    mbar_init(smem_u32(&v_empty), 8);
     mbar_fence_init();
     tma_prefetch_desc(&p.tm_q);
     tma_prefetch_desc(&p.tm_k);
     tma_prefetch_desc(&p.tm_vt);
   }
-  if (warp == 1) {
-    tmem_alloc(smem_u32(&tmem_slot), tcols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t tmem_s = tmem, tmem_o = tmem + 128;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // =============================================================== TMA producer
     if (lane == 0) {
       mbar_arrive_expect_tx(smem_u32(&q_full), chunks * kTileBytes);
@@ -108,169 +88,113 @@ __global__ void __launch_bounds__(kAttnThreads) attn_fused_kernel(const __grid_c
             tma_load_4d(k_smem + (s * chunks + c) * kTileBytes, &p.tm_k, smem_u32(&k_full[s]), c * 64, kt * 128, h, b);
           if (pass == 1) {
             mbar_wait(smem_u32(&v_empty), (kt & 1u) ^ 1u);
-            mbar_arrive_expect_tx(smem_u32(&v_full), 2 * p.d * 128);
+            mbar_arrive_expect_tx(smem_u32(&v_full), 2 * D * 128);
             for (int j = 0; j < 2; ++j) tma_load_3d(v_smem + j * v_blk, &p.tm_vt, smem_u32(&v_full), kt * 128 + j * 64, 0, bh);
           }
         }
     }
-  } else if (warp == 1) {
-    // =============================================================== MMA issuer (warp-uniform, elected-lane predication)
-    const uint32_t leader = elect_one() ? 1u : 0u;
-    const uint32_t idesc_s = umma_idesc_f16(128, 128);
-    const uint32_t idesc_o = umma_idesc_f16(128, p.d);
-    constexpr uint32_t kDescHi = (1024u >> 4) | (1u << 14) | (2u << 29);   // SBO = 1024 B, version 1, SWIZZLE_128B
-    const int ksteps_last = ((p.d - 1) % 64) / 16 + 1;
-    mbar_wait(smem_u32(&q_full), 0);
-    uint32_t ki = 0, si = 0;
-    for (int pass = 0; pass < 2; ++pass)
-      for (int kt = 0; kt < nkt; ++kt, ++ki, ++si) {
-        const uint32_t s = ki % KS;
-        mbar_wait(smem_u32(&k_full[s]), (ki / KS) & 1u);
-        mbar_wait(smem_u32(&s_empty), (si & 1u) ^ 1u);      // the softmax warps have read the previous S tile
-        tc_fence_after();
-        for (int c = 0; c < chunks; ++c) {
-          const uint32_t a_lo = (((q_smem + c * kTileBytes) & 0x3FFFFu) >> 4) | (1u << 16);
-          const uint32_t b_lo = (((k_smem + (s * chunks + c) * kTileBytes) & 0x3FFFFu) >> 4) | (1u << 16);
-          const int ks = (c == chunks - 1) ? ksteps_last : 4;
-          for (int k = 0; k < ks; ++k)
-            umma_f16_lohi_if(leader, tmem_s, a_lo + k * 2, kDescHi, b_lo + k * 2, kDescHi, idesc_s, (c | k) ? 1u : 0u);
-        }
-        umma_commit_if(leader, smem_u32(&k_empty[s]));
-        umma_commit_if(leader, smem_u32(&s_full));
-        if (pass == 1) {
-          // O += P_kt V_kt : A = the fp16 probabilities the softmax warps wrote, B = V^T tile (d rows x 128 keys)
-          mbar_wait(smem_u32(&p_full), kt & 1u);
-          mbar_wait(smem_u32(&v_full), kt & 1u);
-          tc_fence_after();
-          for (int j = 0; j < 2; ++j) {
-            const uint32_t a_lo = (((p_smem + j * kTileBytes) & 0x3FFFFu) >> 4) | (1u << 16);
-            const uint32_t b_lo = (((v_smem + j * v_blk) & 0x3FFFFu) >> 4) | (1u << 16);
-            for (int k = 0; k < 4; ++k)
-              umma_f16_lohi_if(leader, tmem_o, a_lo + k * 2, kDescHi, b_lo + k * 2, kDescHi, idesc_o, (kt | j | k) ? 1u : 0u);
-          }
-          umma_commit_if(leader, smem_u32(&p_empty));
-          umma_commit_if(leader, smem_u32(&v_empty));
-        }
-      }
-    umma_commit_if(leader, smem_u32(&o_full));
-    __syncwarp();
-  } else {
-    // =============================================================== softmax + epilogue: one query row x 64 key columns per thread
-    const int q = warp & 3;                        // TMEM lane quarter of this warp
-    const int half = (warp - 2) >> 2;              // which 64 key columns of every tile
-    const int row = q * 32 + lane;                 // query row inside the tile
-    const uint32_t trow = ((uint32_t)(q * 32) << 16);
-    const int cbase = half * 64;
-    float m = -INFINITY, l = 0.f;
-    uint32_t si = 0;
-    // ---- pass 1: running maximum and sum over this thread's columns
-    for (int kt = 0; kt < nkt; ++kt, ++si) {
-      mbar_wait(smem_u32(&s_full), si & 1u);
-      tc_fence_after();
-      const int lim0 = p.valid - kt * 128 - cbase;     // columns [0, lim0) of this thread's 64 are real keys
-      if (lim0 > 0) {
-        uint32_t v0[32], v1[32];
-        tmem_ld32(tmem_s + trow + cbase, v0);
-        tmem_ld32(tmem_s + trow + cbase + 32, v1);
-        tmem_ld_wait();
-        float tmax = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          if (i < lim0) tmax = fmaxf(tmax, __uint_as_float(v0[i]));
-          if (i + 32 < lim0) tmax = fmaxf(tmax, __uint_as_float(v1[i]));
-        }
-        const float m_new = fmaxf(m, tmax);
-        float lsum = 0.f;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          if (i < lim0) lsum += ex2f((__uint_as_float(v0[i]) - m_new) * p.scale_log2e);
-          if (i + 32 < lim0) lsum += ex2f((__uint_as_float(v1[i]) - m_new) * p.scale_log2e);
-        }
-        l = l * ex2f((m - m_new) * p.scale_log2e) + lsum;   // m = -inf on the first tile: ex2(-inf) = 0
-        m = m_new;
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&s_empty));
-    }
-    // ---- merge the two column halves of every row (named barrier over the 256 softmax threads)
-    row_stat[half][row] = make_float2(m, l);
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    {
-      const float2 o = row_stat[half ^ 1][row];
-      const float mm = fmaxf(m, o.x);
-      // a half with no valid key at all has m = -inf, l = 0: its term vanishes (ex2(-inf) = 0; mm is finite since valid >= 1)
-      l = (m == -INFINITY ? 0.f : l * ex2f((m - mm) * p.scale_log2e)) + (o.x == -INFINITY ? 0.f : o.y * ex2f((o.x - mm) * p.scale_log2e));
-      m = mm;
-    }
-    const float inv_l = 1.f / l;
-    // ---- pass 2: probabilities -> shared memory (A operand of the PV product); this thread fills rows of key block `half`
-    for (int kt = 0; kt < nkt; ++kt, ++si) {
-      mbar_wait(smem_u32(&s_full), si & 1u);
-      tc_fence_after();
-      mbar_wait(smem_u32(&p_empty), (kt & 1u) ^ 1u);     // the PV MMAs of the previous tile have consumed P
-      const int lim0 = p.valid - kt * 128 - cbase;
-      uint8_t* prow = p_ptr + half * kTileBytes + row * 128;
-#pragma unroll
-      for (int c0 = 0; c0 < 64; c0 += 32) {
-        uint32_t v[32];
-        if (lim0 > c0) {
-          tmem_ld32(tmem_s + trow + cbase + c0, v);
-          tmem_ld_wait();
-        }
-        const int lim = lim0 - c0;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {          // 8 keys = one 16-byte chunk of the K-major row
-          uint32_t w[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const int i = g * 8 + 2 * u;
-            const float a = (i < lim) ? ex2f((__uint_as_float(v[i]) - m) * p.scale_log2e) * inv_l : 0.f;
-            const float c = (i + 1 < lim) ? ex2f((__uint_as_float(v[i + 1]) - m) * p.scale_log2e) * inv_l : 0.f;
-            w[u] = f32x2_to_f16x2_sat(a, c);
-          }
-          const int chunk = (c0 >> 3) + g;                  // 0..7 inside the 64-key block
-          *reinterpret_cast<uint4*>(prow + ((chunk ^ (row & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-      }
-      fence_proxy_async_smem();        // generic-proxy writes of P visible to the tensor core's async proxy
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(smem_u32(&p_full));
-        mbar_arrive(smem_u32(&s_empty));
-      }
-    }
-    // ---- epilogue: O (fp32, TMEM) -> fp16 rows of the output
-    mbar_wait(smem_u32(&o_full), 0);
-    tc_fence_after();
-    const int qi = q0 + row;
-    __half* orow = p.out + ((size_t)b * p.nq + qi) * p.out_pitch + h * p.d;
-    for (int c0 = half * 16; c0 < p.d; c0 += 32) {     // the two warps of a quarter alternate 16-column groups
-      uint32_t v[16];
-      tmem_ld16(tmem_o + trow + c0, v);
-      tmem_ld_wait();
-      if (qi < p.nq) {
-        uint4 o0, o1;
-        o0.x = f32x2_to_f16x2_sat(__uint_as_float(v[0]), __uint_as_float(v[1]));
-        o0.y = f32x2_to_f16x2_sat(__uint_as_float(v[2]), __uint_as_float(v[3]));
-        o0.z = f32x2_to_f16x2_sat(__uint_as_float(v[4]), __uint_as_float(v[5]));
-        o0.w = f32x2_to_f16x2_sat(__uint_as_float(v[6]), __uint_as_float(v[7]));
-        o1.x = f32x2_to_f16x2_sat(__uint_as_float(v[8]), __uint_as_float(v[9]));
-        o1.y = f32x2_to_f16x2_sat(__uint_as_float(v[10]), __uint_as_float(v[11]));
-        o1.z = f32x2_to_f16x2_sat(__uint_as_float(v[12]), __uint_as_float(v[13]));
-        o1.w = f32x2_to_f16x2_sat(__uint_as_float(v[14]), __uint_as_float(v[15]));
-        *reinterpret_cast<uint4*>(orow + c0) = o0;
-        *reinterpret_cast<uint4*>(orow + c0 + 8) = o1;
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, tcols);
+  // =============================================================== consumers: warpgroup wg owns queries [64 wg, 64 wg + 64)
+  const int wg = warp >> 2, wq = warp & 3;
+  const int cq = 2 * (lane & 3);
+  constexpr uint32_t kHi = wgmma_hi_128b(1024);   // SBO = 1024 B, SWIZZLE_128B
+  constexpr int ksteps_last = ((D - 1) % 64) / 16 + 1;
+  float s_acc[64];
+  uint32_t ki = 0;
+  // S = Q K^T of key tile kt into s_acc; hands the K stage back
+  auto scores = [&]() {
+    const uint32_t s = ki % KS;
+    mbar_wait(smem_u32(&k_full[s]), (ki / KS) & 1u);
+#pragma unroll
+    for (int i = 0; i < 64; ++i) s_acc[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < chunks; ++c) {
+      const uint32_t a_lo = wgmma_lo(q_smem + c * kTileBytes + wg * 64 * 128);
+      const uint32_t b_lo = wgmma_lo(k_smem + (s * chunks + c) * kTileBytes);
+      const int ks = (c == chunks - 1) ? ksteps_last : 4;
+#pragma unroll
+      for (int k = 0; k < ks; ++k) Wgmma<128>::ss(s_acc, wgmma_lohi(a_lo + k * 2, kHi), wgmma_lohi(b_lo + k * 2, kHi), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s_acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&k_empty[s]));
+    ++ki;
+  };
+  mbar_wait(smem_u32(&q_full), 0);
+  // ---- pass 1: running maximum and sum of the two rows (hh = 0, 1) of this thread
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  for (int kt = 0; kt < nkt; ++kt) {
+    scores();
+    const int lim = p.valid - kt * 128;   // key columns [0, lim) of this tile are real keys
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float tmax = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * i + cq + e < lim) tmax = fmaxf(tmax, s_acc[4 * i + 2 * hh + e]);
+      tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 1));
+      tmax = fmaxf(tmax, __shfl_xor_sync(0xffffffffu, tmax, 2));
+      const float m_new = fmaxf(m[hh], tmax);   // finite: every tile holds at least one valid key
+      float lsum = 0.f;
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * i + cq + e < lim) lsum += ex2f((s_acc[4 * i + 2 * hh + e] - m_new) * p.scale_log2e);
+      lsum += __shfl_xor_sync(0xffffffffu, lsum, 1);
+      lsum += __shfl_xor_sync(0xffffffffu, lsum, 2);
+      l[hh] = l[hh] * ex2f((m[hh] - m_new) * p.scale_log2e) + lsum;   // m = -inf on the first tile: ex2(-inf) = 0
+      m[hh] = m_new;
+    }
+  }
+  const float inv_l[2] = {1.f / l[0], 1.f / l[1]};
+  // ---- pass 2: probabilities (fp16 A fragments in registers) times V
+  float o_acc[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) o_acc[i] = 0.f;
+  for (int kt = 0; kt < nkt; ++kt) {
+    scores();
+    const int lim = p.valid - kt * 128;
+    uint32_t pf[32];   // 8 K steps x 4 registers: fragment of rows (l/4, l/4 + 8) x keys (16 kk + 2(l%4) (+8))
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int col = 8 * i + cq;
+        const float a = (col < lim) ? ex2f((s_acc[4 * i + 2 * hh] - m[hh]) * p.scale_log2e) * inv_l[hh] : 0.f;
+        const float c = (col + 1 < lim) ? ex2f((s_acc[4 * i + 2 * hh + 1] - m[hh]) * p.scale_log2e) * inv_l[hh] : 0.f;
+        // key block i = 2 kk + half: register 4 kk + 2 half + hh
+        pf[4 * (i >> 1) + 2 * (i & 1) + hh] = f32x2_to_f16x2_sat(a, c);
+      }
+    mbar_wait(smem_u32(&v_full), kt & 1u);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      const uint32_t b_lo = wgmma_lo(v_smem + (kk >> 2) * v_blk + (kk & 3) * 32);
+      Wgmma<D>::rs(o_acc, *reinterpret_cast<const uint32_t(*)[4]>(&pf[4 * kk]), wgmma_lohi(b_lo, kHi), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o_acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(smem_u32(&v_empty));
+  }
+  // ---- epilogue: O (fp32 registers) -> fp16 rows of the output
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int qi = q0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * hh;
+    if (qi >= p.nq) continue;
+    __half* orow = p.out + ((size_t)b * p.nq + qi) * p.out_pitch + h * D;
+#pragma unroll
+    for (int i = 0; i < D / 8; ++i)
+      *reinterpret_cast<uint32_t*>(orow + 8 * i + cq) = f32x2_to_f16x2_sat(o_acc[4 * i + 2 * hh], o_acc[4 * i + 2 * hh + 1]);
   }
 }
 
@@ -340,12 +264,23 @@ cudaError_t launch_attn_fused(const __half* q, int q_pitch, const __half* k, int
   const int chunks = (d + 63) / 64;
   const int v_blk = (d * 128 + 1023) & ~1023;
   p.kstages = chunks <= 2 ? 2 : 1;
-  const int smem = (1 + p.kstages) * chunks * kTileBytes + 2 * v_blk + 2 * kTileBytes + 1024;
+  const int smem = (1 + p.kstages) * chunks * kTileBytes + 2 * v_blk + 1024;
   constexpr int kMaxSmem = 200 * 1024;
-  static SmemConfigOnce once;
-  if (cudaError_t e = once.ensure(attn_fused_kernel, kMaxSmem); e != cudaSuccess) return e;
   if (smem > kMaxSmem) return cudaErrorInvalidValue;
-  attn_fused_kernel<<<dim3((nq + 127) / 128, B * H), kAttnThreads, smem, st>>>(p);
+  const dim3 grid((nq + 127) / 128, B * H);
+  switch (d) {
+#define LTB_ATTN_CASE(DD)                                                            \
+  case DD: {                                                                          \
+    static SmemConfigOnce once;                                                       \
+    if (cudaError_t e = once.ensure(attn_fused_kernel<DD>, kMaxSmem); e != cudaSuccess) return e; \
+    attn_fused_kernel<DD><<<grid, kAttnThreads, smem, st>>>(p);                       \
+    break;                                                                            \
+  }
+    LTB_ATTN_CASE(16) LTB_ATTN_CASE(32) LTB_ATTN_CASE(48) LTB_ATTN_CASE(64) LTB_ATTN_CASE(80)
+    LTB_ATTN_CASE(96) LTB_ATTN_CASE(112) LTB_ATTN_CASE(128) LTB_ATTN_CASE(144) LTB_ATTN_CASE(160)
+#undef LTB_ATTN_CASE
+    default: return cudaErrorInvalidValue;
+  }
   return cudaGetLastError();
 }
 

@@ -1,35 +1,35 @@
-// Generic implicit-GEMM convolution on tcgen05 tensor cores (sm_100a).
+// Generic implicit-GEMM convolution on Hopper tensor cores (sm_90a wgmma).
 //
 //   A (im2col rows, 128 output pixels x KB channels of one tap) : gathered with cp.async (zero-fill = padding)
 //                                                                 into the canonical K-major swizzled smem layout
 //   B (weights, BN x KB)                                         : cp.async, same layout
-//   D (128 x BN fp32)                                            : TMEM accumulator, tcgen05.mma kind::f16
-//   epilogue                                                     : tcgen05.ld -> +bias (+residual) -> ReLU -> fp16 NHWC,
-//                                                                  written straight into a channel slice of the
-//                                                                  destination (concat-free U-Net skips)
+//   D (128 x BN fp32)                                            : registers of two warpgroups (64 rows each), wgmma
+//   epilogue                                                     : +bias (+residual) -> ReLU -> fp16 NHWC, written straight
+//                                                                  into a channel slice of the destination (concat-free skips)
 //
 // This kernel handles EVERY conv geometry of the hot path (any stride / padding / kernel size, ConvTranspose
-// sub-pixel phases, channel-sliced inputs/outputs).  conv_tma.cu is the TMA-fed fast path for the FLOP-heavy
+// sub-pixel phases, channel-sliced inputs/outputs).  conv_halo.cu is the TMA-fed fast path for the FLOP-heavy
 // stride-1 layers.  Reference op being replaced: avatars/wav2lip/models/conv.py:5-19,33-44 (cuDNN conv + BN + add + ReLU).
 #include "conv_params.h"
 #include "ltb_internal.h"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace ltb {
 
+constexpr int kGatherThreads = 256;   // two warpgroups: every thread gathers, each warpgroup owns 64 output rows
+
 template <int BN, int KB>
 struct GatherCfg {
-  static constexpr int CH = KB / 8;      // 16-byte chunks per smem row
-  static constexpr int ROWB = KB * 2;    // bytes per smem row (= swizzle span)
-  static constexpr int RSTEP = 128 / CH; // row step between the rows one producer thread fills
+  static constexpr int CH = KB / 8;                 // 16-byte chunks per smem row
+  static constexpr int ROWB = KB * 2;               // bytes per smem row (= swizzle span)
+  static constexpr int RSTEP = kGatherThreads / CH; // row step between the rows one thread fills
+  static constexpr int RPT = 128 / RSTEP;           // rows per thread
   static constexpr int A_BYTES = 128 * ROWB;
   static constexpr int B_BYTES = (BN * ROWB < 1024) ? 1024 : BN * ROWB;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (STAGE_BYTES >= 32768) ? 3 : 4;
-  static constexpr int LAG = STAGES - 1;
-  static constexpr uint32_t LAYOUT = (KB == 64) ? 2u : (KB == 32) ? 4u : 6u;
+  static constexpr uint32_t LAYOUT = (KB == 64) ? 1u : (KB == 32) ? 2u : 3u;
   static constexpr uint32_t SBO = 8 * ROWB;
-  static constexpr int TCOLS = (BN < 32) ? 32 : BN;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;
 };
 
@@ -41,16 +41,11 @@ __device__ __forceinline__ uint32_t swz_chunk(int row, int j) {
 }
 
 template <int BN, int KB>
-__global__ void __launch_bounds__(160) conv_gather_umma_kernel(const __grid_constant__ ConvParams p) {
+__global__ void __launch_bounds__(kGatherThreads) conv_gather_wgmma_kernel(const __grid_constant__ ConvParams p) {
   using C = GatherCfg<BN, KB>;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_full[C::STAGES];
-  __shared__ __align__(8) uint64_t bar_empty[C::STAGES];
-  __shared__ __align__(8) uint64_t bar_accum;
-  __shared__ uint32_t tmem_base_slot;
-
   const int tid = threadIdx.x;
-  const int warp = tid >> 5;
+  const int wg = tid >> 7, wq = (tid >> 5) & 3, lane = tid & 31;
   const uint32_t tiles = (smem_u32(smem_raw) + 1023u) & ~1023u;
 
   const int zphase = (p.ksplit > 1) ? 0 : ((p.zbatch > 1) ? (int)(blockIdx.z % p.nphases) : (int)blockIdx.z);
@@ -74,197 +69,125 @@ __global__ void __launch_bounds__(160) conv_gather_umma_kernel(const __grid_cons
     it_begin = (int)blockIdx.z * per;
     kiters = min(per, kiters - it_begin);
   }
-
-  if (tid == 0) {
-    for (int s = 0; s < C::STAGES; ++s) {
-      mbar_init(smem_u32(&bar_full[s]), 128);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
-    }
-    mbar_init(smem_u32(&bar_accum), 1);
-    mbar_fence_init();
-  }
-  if (warp == 4) {
-    tmem_alloc(smem_u32(&tmem_base_slot), C::TCOLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_base_slot;
-  // PDL: the prologue above overlaps the predecessor's tail; everything below touches activations
+  // PDL: everything below touches activations
   pdl_launch_dependents();
   pdl_wait();
 
-  if (warp < 4) {
-    // ------------------------------------------------------------------ producers
-    const int j = tid % C::CH;
-    const int r0 = tid / C::CH;
-    // per producer row: input coordinates of tap (0,0) and the element offset of that pixel (+ this thread's 16-byte K chunk);
-    // per K iteration only one uniform tap offset is added — the address arithmetic used to be three 64-bit multiplies per
-    // cp.async and made the small-channel layers issue bound (ncu r02f: 60 % issue slots busy at 4.7 % tensor pipe)
-    int riy[C::CH], rix[C::CH];
-    long long rbase[C::CH];
-    const int gsz = p.GH * p.GW;
+  // per gathered row: input coordinates of tap (0,0) and the element offset of that pixel (+ this thread's 16-byte K chunk);
+  // per K iteration only one uniform tap offset is added
+  const int j = tid % C::CH;
+  const int r0 = tid / C::CH;
+  int riy[C::RPT], rix[C::RPT];
+  long long rbase[C::RPT];
+  const int gsz = p.GH * p.GW;
 #pragma unroll
-    for (int i = 0; i < C::CH; ++i) {
-      const int m = m0 + r0 + i * C::RSTEP;
-      if (m < p.M) {
-        const int b = m / gsz;
-        const int rem = m - b * gsz;
-        const int gy = rem / p.GW;
-        const int gx = rem - gy * p.GW;
-        riy[i] = gy * p.sy;
-        rix[i] = gx * p.sx;
-        rbase[i] = ((long long)(b * p.IH + riy[i]) * p.IW + rix[i]) * p.ICtot + p.ic_off + j * 8;
-      } else {
-        riy[i] = -(1 << 20);  // forces the bounds test to fail -> zero rows
-        rix[i] = 0;
-        rbase[i] = 0;
-      }
-    }
-    int tap = it_begin / cpt, cc = it_begin % cpt;
-    for (int it = 0; it < kiters; ++it) {
-      const int stage = it % C::STAGES;
-      mbar_wait(smem_u32(&bar_empty[stage]), (((uint32_t)it / C::STAGES) & 1u) ^ 1u);
-      const uint32_t a_base = tiles + stage * C::STAGE_BYTES;
-      const uint32_t b_base = a_base + C::A_BYTES;
-      const int dy = ph.dy[tap], dx = ph.dx[tap];
-      const long long toff = (long long)(dy * p.IW + dx) * p.ICtot + cc * KB;   // uniform over the CTA
-#pragma unroll
-      for (int i = 0; i < C::CH; ++i) {
-        const int row = r0 + i * C::RSTEP;
-        const int iy = riy[i] + dy, ix = rix[i] + dx;
-        const bool inb = ((unsigned)iy < (unsigned)p.IH) && ((unsigned)ix < (unsigned)p.IW);
-        const __half* src = inb ? (in_base + rbase[i] + toff) : in_base;
-        cp_async16(a_base + row * C::ROWB + swz_chunk<KB>(row, j) * 16, src, inb ? 16u : 0u);
-      }
-      const size_t wk = (size_t)ph.koff + (size_t)tap * p.Cin + cc * KB + j * 8;
-#pragma unroll
-      for (int i = 0; i < C::CH; ++i) {
-        const int n = r0 + i * C::RSTEP;
-        if (n < BN) {
-          cp_async16(b_base + n * C::ROWB + swz_chunk<KB>(n, j) * 16, w_base + (size_t)(n0 + n) * p.Ktot + wk, 16u);
-        }
-      }
-      cp_async_commit();
-      if (it >= C::LAG) {
-        cp_async_wait<C::LAG>();
-        fence_proxy_async_smem();
-        mbar_arrive(smem_u32(&bar_full[(it - C::LAG) % C::STAGES]));
-      }
-      if (++cc == cpt) {
-        cc = 0;
-        ++tap;
-      }
-    }
-    cp_async_wait<0>();
-    fence_proxy_async_smem();
-    for (int it = (kiters > C::LAG ? kiters - C::LAG : 0); it < kiters; ++it) mbar_arrive(smem_u32(&bar_full[it % C::STAGES]));
-
-    // ------------------------------------------------------------------ epilogue (same 4 warps)
-    mbar_wait(smem_u32(&bar_accum), 0);
-    tc_fence_after();
-    const int m = m0 + tid;
-    const bool valid = m < p.M;
-    size_t opix = 0;
-    if (valid) {
+  for (int i = 0; i < C::RPT; ++i) {
+    const int m = m0 + r0 + i * C::RSTEP;
+    if (m < p.M) {
       const int b = m / gsz;
       const int rem = m - b * gsz;
       const int gy = rem / p.GW;
       const int gx = rem - gy * p.GW;
-      opix = (size_t)(b * p.OH + gy * p.osy + ph.ooy) * p.OW + gx * p.osx + ph.oox;
+      riy[i] = gy * p.sy;
+      rix[i] = gx * p.sx;
+      rbase[i] = ((long long)(b * p.IH + riy[i]) * p.IW + rix[i]) * p.ICtot + p.ic_off + j * 8;
+    } else {
+      riy[i] = -(1 << 20);  // forces the bounds test to fail -> zero rows
+      rix[i] = 0;
+      rbase[i] = 0;
     }
+  }
+  auto load = [&](int it) {
+    const int kk = it_begin + it;
+    const int tap = kk / cpt, cc = kk - tap * cpt;
+    const uint32_t a_base = tiles + (it % C::STAGES) * C::STAGE_BYTES;
+    const uint32_t b_base = a_base + C::A_BYTES;
+    const int dy = ph.dy[tap], dx = ph.dx[tap];
+    const long long toff = (long long)(dy * p.IW + dx) * p.ICtot + cc * KB;   // uniform over the CTA
+#pragma unroll
+    for (int i = 0; i < C::RPT; ++i) {
+      const int row = r0 + i * C::RSTEP;
+      const int iy = riy[i] + dy, ix = rix[i] + dx;
+      const bool inb = ((unsigned)iy < (unsigned)p.IH) && ((unsigned)ix < (unsigned)p.IW);
+      const __half* src = inb ? (in_base + rbase[i] + toff) : in_base;
+      cp_async16(a_base + row * C::ROWB + swz_chunk<KB>(row, j) * 16, src, inb ? 16u : 0u);
+    }
+    const size_t wk = (size_t)ph.koff + (size_t)tap * p.Cin + cc * KB + j * 8;
+#pragma unroll
+    for (int i = 0; i < C::RPT; ++i) {
+      const int n = r0 + i * C::RSTEP;
+      if (n < BN) cp_async16(b_base + n * C::ROWB + swz_chunk<KB>(n, j) * 16, w_base + (size_t)(n0 + n) * p.Ktot + wk, 16u);
+    }
+  };
+
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+#pragma unroll
+  for (int s = 0; s < C::STAGES - 1; ++s) {
+    if (s < kiters) load(s);
+    cp_async_commit();
+  }
+  for (int it = 0; it < kiters; ++it) {
+    cp_async_wait<C::STAGES - 2>();
+    fence_proxy_async_smem();   // cp.async (generic proxy) writes -> wgmma operand reads (async proxy)
+    __syncthreads();            // stage it is complete for every thread; every wgmma of iteration it-1 has retired
+    if (it + C::STAGES - 1 < kiters) load(it + C::STAGES - 1);
+    cp_async_commit();
+    const uint32_t a_base = tiles + (it % C::STAGES) * C::STAGE_BYTES;
+    const uint32_t b_base = a_base + C::A_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < KB / 16; ++k) {
+      const uint64_t ad = wgmma_desc(a_base + wg * 64 * C::ROWB + k * 32, 16, C::SBO, C::LAYOUT);
+      const uint64_t bd = wgmma_desc(b_base + k * 32, 16, C::SBO, C::LAYOUT);
+      Wgmma<BN>::ss(acc, ad, bd, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+  }
+  cp_async_wait<0>();
+
+  // ------------------------------------------------------------------ epilogue straight from the accumulator fragments
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int m = m0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * hh;
+    if (m >= p.M) continue;
+    if (p.ksplit > 1) {
+      // split-K: this CTA's fp32 partial goes to its own slice ws[split][m][co] (plain stores, no atomics)
+      float* wrow = p.ws + ((size_t)blockIdx.z * p.M + m) * p.Cout + n0;
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i)
+        *reinterpret_cast<float2*>(wrow + 8 * i + cq) = make_float2(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
+      continue;
+    }
+    const int b = m / gsz;
+    const int rem = m - b * gsz;
+    const int gy = rem / p.GW;
+    const int gx = rem - gy * p.GW;
+    const size_t opix = (size_t)(b * p.OH + gy * p.osy + ph.ooy) * p.OW + gx * p.osx + ph.oox;
     __half* optr = out_base + opix * p.OCtot + p.oc_off + n0;
     const __half* rptr = p.res ? (p.res + opix * p.RCtot + p.rc_off + n0) : nullptr;
-    const uint32_t trow = tmem + ((uint32_t)(warp * 32) << 16);
-    constexpr int CW = (BN >= 32) ? 32 : 16;
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += CW) {
-      uint32_t v[CW];
-      if constexpr (CW == 32) {
-        tmem_ld32(trow + c0, v);
-      } else {
-        tmem_ld16(trow + c0, reinterpret_cast<uint32_t(&)[16]>(v));
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      const int c = 8 * i + cq;
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c));
+      float x = acc[4 * i + 2 * hh] + bb.x, y = acc[4 * i + 2 * hh + 1] + bb.y;
+      if (rptr) {
+        const float2 rf = __half22float2(__ldcg(reinterpret_cast<const __half2*>(rptr + c)));
+        x += rf.x;
+        y += rf.y;
       }
-      tmem_ld_wait();
-      if (valid && p.ksplit > 1) {
-        // split-K: this CTA's fp32 partial goes to its own slice ws[split][m][co] (plain 16-byte stores, no atomics)
-        float4* wrow = reinterpret_cast<float4*>(p.ws + ((size_t)blockIdx.z * p.M + m) * p.Cout + n0 + c0);
-#pragma unroll
-        for (int g = 0; g < CW / 4; ++g)
-          wrow[g] = make_float4(__uint_as_float(v[4 * g]), __uint_as_float(v[4 * g + 1]), __uint_as_float(v[4 * g + 2]),
-                                __uint_as_float(v[4 * g + 3]));
-      } else if (valid) {
-#pragma unroll
-        for (int g = 0; g < CW; g += 8) {
-          float f[8];
-          const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + c0 + g));
-          const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + c0 + g + 4));
-          f[0] = __uint_as_float(v[g + 0]) + b0.x;
-          f[1] = __uint_as_float(v[g + 1]) + b0.y;
-          f[2] = __uint_as_float(v[g + 2]) + b0.z;
-          f[3] = __uint_as_float(v[g + 3]) + b0.w;
-          f[4] = __uint_as_float(v[g + 4]) + b1.x;
-          f[5] = __uint_as_float(v[g + 5]) + b1.y;
-          f[6] = __uint_as_float(v[g + 6]) + b1.z;
-          f[7] = __uint_as_float(v[g + 7]) + b1.w;
-          if (rptr) {
-            const uint4 rv = __ldcg(reinterpret_cast<const uint4*>(rptr + c0 + g));
-            const __half2* rh = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const float2 rf = __half22float2(rh[q]);
-              f[2 * q] += rf.x;
-              f[2 * q + 1] += rf.y;
-            }
-          }
-          uint4 ov;
-          __half2* oh = reinterpret_cast<__half2*>(&ov);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            float x = f[2 * q], y = f[2 * q + 1];
-            if (p.relu) {
-              x = fmaxf(x, 0.f);
-              y = fmaxf(y, 0.f);
-            }
-            x = fminf(fmaxf(x, -65504.f), 65504.f);
-            y = fminf(fmaxf(y, -65504.f), 65504.f);
-            oh[q] = __floats2half2_rn(x, y);
-          }
-          *reinterpret_cast<uint4*>(optr + c0 + g) = ov;
-        }
+      if (p.relu) {
+        x = fmaxf(x, 0.f);
+        y = fmaxf(y, 0.f);
       }
+      x = fminf(fmaxf(x, -65504.f), 65504.f);
+      y = fminf(fmaxf(y, -65504.f), 65504.f);
+      *reinterpret_cast<__half2*>(optr + c) = __floats2half2_rn(x, y);
     }
-  } else {
-    // ------------------------------------------------------------------ MMA issuer (warp 4; warp-uniform control flow,
-    // tcgen05 instructions predicated on the elected lane — see umma_f16_lohi_if)
-    {
-      const uint32_t leader = elect_one() ? 1u : 0u;
-      constexpr uint32_t idesc = umma_idesc_f16(128, BN);
-      for (int it = 0; it < kiters; ++it) {
-        const int stage = it % C::STAGES;
-        mbar_wait(smem_u32(&bar_full[stage]), ((uint32_t)it / C::STAGES) & 1u);
-        tc_fence_after();
-        const uint32_t a_base = tiles + stage * C::STAGE_BYTES;
-        const uint32_t b_base = a_base + C::A_BYTES;
-#pragma unroll
-        for (int k = 0; k < KB / 16; ++k) {
-          const uint64_t ad = umma_smem_desc(a_base + k * 32, C::SBO, C::LAYOUT);
-          const uint64_t bd = umma_smem_desc(b_base + k * 32, C::SBO, C::LAYOUT);
-          umma_f16_if(leader, tmem, ad, bd, idesc, (it | k) != 0 ? 1u : 0u);
-        }
-        umma_commit_if(leader, smem_u32(&bar_empty[stage]));
-      }
-      umma_commit_if(leader, smem_u32(&bar_accum));
-    }
-    __syncwarp();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem, C::TCOLS);
   }
 }
 
@@ -272,9 +195,9 @@ template <int BN, int KB>
 static cudaError_t launch_one(const ConvParams& p, cudaStream_t st) {
   using C = GatherCfg<BN, KB>;
   static SmemConfigOnce once;
-  if (cudaError_t e = once.ensure(conv_gather_umma_kernel<BN, KB>, C::SMEM_BYTES); e != cudaSuccess) return e;
+  if (cudaError_t e = once.ensure(conv_gather_wgmma_kernel<BN, KB>, C::SMEM_BYTES); e != cudaSuccess) return e;
   dim3 grid((p.M + 127) / 128, p.Cout / BN, p.ksplit > 1 ? p.ksplit : p.nphases * (p.zbatch > 1 ? p.zbatch : 1));
-  return launch_kernel_pdl(conv_gather_umma_kernel<BN, KB>, grid, dim3(160), C::SMEM_BYTES, st, p);
+  return launch_kernel_pdl(conv_gather_wgmma_kernel<BN, KB>, grid, dim3(kGatherThreads), C::SMEM_BYTES, st, p);
 }
 
 template <int KB>
@@ -296,10 +219,10 @@ int conv_gather_pick_bn(const ConvParams& p) {
       break;
     }
   if (!bn) return 0;
-  // small-M layers are weight-bandwidth bound: prefer more, narrower CTAs until the grid fills the 148 SMs
+  // small-M layers are weight-bandwidth bound: prefer more, narrower CTAs until the grid fills the SMs
   const long mt = (p.M + 127) / 128;
   const long zb = p.zbatch > 1 ? p.zbatch : 1;
-  while (bn > 32 && mt * (p.Cout / bn) * p.nphases * zb < 148) bn >>= 1;
+  while (bn > 32 && mt * (p.Cout / bn) * p.nphases * zb < 132) bn >>= 1;
   return bn;
 }
 
@@ -365,7 +288,7 @@ cudaError_t launch_conv_gather(const ConvParams& p_in, cudaStream_t st, float* s
       }
     const long tiles = mt * (p.Cout / bn2);
     if (tiles < 64) {
-      int ks = (int)((296 + tiles - 1) / tiles);
+      int ks = (int)((264 + tiles - 1) / tiles);   // two CTAs per SM
       if (ks > kiters / 8) ks = kiters / 8;   // >= 8 K blocks per split
       if (ks > 32) ks = 32;
       while (ks >= 2 && (size_t)ks * p.M * p.Cout > splitk_ws_floats) --ks;

@@ -1,26 +1,28 @@
-// Halo-resident 3x3 convolution / sub-pixel ConvTranspose on tcgen05 (sm_100a) — the fast path for the FLOP-heavy
+// Halo-resident 3x3 convolution / sub-pixel ConvTranspose on Hopper wgmma (sm_90a) — the fast path for the FLOP-heavy
 // stride-1 layers of the U-Net (reference ops: avatars/wav2lip/models/conv.py:5-19 Conv2d+BN+residual+ReLU and
 // :33-44 ConvTranspose2d+BN+ReLU; the same kernel serves the MuseTalk VAE/UNet 3x3 convs).
 //
 // Idea: the nine im2col operands of a 3x3 conv are nine SHIFTED VIEWS of one input halo tile.  A CTA therefore TMA-loads
 // ONE (16*NSUB+2) x 10 pixel x 64 channel halo per K chunk into shared memory (128-byte rows, SWIZZLE_128B) and addresses
-// all nine views purely through the tcgen05 shared-memory descriptor: start address = halo + (dy*10+dx) rows, 8-row
+// all nine views purely through the wgmma shared-memory descriptor: start address = halo + (dy*10+dx) rows, 8-row
 // groups 10 rows (1280 B) apart.  The 128B swizzle is a function of the absolute smem address, so unaligned starts and
-// an SBO that is not a multiple of 1024 B are legal (verified on hardware by umma_probe.cu / tests/probe_umma.py).
-// Compared with one tile load per tap this cuts L2->SM operand traffic for A by 6.4x; weights are streamed 3 taps at a
-// time and amortised over NSUB=2 stacked 128-pixel sub-tiles (M = 256 per CTA).
+// an SBO that is not a multiple of 1024 B read exactly the rows TMA wrote.  Compared with one tile load per tap this cuts
+// L2->SM operand traffic for A by 6.4x; weights are streamed 3 taps at a time and amortised over NSUB stacked 128-pixel
+// sub-tiles (M = 128 * NSUB per CTA).
 //
-// Roles (320 threads): warp 0 = TMA producer, warp 1 = MMA issuer + TMEM owner, warps 2..9 = epilogue
-// (TMEM -> registers -> +bias (+residual) -> ReLU -> fp16 NHWC channel slice).  Persistent CTAs, double-buffered TMEM
-// accumulators: the epilogue of tile i overlaps the MMAs of tile i+1.
+// Roles (288 threads): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer.  Consumer warpgroup g owns pixel rows
+// [8g, 8g+8) of every 16-row sub-tile (64 MMA rows), issues its own wgmma into register accumulators and runs the epilogue
+// (+bias (+residual) -> ReLU -> fp16 NHWC channel slice) straight from the accumulator fragments.  Persistent CTAs: the
+// producer runs ahead across tiles, so the loads of tile i+1 overlap the epilogue of tile i.
 #include <cuda.h>
 
 #include <atomic>
 #include <mutex>
+#include <utility>
 
 #include "conv_halo.h"
 #include "ltb_internal.h"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 #ifdef LTB_HALO_DIAG
 #include <cstdlib>
@@ -32,12 +34,13 @@
 namespace ltb {
 
 constexpr int kHaloP = 10;  // halo row pitch in pixels (8 + 2)
+constexpr int kHaloThreads = 288;
+constexpr int kSms = 132;   // H100 SXM: tile-count heuristics; launches read the device's own SM count
 
 // TAPS = 9: 3x3 conv / sub-pixel ConvT over a (16*NSUB+2) x 10 pixel halo.
 // TAPS = 1: plain GEMM (1x1 conv / nn.Linear): the "halo" is the 128*NSUB-row tile itself (pitch 8 -> SBO 1024 B).
 // RC > 0: "weights resident" variant for layers whose whole tap-major weight set (RC K-chunks x 9 taps x BN rows) fits
-// next to the halo ring — the CTA loads it once instead of once per tile (for the 64-channel 256x256 layers the
-// re-streamed weights were 60 % of all L2->SM traffic).  Requires Cout == BN (every tile uses the same weights).
+// next to the halo ring — the CTA loads it once instead of once per tile.  Requires Cout == BN.
 template <int BN, int NSUB, int NACC, int TAPS, int RC = 0>
 struct HaloCfg {
   static constexpr bool HALO = (TAPS != 1);                                 // 9: 3x3 conv / ConvT, 16: nearest-2x upsample + 3x3 conv
@@ -57,32 +60,67 @@ struct HaloCfg {
   static constexpr int A_STAGES_RES = ((BUDGET - RC * TG * B_BYTES) / A_BYTES) > 4 ? 4 : ((BUDGET - RC * TG * B_BYTES) / A_BYTES);
   static constexpr int A_STAGES = RC ? A_STAGES_RES : A_STAGES_STREAM;
   static constexpr int B_STAGES_MAX = (BUDGET - A_STAGES * A_BYTES) / B_BYTES;
-  static constexpr int B_STAGES = RC ? RC * TG : (B_STAGES_MAX > 6 ? 6 : B_STAGES_MAX);
-  static constexpr int ACC_COLS = NACC * NSUB * BN;                         // fp32 columns per accumulator buffer
-  // accumulator buffers: two (the epilogue of tile i overlaps the MMAs of tile i+1) unless one set already fills the 512
-  // TMEM columns (ConvT with BN = 128: four 128-column phase accumulators)
-  static constexpr int NBUF = (2 * ACC_COLS <= 512) ? 2 : 1;
-  static constexpr int TCOLS = (NBUF * ACC_COLS <= 32) ? 32 : (NBUF * ACC_COLS <= 64) ? 64 : (NBUF * ACC_COLS <= 128) ? 128
-                               : (NBUF * ACC_COLS <= 256) ? 256 : 512;
+  static constexpr int B_STAGES = RC ? RC * TG : (B_STAGES_MAX > 8 ? 8 : B_STAGES_MAX);
+  // release the stages of chunk c only once chunk c+1 is issued (one wgmma group in flight) when the weight ring can hold
+  // two chunks; otherwise each weight stage is waited for and handed back right after its MMAs
+  static constexpr bool LAG = RC || B_STAGES >= 2 * TG;
+  static constexpr int ACOLS = NACC * BN;                                   // accumulator columns per sub-tile
   static constexpr int SMEM_BYTES = A_STAGES * A_BYTES + B_STAGES * B_BYTES + 1024;
-  static_assert(NBUF * ACC_COLS <= 512, "TMEM overflow");
+  static_assert(NSUB * ACOLS <= 256, "register accumulator overflow");
   static_assert(B_STAGES >= 2, "not enough shared memory for the weight ring");
   static_assert(A_STAGES >= 2, "not enough shared memory for the halo ring");
   static_assert(SMEM_BYTES + 3584 <= 227 * 1024, "shared memory overflow (dynamic + static)");
 };
 
+// Sub-pixel layers ("fat-N" issue): the (phase, tap) weight slices are stored view-major so that ONE wgmma per halo view
+// feeds every phase accumulator that reads it.  Accumulator slots are ordered p0, p1, p3, p2 (phase = oy*2 + ox) so that
+// slots sharing a view are adjacent.  {weight stage, halo view (row offset), first slot, first weight slice, slots}
+struct FatMma {
+  int stage, view, slot0, brow, nslots;
+};
+constexpr int fat_view(int vy, int vx) { return (vy + 1) * kHaloP + (vx + 1); }
+template <int TAPS>
+struct FatTable;
+// ConvT(k3, s2): stage 0: v00->p0,p1,p3 | stage 1: v01->p1,p3 ; v11->p3 | stage 2: v00->p2 ; v10->p3,p2  (ConvT halos start at the
+// tile origin: view = dy*10 + dx)
+template <>
+struct FatTable<9> {
+  static constexpr int NG = 5;
+  static constexpr FatMma g[NG] = {{0, 0, 0, 0, 3}, {1, 1, 1, 0, 2}, {1, kHaloP + 1, 2, 2, 1}, {2, 0, 3, 2, 1}, {2, kHaloP, 2, 0, 2}};
+};
+// Upsample(nearest 2x) + conv3x3: output phase (a, b) = 2x2 conv over the low-res halo, 16 (phase, view) slices in 4 stages
+template <>
+struct FatTable<16> {
+  static constexpr int NG = 10;
+  static constexpr FatMma g[NG] = {{0, fat_view(0, 0), 0, 0, 4},
+                                   {1, fat_view(-1, 0), 0, 0, 2},  {1, fat_view(0, 1), 1, 2, 2},
+                                   {2, fat_view(1, 0), 2, 0, 2},   {2, fat_view(0, -1), 0, 2, 1}, {2, fat_view(0, -1), 3, 3, 1},
+                                   {3, fat_view(-1, -1), 0, 0, 1}, {3, fat_view(-1, 1), 1, 1, 1}, {3, fat_view(1, 1), 2, 2, 1},
+                                   {3, fat_view(1, -1), 3, 3, 1}};
+};
+
+template <int BN, int TAPS, int R, size_t... G>
+__device__ __forceinline__ void fat_issue(float (&acc)[R], int j, int k, uint32_t a_lo0, uint32_t b_lo0, uint32_t a_hi, uint32_t b_hi,
+                                          std::index_sequence<G...>) {
+  (
+      [&] {
+        constexpr FatMma g = FatTable<TAPS>::g[G];
+        if (j == g.stage)
+          wgmma_ss_at<g.nslots * BN, g.slot0 * BN>(acc, wgmma_lohi(a_lo0 + g.view * 8u + k * 2u, a_hi),
+                                                   wgmma_lohi(b_lo0 + g.brow * BN * 8u + k * 2u, b_hi), 1u);
+      }(),
+      ...);
+}
+
 template <int BN, int NSUB, int NACC, int TAPS, int RC>
-__global__ void __launch_bounds__(320, 1) conv_halo_umma_kernel(const __grid_constant__ HaloParams p) {
+__global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const __grid_constant__ HaloParams p) {
   using C = HaloCfg<BN, NSUB, NACC, TAPS, RC>;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t a_full[C::A_STAGES], a_empty[C::A_STAGES];
   __shared__ __align__(8) uint64_t b_full[C::B_STAGES], b_empty[C::B_STAGES];
-  __shared__ __align__(8) uint64_t acc_full[2], acc_empty[2];
-  __shared__ uint32_t tmem_slot;
   __shared__ float head_sw[100];   // fused head: 3 x 32 weights + 3 biases
   // fused GroupNorm statistics: (sum, sum of squares) per (image, group) accumulated in SHARED memory across all tiles of this
-  // persistent CTA and flushed with one global atomic per entry at the end.  (Round 1 issued global float atomics from every
-  // epilogue warp and item on the same few addresses and measured slower than a separate statistics pass.)
+  // persistent CTA and flushed with one global atomic per entry at the end
   constexpr int kGnSmem = (NACC == 1) ? 512 : 1;   // 8 images x 32 groups x (sum, sumsq); larger tables fall back to global atomics
   __shared__ float gn_acc[kGnSmem];
 
@@ -90,9 +128,9 @@ __global__ void __launch_bounds__(320, 1) conv_halo_umma_kernel(const __grid_con
   constexpr bool kHeadOk = (BN == 32 && NACC == 1 && TAPS == 9);
   const bool gn_smem = NACC == 1 && p.gn_stats != nullptr && p.gn_images * p.gn_groups * 2 <= kGnSmem;
   if (gn_smem)
-    for (int i = tid; i < p.gn_images * p.gn_groups * 2; i += 320) gn_acc[i] = 0.f;
+    for (int i = tid; i < p.gn_images * p.gn_groups * 2; i += kHaloThreads) gn_acc[i] = 0.f;
   constexpr bool kHaloMode = C::HALO;
-  if (kHeadOk && p.head_out && tid >= 64 && tid < 64 + 99) head_sw[tid - 64] = (tid - 64 < 96) ? p.head_w[tid - 64] : p.head_b[tid - 64 - 96];
+  if (kHeadOk && p.head_out && tid < 99) head_sw[tid] = (tid < 96) ? p.head_w[tid] : p.head_b[tid - 96];
   const uint32_t smem0 = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t a_smem = smem0;
   const uint32_t b_smem = smem0 + C::A_STAGES * C::A_BYTES;
@@ -101,35 +139,24 @@ __global__ void __launch_bounds__(320, 1) conv_halo_umma_kernel(const __grid_con
   if (tid == 0) {
     for (int s = 0; s < C::A_STAGES; ++s) {
       mbar_init(smem_u32(&a_full[s]), 1);
-      mbar_init(smem_u32(&a_empty[s]), 1);
+      mbar_init(smem_u32(&a_empty[s]), 8);   // one arrival per consumer warp
     }
     for (int s = 0; s < C::B_STAGES; ++s) {
       mbar_init(smem_u32(&b_full[s]), 1);
-      mbar_init(smem_u32(&b_empty[s]), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&acc_full[s]), 1);
-      mbar_init(smem_u32(&acc_empty[s]), 8);
+      mbar_init(smem_u32(&b_empty[s]), 8);
     }
     mbar_fence_init();
     tma_prefetch_desc(&p.tm_in);
     tma_prefetch_desc(&p.tm_w);
   }
-  if (warp == 1) {
-    tmem_alloc(smem_u32(&tmem_slot), C::TCOLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
 
   const int tiles_m = kHaloMode ? p.tiles_x * p.tiles_y * p.N : p.tiles_x;
 
   // PDL: the next kernel of the stream may start its own prologue now; resident weights (constants) are fetched before
   // this kernel waits for its predecessor, everything that touches activations comes after pdl_wait()
   pdl_launch_dependents();
-  if (RC && warp == 0 && lane == 0) {
+  if (RC && warp == 8 && lane == 0) {
     // resident weights: every (chunk, tap-group) box once, all on b_full[0]
     mbar_arrive_expect_tx(smem_u32(&b_full[0]), RC * C::TG * C::B_BYTES);
     for (int c = 0; c < RC; ++c)
@@ -138,7 +165,7 @@ __global__ void __launch_bounds__(320, 1) conv_halo_umma_kernel(const __grid_con
   }
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == 8) {
     // =============================================================== TMA producer
     if (lane == 0) {
       uint32_t ai = 0, bi = 0;  // running stage counters
@@ -187,116 +214,101 @@ __global__ void __launch_bounds__(320, 1) conv_halo_umma_kernel(const __grid_con
         }
       }
     }
-  } else if (warp == 1) {
-    // =============================================================== MMA issuer
-    // warp-uniform: all 32 lanes walk the pipeline, the tcgen05 instructions are predicated on the elected lane
-    {
-      const uint32_t leader = elect_one() ? 1u : 0u;
-      constexpr uint32_t idesc = umma_idesc_f16(128, BN);
-      constexpr uint32_t kADescHi = ((C::P * 128) >> 4) | (1u << 14) | (2u << 29);    // SBO = halo pitch (1280 B) / 1024 B in GEMM mode
-      constexpr uint32_t kBDescHi = (1024u >> 4) | (1u << 14) | (2u << 29);            // SBO = 1024 B
-      uint32_t ai = 0, bi = 0, it = 0;
-      // ConvT (NACC == 4): per-stage "fat" MMA list in registers (see HaloParams::fat): one instruction feeds every
-      // sub-pixel accumulator that reads the same halo view, N = 64..256 instead of nine N = BN instructions
-      constexpr int FS = (NACC == 4) ? C::TG : 1, FQ = (NACC == 4) ? (TAPS == 16 ? 4 : 3) : 1;   // stages x instructions per stage
-      uint32_t fat_n[FS], fat_aoff[FS][FQ], fat_doff[FS][FQ], fat_boff[FS][FQ], fat_idesc[FS][FQ], fat_acc0[FS][FQ];
+  } else {
+    // =============================================================== consumers: wgmma + epilogue
+    const int wg = warp >> 2, wq = warp & 3;
+    const int cq = 2 * (lane & 3);
+    constexpr uint32_t kAHi = wgmma_hi_128b(C::P * 128);   // SBO = halo pitch (1280 B) / 1024 B in GEMM mode
+    constexpr uint32_t kBHi = wgmma_hi_128b(1024);
+    // this warpgroup's first MMA row inside a sub-tile / plane: pixel row 8*wg (halo modes), row 64*wg (GEMM mode)
+    constexpr uint32_t kRowsPerSub = C::HALO ? 16u * C::P : 128u;
+    const uint32_t wg_off = (uint32_t)wg * (C::HALO ? 8u * C::P : 64u) * 8u;   // in 16-byte descriptor units
+    if (RC) mbar_wait(smem_u32(&b_full[0]), 0);
+    uint32_t ai = 0, bi = 0;
+    for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+      float acc[NSUB][C::ACOLS / 2];
 #pragma unroll
-      for (int j = 0; j < FS; ++j) {
-        fat_n[j] = (NACC == 4) ? (uint32_t)p.fat_n[j] : 0u;
+      for (int s = 0; s < NSUB; ++s)
 #pragma unroll
-        for (int q = 0; q < FQ; ++q) {
-          fat_aoff[j][q] = (uint32_t)p.fat[j][q].view * 8u;
-          fat_doff[j][q] = (uint32_t)p.fat[j][q].dcol;
-          fat_boff[j][q] = (uint32_t)p.fat[j][q].brow * 8u;
-          fat_idesc[j][q] = umma_idesc_f16(128, 8) + ((uint32_t)(p.fat[j][q].n >> 3) - 1u) * (1u << 17);
-          fat_acc0[j][q] = p.fat[j][q].first ? 0u : 1u;
-        }
-      }
-      if (RC) mbar_wait(smem_u32(&b_full[0]), 0);
-      for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++it) {
-        const uint32_t buf = it % C::NBUF;
-        mbar_wait(smem_u32(&acc_empty[buf]), ((it / C::NBUF) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t dbase = tmem + buf * C::ACC_COLS;
+        for (int i = 0; i < C::ACOLS / 2; ++i) acc[s][i] = 0.f;
+      uint32_t pend_as = 0, pend_bs = 0;   // stages of the previous chunk (LAG mode), released once its wgmma group retired
+      bool pend = false;
 #pragma unroll 1
-        for (int c = 0; c < chunks; ++c) {
-          const uint32_t as = ai % C::A_STAGES;
-          mbar_wait(smem_u32(&a_full[as]), (ai / C::A_STAGES) & 1u);
-          const uint32_t a_lo0 = (((a_smem + as * C::A_BYTES) & 0x3FFFFu) >> 4) | (1u << 16);
-          const int ksteps = (c == chunks - 1) ? p.last_ksteps : 4;   // skip the all-zero K steps of a ragged last chunk
-          const uint32_t later = (c != 0) ? 1u : 0u;
-          // plain convs: tap geometry is arithmetic, the tap-group loop stays rolled (3x less code: the kernel was losing
-          // 18 % of its issue slots to instruction-cache misses); ConvT: per-tap tables in registers, fully unrolled
-#pragma unroll(NACC == 1 ? 1 : C::TG)
-          for (int j = 0; j < C::TG; ++j) {
-            const uint32_t bs = RC ? (uint32_t)(c * C::TG + j) : bi % C::B_STAGES;
-            if (!RC) mbar_wait(smem_u32(&b_full[bs]), (bi / C::B_STAGES) & 1u);
-            tc_fence_after();
-            // descriptor words: hi = {SBO, version 1, SWIZZLE_128B} is loop invariant; lo = (addr >> 4) | LBO(1) << 16
-            const uint32_t b_lo0 = (((b_smem + bs * C::B_BYTES) & 0x3FFFFu) >> 4) | (1u << 16);
+      for (int c = 0; c < chunks; ++c) {
+        const uint32_t as = ai % C::A_STAGES;
+        mbar_wait(smem_u32(&a_full[as]), (ai / C::A_STAGES) & 1u);
+        const uint32_t a_lo0 = wgmma_lo(a_smem + as * C::A_BYTES) + wg_off;
+        const uint32_t bs0 = bi % C::B_STAGES;
+        // 3x3 / GEMM layers: unrolled (a data-dependent branch around wgmma makes ptxas serialise the wgmma pipeline).  Sub-pixel
+        // layers stay rolled: two fat groups of one stage may accumulate into overlapping column ranges of different N, which must
+        // not be in flight together; the runtime stage select makes ptxas wait between them.
+#pragma unroll(NACC == 1 ? C::TG : 1)
+        for (int j = 0; j < C::TG; ++j) {
+          const uint32_t bs = RC ? (uint32_t)(c * C::TG + j) : (bi + j) % C::B_STAGES;
+          if (!RC) mbar_wait(smem_u32(&b_full[bs]), ((bi + j) / C::B_STAGES) & 1u);
+          const uint32_t b_lo0 = wgmma_lo(b_smem + bs * C::B_BYTES);
+          if (!LTB_DIAG(4)) wgmma_fence();
+          // all four K steps, also in a ragged last chunk: TMA zero-fills the channels >= Cin of both operands
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            if (LTB_DIAG(4)) break;
             if constexpr (NACC == 1) {
 #pragma unroll
               for (int tt = 0; tt < C::TG; ++tt) {
                 // stride 2: tap (dy = j, dx = tt) reads plane (dy != 1, dx != 1) at view (dy == 2, dx == 2)
                 const uint32_t aoff = C::S2 ? (uint32_t)(((j != 1) * 2 + (tt != 1)) * (C::PLANE_BYTES / 16) + ((j == 2) * C::P + (tt == 2)) * 8)
                                             : (kHaloMode ? (uint32_t)(j * C::P + tt) * 8u : 0u);
-                const uint32_t acc0 = later | ((j | tt) ? 1u : 0u);
+                const uint64_t bd = wgmma_lohi(b_lo0 + tt * (BN * 8) + k * 2, kBHi);
 #pragma unroll
-                for (int sub = 0; sub < NSUB; ++sub) {
-                  const uint32_t d = dbase + sub * BN;
-                  const uint32_t a_lo = a_lo0 + aoff + sub * (16 * C::P * 8);
-                  const uint32_t b_lo = b_lo0 + tt * (BN * 8);
-                  if (LTB_DIAG(4)) continue;
-                  if (ksteps == 4) {   // warp-uniform; straight-line issue of the four K steps
-                    umma_f16_lohi_x4_if(leader, d, a_lo, kADescHi, b_lo, kBDescHi, idesc, acc0);
-                  } else {             // ragged last chunk: only the K steps that carry channels
-#pragma unroll 1
-                    for (int k = 0; k < ksteps; ++k)
-                      umma_f16_lohi_if(leader, d, a_lo + k * 2, kADescHi, b_lo + k * 2, kBDescHi, idesc, k ? 1u : acc0);
-                  }
-                }
+                for (int sub = 0; sub < NSUB; ++sub)
+                  Wgmma<BN>::ss(acc[sub], wgmma_lohi(a_lo0 + aoff + sub * kRowsPerSub * 8 + k * 2, kAHi), bd, 1u);
               }
             } else {
-#pragma unroll
-              for (int q = 0; q < FQ; ++q) {
-                if (q < (int)fat_n[j]) {   // warp-uniform
-                  const uint32_t d = dbase + fat_doff[j][q];
-                  const uint32_t a_lo = a_lo0 + fat_aoff[j][q];
-                  const uint32_t b_lo = b_lo0 + fat_boff[j][q];
-                  const uint32_t acc0 = later | fat_acc0[j][q];
-                  if (LTB_DIAG(4)) continue;
-                  if (ksteps == 4) {
-                    umma_f16_lohi_x4_if(leader, d, a_lo, kADescHi, b_lo, kBDescHi, fat_idesc[j][q], acc0);
-                  } else {
-#pragma unroll 1
-                    for (int k = 0; k < ksteps; ++k)
-                      umma_f16_lohi_if(leader, d, a_lo + k * 2, kADescHi, b_lo + k * 2, kBDescHi, fat_idesc[j][q], k ? 1u : acc0);
-                  }
-                }
-              }
+              fat_issue<BN, TAPS>(acc[0], j, k, a_lo0, b_lo0, kAHi, kBHi, std::make_index_sequence<FatTable<TAPS>::NG>{});
             }
-            if (!RC) umma_commit_if(leader, smem_u32(&b_empty[bs]));
-            ++bi;
           }
-          umma_commit_if(leader, smem_u32(&a_empty[as]));
-          ++ai;
+          if constexpr (!C::LAG) {   // the weight ring holds less than two chunks: hand each weight stage back as soon as it is read
+            wgmma_commit();
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(smem_u32(&b_empty[bs]));
+          }
         }
-        umma_commit_if(leader, smem_u32(&acc_full[buf]));
+        if (C::LAG) {
+          wgmma_commit();
+          wgmma_wait<1>();   // the group of chunk c-1 has retired: its stages go back to the producer
+          if (pend) {
+            __syncwarp();
+            if (lane == 0) {
+              mbar_arrive(smem_u32(&a_empty[pend_as]));
+              if (!RC)
+                for (int j = 0; j < C::TG; ++j) mbar_arrive(smem_u32(&b_empty[(pend_bs + j) % C::B_STAGES]));
+            }
+          }
+          pend = true;
+          pend_as = as;
+          pend_bs = bs0;
+        } else {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(smem_u32(&a_empty[as]));
+        }
+        ++ai;
+        if (!RC) bi += C::TG;
       }
-    }
-    __syncwarp();
-  } else {
-    // =============================================================== epilogue (warps 2..9 -> TMEM lane quarter warp%4).
-    // Two warps per quarter (one per 32-column chunk parity): with a single warp per scheduler the epilogue was
-    // issue-latency bound on the narrow HBM-bound layers (ncu: 32 % tensor, 22 % DRAM, IPC 0.2 per warp).
-    const int q = warp & 3;
-    const int grp = (warp - 2) >> 2;
-    const int row = q * 32 + lane;       // 0..127 inside a sub-tile
-    const int ry = row >> 3, rx = row & 7;
-    uint32_t it = 0;
-    float4 bb[8];        // bias of channels [bb_col, bb_col + 32)
-    int bb_col = -1;
-    for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x, ++it) {
+      wgmma_wait<0>();
+#pragma unroll
+      for (int s = 0; s < NSUB; ++s) wgmma_fence_regs(acc[s]);
+      if (C::LAG && pend) {
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(smem_u32(&a_empty[pend_as]));
+          if (!RC)
+            for (int j = 0; j < C::TG; ++j) mbar_arrive(smem_u32(&b_empty[(pend_bs + j) % C::B_STAGES]));
+        }
+      }
+      if (LTB_DIAG(2)) continue;
+
+      // ---------------------------------------------------------- epilogue from the accumulator fragments
       const int nt = t / tiles_m;
       int mt = t - nt * tiles_m;
       int img = 0, ty = 0, tx = 0;
@@ -306,219 +318,132 @@ __global__ void __launch_bounds__(320, 1) conv_halo_umma_kernel(const __grid_con
         ty = mt / p.tiles_x;
         tx = mt - ty * p.tiles_x;
       }
-      const uint32_t buf = it % C::NBUF;
       const int n0 = nt * BN;
-      // Work items of this warp: the 32-column accumulator chunks ci = grp, grp+2, ...  (ci -> phase acc, sub-tile sub, column c0)
-      constexpr int NCH = NACC * NSUB * BN / 32;
-      auto item_pix = [&](int ci, int& acc, int& sub, int& c0, size_t& opix, bool& row_ok) {
-        acc = (ci * 32) / (NSUB * BN);
-        sub = ((ci * 32) / BN) % NSUB;
-        c0 = (ci * 32) % BN;
-        row_ok = true;
-        if (kHaloMode) {
-          const int gy = ty * (16 * NSUB) + sub * 16 + ry, gx = tx * 8 + rx;
-          opix = ((size_t)img * p.OH + gy * p.osy + p.acc_oy[acc]) * p.OW + gx * p.osx + p.acc_ox[acc];
-          row_ok = gy < p.GH && gx < p.GW;   // tiles may overhang small / odd-sized maps
-        } else {
-          opix = (size_t)mt * (128 * NSUB) + sub * 128 + row;      // GEMM mode: output row index
-          row_ok = opix < (size_t)p.M;
-        }
-      };
-      // Residual prefetch, one work item ahead: item 0's residual (64 B per thread) is requested BEFORE waiting for the
-      // accumulator and item i+1's while item i is processed, so the DRAM/L2 latency overlaps the MMAs / the previous item
-      // instead of serialising a load->store round trip per item (tools/diag_halo.py).  The item loop stays rolled: the
-      // unrolled variant pushed the kernel past the instruction cache (ncu: 61 % icc hit rate, 18 % no-instruction stalls).
-      uint4 rnext[4];
       const bool has_res = (p.res != nullptr) && !LTB_DIAG(1);
-      auto load_res = [&](int ci) {
-        int acc, sub, c0;
-        size_t opix;
-        bool row_ok;
-        item_pix(ci, acc, sub, c0, opix, row_ok);
-        if (row_ok) {
-          const __half* rptr = p.res + opix * p.RCtot + p.rc_off + n0 + c0;
-          if (p.wide_io) {
-            ldg256(rptr, rnext[0], rnext[1]);
-            ldg256(rptr + 16, rnext[2], rnext[3]);
-          } else {
+      const bool head = kHeadOk && p.head_out != nullptr;
+      float2 bb[BN / 8];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) rnext[u] = __ldcg(reinterpret_cast<const uint4*>(rptr + 8 * u));
-          }
-        } else {
+      for (int i = 0; i < BN / 8; ++i) bb[i] = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * i + cq));
+      const __half2 hmax = __floats2half2_rn(65504.f, 65504.f);
+      const __half2 hlo = p.relu ? __floats2half2_rn(0.f, 0.f) : __floats2half2_rn(-65504.f, -65504.f);
 #pragma unroll
-          for (int u = 0; u < 4; ++u) rnext[u] = make_uint4(0u, 0u, 0u, 0u);
-        }
-      };
-      if (has_res && grp < NCH) load_res(grp);
-      mbar_wait(smem_u32(&acc_full[buf]), (it / C::NBUF) & 1u);
-      tc_fence_after();
-      const uint32_t tbase = tmem + buf * C::ACC_COLS + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-      for (int ci = grp; ci < NCH; ci += 2) {
-        uint4 rcur[4];
+      for (int sub = 0; sub < NSUB; ++sub) {
+        // GroupNorm partial sums of this warp's 16 rows, per 8-column block
+        float gs[BN / 8], gq[BN / 8];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) rcur[u] = rnext[u];
-        if (has_res && ci + 2 < NCH) load_res(ci + 2);
-        {
-          int acc, sub, c0;
-          size_t opix;
-          bool row_ok;
-          item_pix(ci, acc, sub, c0, opix, row_ok);
-          __half* optr = p.out + opix * p.OCtot + p.oc_off + n0;
-          {
-            if (LTB_DIAG(2)) continue;
-            // bias first: its L1 latency overlaps the TMEM read instead of stalling the first add of every group.  The 32
-            // values stay in registers while consecutive items use the same channels (ConvT: the four sub-pixel phases of a
-            // warp share c0, so the bias is loaded once per kernel instead of once per item)
-            if (bb_col != n0 + c0) {
-              bb_col = n0 + c0;
+        for (int i = 0; i < BN / 8; ++i) gs[i] = gq[i] = 0.f;
 #pragma unroll
-              for (int u = 0; u < 8; ++u) bb[u] = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + c0) + u);
+        for (int sl = 0; sl < NACC; ++sl) {
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int r = wq * 16 + (lane >> 2) + 8 * hh;   // MMA row inside this warpgroup's 64
+            size_t opix;
+            bool row_ok;
+            if (kHaloMode) {
+              const int gy = ty * (16 * NSUB) + sub * 16 + wg * 8 + (r >> 3), gx = tx * 8 + (r & 7);
+              opix = ((size_t)img * p.OH + gy * p.osy + p.acc_oy[sl]) * p.OW + gx * p.osx + p.acc_ox[sl];
+              row_ok = gy < p.GH && gx < p.GW;   // tiles may overhang small / odd-sized maps
+            } else {
+              opix = (size_t)mt * (128 * NSUB) + sub * 128 + wg * 64 + r;   // GEMM mode: output row index
+              row_ok = opix < (size_t)p.M;
             }
-            uint32_t v[32];
-            tmem_ld32(tbase + ci * 32, v);
-            tmem_ld_wait();
-            float gs[8], gq[8];
+            __half* optr = p.out + opix * p.OCtot + p.oc_off + n0;
+            const __half* rptr = has_res ? p.res + opix * p.RCtot + p.rc_off + n0 : nullptr;
+            __half2 oh[BN / 8];
 #pragma unroll
-            for (int i = 0; i < 8; ++i) gs[i] = gq[i] = 0.f;
-            const bool head = kHeadOk && p.head_out != nullptr;
-            float ha0 = 0.f, ha1 = 0.f, ha2 = 0.f;
-            if (head) {
-              ha0 = head_sw[96];
-              ha1 = head_sw[97];
-              ha2 = head_sw[98];
+            for (int i = 0; i < BN / 8; ++i) {
+              const float f0 = acc[sub][sl * BN / 2 + 4 * i + 2 * hh] + bb[i].x;
+              const float f1 = acc[sub][sl * BN / 2 + 4 * i + 2 * hh + 1] + bb[i].y;
+              uint32_t w;
+              if (!has_res && p.relu) {
+                w = f32x2_to_f16x2_sat_relu(f0, f1);
+              } else {
+                w = f32x2_to_f16x2_sat(f0, f1);
+                if (has_res && row_ok) {
+                  const __half2 rh = __ldcg(reinterpret_cast<const __half2*>(rptr + 8 * i + cq));
+                  __half2 o = *reinterpret_cast<__half2*>(&w);
+                  o = __hmin2(__hmax2(__hadd2(o, rh), hlo), hmax);
+                  w = *reinterpret_cast<uint32_t*>(&o);
+                }
+              }
+              oh[i] = *reinterpret_cast<__half2*>(&w);
+              if (row_ok && !head && !LTB_DIAG(1)) *reinterpret_cast<__half2*>(optr + 8 * i + cq) = oh[i];
+              if (p.gn_stats && row_ok) {
+                const float2 f = __half22float2(oh[i]);
+                gs[i] += f.x + f.y;
+                gq[i] += f.x * f.x + f.y * f.y;
+              }
             }
+            if constexpr (kHeadOk) {
+              if (head) {
+                // the four lanes of a row hold channels 8i + 2(lane%4) (+1): gather all 32 at the row's first lane and sum them in
+                // channel order (the order of w2l_head_kernel, so the fused head is bit-identical to the separate one)
+                uint32_t hv[4][4];
 #pragma unroll
-            for (int g16 = 0; g16 < 32; g16 += 16) {
-              // packed-half epilogue: fp32 accumulator + fp32 bias -> half2, then residual add / ReLU / saturation as half2 ops.
-              // 16 channels (32 bytes = one full sector) per thread and instruction: 256-bit residual loads and output stores.
-              uint4 ovv[2];
+                for (int src = 0; src < 4; ++src)
 #pragma unroll
-              for (int hh = 0; hh < 2; ++hh) {
-                const int g = g16 + hh * 8;
-                const float4 b0 = bb[g / 4], b1 = bb[g / 4 + 1];
-                __half2* oh = reinterpret_cast<__half2*>(&ovv[hh]);
-                uint32_t* ow = reinterpret_cast<uint32_t*>(&ovv[hh]);
-                const float f0 = __uint_as_float(v[g + 0]) + b0.x, f1 = __uint_as_float(v[g + 1]) + b0.y;
-                const float f2 = __uint_as_float(v[g + 2]) + b0.z, f3 = __uint_as_float(v[g + 3]) + b0.w;
-                const float f4 = __uint_as_float(v[g + 4]) + b1.x, f5 = __uint_as_float(v[g + 5]) + b1.y;
-                const float f6 = __uint_as_float(v[g + 6]) + b1.z, f7 = __uint_as_float(v[g + 7]) + b1.w;
-                if (!has_res && p.relu) {   // warp-uniform: convert + ReLU + saturation in one instruction per channel pair
-                  ow[0] = f32x2_to_f16x2_sat_relu(f0, f1);
-                  ow[1] = f32x2_to_f16x2_sat_relu(f2, f3);
-                  ow[2] = f32x2_to_f16x2_sat_relu(f4, f5);
-                  ow[3] = f32x2_to_f16x2_sat_relu(f6, f7);
-                } else {
-                  ow[0] = f32x2_to_f16x2_sat(f0, f1);
-                  ow[1] = f32x2_to_f16x2_sat(f2, f3);
-                  ow[2] = f32x2_to_f16x2_sat(f4, f5);
-                  ow[3] = f32x2_to_f16x2_sat(f6, f7);
-                  if (has_res) {
-                    const __half2* rh = reinterpret_cast<const __half2*>(&rcur[(g16 >> 3) + hh]);
-                    const __half2 hmax = __floats2half2_rn(65504.f, 65504.f);
-                    const __half2 lo = p.relu ? __floats2half2_rn(0.f, 0.f) : __floats2half2_rn(-65504.f, -65504.f);
+                  for (int i = 0; i < 4; ++i)
+                    hv[src][i] = __shfl_sync(0xffffffffu, *reinterpret_cast<uint32_t*>(&oh[i]), (lane & ~3) + src);
+                if ((lane & 3) == 0 && row_ok) {
+                  float ha0 = head_sw[96], ha1 = head_sw[97], ha2 = head_sw[98];
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) oh[u] = __hmin2(__hmax2(__hadd2(oh[u], rh[u]), lo), hmax);
-                  }
-                }
-                if (kHeadOk && head) {
+                  for (int i = 0; i < 4; ++i)
 #pragma unroll
-                  for (int u = 0; u < 4; ++u) {
-                    const float2 f = __half22float2(oh[u]);
-                    const int c = g + 2 * u;
-                    ha0 = fmaf(f.x, head_sw[c], ha0);
-                    ha0 = fmaf(f.y, head_sw[c + 1], ha0);
-                    ha1 = fmaf(f.x, head_sw[32 + c], ha1);
-                    ha1 = fmaf(f.y, head_sw[32 + c + 1], ha1);
-                    ha2 = fmaf(f.x, head_sw[64 + c], ha2);
-                    ha2 = fmaf(f.y, head_sw[64 + c + 1], ha2);
-                  }
-                }
-                if (p.gn_stats && row_ok) {
-                  float ps[4], pq[4];
-#pragma unroll
-                  for (int u = 0; u < 4; ++u) {
-                    const float2 f2 = __half22float2(oh[u]);
-                    ps[u] = f2.x + f2.y;
-                    pq[u] = f2.x * f2.x + f2.y * f2.y;
-                  }
-                  if (p.gn_cpg == 4) {
-                    gs[g / 4] += ps[0] + ps[1];
-                    gq[g / 4] += pq[0] + pq[1];
-                    gs[g / 4 + 1] += ps[2] + ps[3];
-                    gq[g / 4 + 1] += pq[2] + pq[3];
-                  } else {
-                    const float ts = (ps[0] + ps[1]) + (ps[2] + ps[3]), tq = (pq[0] + pq[1]) + (pq[2] + pq[3]);
-                    if (p.gn_cpg == 8) {
-                      gs[g / 8] += ts;
-                      gq[g / 8] += tq;
-                    } else if (p.gn_cpg == 16) {
-                      gs[g / 16] += ts;
-                      gq[g / 16] += tq;
-                    } else {
-                      gs[0] += ts;
-                      gq[0] += tq;
+                    for (int src = 0; src < 4; ++src) {
+                      const float2 f = __half22float2(*reinterpret_cast<__half2*>(&hv[src][i]));
+                      const int cc = 8 * i + 2 * src;
+                      ha0 = fmaf(f.x, head_sw[cc], ha0);
+                      ha0 = fmaf(f.y, head_sw[cc + 1], ha0);
+                      ha1 = fmaf(f.x, head_sw[32 + cc], ha1);
+                      ha1 = fmaf(f.y, head_sw[32 + cc + 1], ha1);
+                      ha2 = fmaf(f.x, head_sw[64 + cc], ha2);
+                      ha2 = fmaf(f.y, head_sw[64 + cc + 1], ha2);
                     }
-                  }
-                }
-              }
-              if (row_ok && !head && !LTB_DIAG(1)) {
-                if (p.wide_io) {
-                  stg256(optr + c0 + g16, ovv[0], ovv[1]);
-                } else {
-                  *reinterpret_cast<uint4*>(optr + c0 + g16) = ovv[0];
-                  *reinterpret_cast<uint4*>(optr + c0 + g16 + 8) = ovv[1];
+                  float* o = p.head_out + opix * 3;
+                  o[0] = (1.f / (1.f + expf(-ha0))) * 255.f;
+                  o[1] = (1.f / (1.f + expf(-ha1))) * 255.f;
+                  o[2] = (1.f / (1.f + expf(-ha2))) * 255.f;
                 }
               }
             }
-            if (kHeadOk && head && row_ok) {
-              float* o = p.head_out + opix * 3;
-              o[0] = (1.f / (1.f + expf(-ha0))) * 255.f;
-              o[1] = (1.f / (1.f + expf(-ha1))) * 255.f;
-              o[2] = (1.f / (1.f + expf(-ha2))) * 255.f;
+          }
+        }
+        if (p.gn_stats) {
+          int gimg = img;
+          if (!kHaloMode) gimg = (int)(((size_t)mt * (128 * NSUB) + sub * 128 + wg * 64 + wq * 16) / (size_t)p.gn_hw);
+          float* sbase = (gn_smem ? gn_acc : p.gn_stats) + (size_t)gimg * p.gn_groups * 2;
+#pragma unroll
+          for (int i = 0; i < BN / 8; ++i) {
+            float a = gs[i], b = gq[i];
+            // rows (lane / 4) always reduce; the column lanes reduce within a group: 4 channels = lane pairs
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) {
+              a += __shfl_xor_sync(0xffffffffu, a, o);
+              b += __shfl_xor_sync(0xffffffffu, b, o);
             }
-            if (p.gn_stats) {
-              const int ng = p.gn_cpg >= 32 ? 1 : 32 / p.gn_cpg;
-              int gimg = img;
-              if (!kHaloMode) gimg = (int)(((size_t)mt * (128 * NSUB) + sub * 128 + q * 32) / (size_t)p.gn_hw);
-              float* sbase = (gn_smem ? gn_acc : p.gn_stats) + ((size_t)gimg * p.gn_groups + (n0 + c0) / p.gn_cpg) * 2;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                if (i < ng) {
-                  float a = gs[i], b = gq[i];
-#pragma unroll
-                  for (int o = 16; o > 0; o >>= 1) {
-                    a += __shfl_xor_sync(0xffffffffu, a, o);
-                    b += __shfl_xor_sync(0xffffffffu, b, o);
-                  }
-                  if (lane == 0) {
-                    atomicAdd(sbase + 2 * i, a);
-                    atomicAdd(sbase + 2 * i + 1, b);
-                  }
-                }
-              }
+            a += __shfl_xor_sync(0xffffffffu, a, 1);
+            b += __shfl_xor_sync(0xffffffffu, b, 1);
+            if (p.gn_cpg >= 8) {
+              a += __shfl_xor_sync(0xffffffffu, a, 2);
+              b += __shfl_xor_sync(0xffffffffu, b, 2);
+            }
+            if (lane == 0 || (p.gn_cpg == 4 && lane == 2)) {
+              const int g = (n0 + 8 * i + cq) / p.gn_cpg;
+              atomicAdd(sbase + 2 * g, a);
+              atomicAdd(sbase + 2 * g + 1, b);
             }
           }
         }
       }
-      // this accumulator buffer may be overwritten by the MMAs of tile it+2
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&acc_empty[buf]));
     }
   }
 
-  tc_fence_before();
   __syncthreads();
   if (gn_smem) {
-    for (int i = tid; i < p.gn_images * p.gn_groups * 2; i += 320) {
+    for (int i = tid; i < p.gn_images * p.gn_groups * 2; i += kHaloThreads) {
       const float v = gn_acc[i];
       if (v != 0.f) atomicAdd(p.gn_stats + i, v);
     }
-  }
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, C::TCOLS);
   }
 }
 
@@ -615,35 +540,10 @@ bool conv_halo_supported(const ConvParams& p) {
     int BN, NSUB, NACC;
     if (!pick_cfg(p, &BN, &NSUB, &NACC)) return false;
     const long tiles = (long)p.N * ((p.GH + 16 * NSUB - 1) / (16 * NSUB)) * ((p.GW + 7) / 8) * (p.Cout / BN);
-    const long waves = (tiles + 147) / 148, chunks = (p.Cin + 63) / 64;
+    const long waves = (tiles + kSms - 1) / kSms, chunks = (p.Cin + 63) / 64;
     if (waves * chunks > 16) return false;
   }
   return get_encode() != nullptr;
-}
-
-// The 32-channel output conv (80 -> 32 + fused head @256x256) goes to the y-stacked kernel (conv_ystack.cu: N = 3*BN = 96 per
-// instruction instead of nine N = 32 instructions) when the two overlap rows per tile cost at most 35 % extra MMA rows.
-// Measured on B200 (profiles/r02c_per_op.json vs r02a): 108.5 -> 93.7 us for that layer; the same trick LOSES on the 64-channel
-// layers (84 -> 157 us: three accumulators per output triple the TMEM read volume, 1536 cycles per 112-pixel tile against
-// 1116 cycles of MMAs, and the epilogue handles half as many pixels per pass) and on the 32->32 encoder convs (one ragged K
-// chunk: nothing to amortise), so those stay on the halo kernel.  LTB_YSTACK=0 disables it, LTB_YSTACK=all forces every
-// eligible narrow layer (A/B tests, tests/test_gpu_conv.py).
-static bool pick_ystack(const ConvParams& p, int* BN, int* NSUB) {
-  static const int mode = [] {
-    const char* e = std::getenv("LTB_YSTACK");
-    if (!e || !e[0]) return 1;
-    if (e[0] == '0') return 0;
-    return (e[0] == 'a') ? 2 : 1;
-  }();
-  if (mode == 0 || !is_conv3x3(p) || (p.Cout != 32 && p.Cout != 64) || p.zbatch > 1) return false;
-  if (mode == 1 && !(p.Cout == 32 && p.Cin > 64)) return false;
-  const int nsub = p.Cout == 32 ? 2 : 1;
-  const int valid = 16 * nsub - 2;
-  const int tiles_y = (p.GH + valid - 1) / valid;
-  if (tiles_y * 16 * nsub > (p.GH * 135) / 100) return false;
-  *BN = p.Cout;
-  *NSUB = nsub;
-  return true;
 }
 
 // picks (BN, NSUB, NACC) ; returns false if unsupported
@@ -652,8 +552,10 @@ static bool pick_cfg(const ConvParams& p, int* BN, int* NSUB, int* NACC) {
     *NACC = 1;
     *BN = (p.Cout % 128 == 0) ? 128 : (p.Cout % 64 == 0) ? 64 : 32;
     auto tiles = [&](int bn, int nsub) { return (long)((p.M + 128 * nsub - 1) / (128 * nsub)) * (p.Cout / bn); };
-    *NSUB = tiles(*BN, 2) >= 148 ? 2 : 1;
-    while (*BN > 32 && tiles(*BN, *NSUB) < 120) *BN >>= 1;
+    *NSUB = tiles(*BN, 2) >= kSms ? 2 : 1;
+    while (*BN > 32 && tiles(*BN, *NSUB) < kSms - kSms / 8) *BN >>= 1;
+    // 256 x 128 fp32 accumulators spill and unroll past the instruction cache in GEMM mode: 128-wide tiles take one sub-tile
+    if (*BN == 128) *NSUB = 1;
     return true;
   }
   if (is_upconv(p)) {
@@ -672,18 +574,13 @@ static bool pick_cfg(const ConvParams& p, int* BN, int* NSUB, int* NACC) {
   *NACC = tr ? 4 : 1;
   if (tr) {
     *NSUB = 1;
+    // four phase accumulators of BN columns live in the registers of each consumer warpgroup: BN <= 64
     *BN = (p.Cout % 64 == 0) ? 64 : 32;
-    // BN = 128 (single accumulator set, no epilogue overlap) halves the halo re-reads and the MMA count per FLOP: pays off
-    // once BN = 64 would need more than one wave of tiles
-    const long t64 = (long)p.N * ((p.GH + 15) / 16) * ((p.GW + 7) / 8) * (p.Cout / 64);
-    // ... and the K loop is long enough (>= 8 chunks) to amortise the now serialised epilogue (320->128 @64x64 measured slower)
-    if (p.Cout % 128 == 0 && t64 > 148 && p.Cin >= 512) *BN = 128;
     return true;
   }
-  // 3x3 conv: pick the (BN, NSUB) with the lowest modelled MMA time.  One M=128,K=16 tcgen05.mma costs ~55 + 0.2*N cycles
-  // (the 4 KB A fetch dominates at small N), a tile issues ksteps*9*NSUB of them, the persistent grid walks
-  // ceil(tiles/148) waves; ~800 cycles per tile for pipeline fill / accumulator hand-off.  (384 channels @32x32, batch 16:
-  // BN=128,NSUB=2 is 192 tiles = 2 waves of 35k cycles; NSUB=1 is 384 tiles = 3 waves of 17.5k.)
+  // 3x3 conv: pick the (BN, NSUB) with the lowest modelled MMA time.  An M=128,K=16 step costs ~55 + 0.2*N cycles (the A
+  // fetch dominates at small N), a tile issues ksteps*9*NSUB of them, the persistent grid walks ceil(tiles/SMs) waves;
+  // ~800 cycles per tile for pipeline fill and the epilogue.
   const long ksteps = (p.Cin + 15) / 16;
   double best = 1e30;
   for (int bn : {128, 64, 32}) {
@@ -691,9 +588,9 @@ static bool pick_cfg(const ConvParams& p, int* BN, int* NSUB, int* NACC) {
     for (int nsub : {2, 1}) {
       if (nsub == 2 && (p.GH % 32) != 0) continue;
       const long tiles = (long)p.N * ((p.GH + 16 * nsub - 1) / (16 * nsub)) * ((p.GW + 7) / 8) * (p.Cout / bn);
-      const long waves = (tiles + 147) / 148;
+      const long waves = (tiles + kSms - 1) / kSms;
       const double tile = (double)ksteps * 9 * nsub * (55.0 + 0.2 * bn) + 800.0;
-      // single-wave launches cannot overlap their epilogue with the next tile's MMAs
+      // single-wave launches cannot overlap their epilogue with the next tile's loads
       const double epi = (waves == 1) ? 40.0 * nsub * bn : 0.0;
       const double cost = waves * tile + epi;
       if (cost < best * 0.9) {   // prefer the earlier (wider) candidate unless the model predicts a clear (>10 %) win
@@ -712,8 +609,6 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
   std::memset(&h, 0, sizeof(h));
   int BN, NSUB, NACC;
   if (!pick_cfg(p, &BN, &NSUB, &NACC)) return 1;
-  const bool ys = pick_ystack(p, &BN, &NSUB);
-  out->YS = ys ? 1 : 0;
   out->BN = BN;
   out->NSUB = NSUB;
   out->NACC = NACC;
@@ -737,7 +632,7 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
   {
     cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.IW, (cuuint64_t)p.IH, (cuuint64_t)p.N};
     cuuint64_t strides[3] = {(cuuint64_t)p.ICtot * 2, (cuuint64_t)p.IW * p.ICtot * 2, (cuuint64_t)p.IH * p.IW * p.ICtot * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)kHaloP, (cuuint32_t)(ys ? 16 * NSUB : 16 * NSUB + 2), 1};
+    cuuint32_t box[4] = {64, (cuuint32_t)kHaloP, (cuuint32_t)(16 * NSUB + 2), 1};
     if (s2) {   // one parity plane per load: 9 x (16*NSUB + 1) pixels picked with traversal stride 2 (box extent 2n - 1)
       box[1] = 2 * 9 - 1;
       box[2] = 2 * (16 * NSUB + 1) - 1;
@@ -745,13 +640,7 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
     if (!encode(&h.tm_in, 4, p.in + p.ic_off, dims, strides, box, s2 ? 2 : 1)) return 2;
   }
   // weights: 3-D (k = Cin, n = Cout, tap = 9) view of the tap-major copy [9][Cout][Cin]
-  if (ys) {
-    // 4-D (k, n, dx, dy) view of the tap-major copy [dy*3+dx][Cout][Cin]: box (64, BN, 1, 3) = the three taps of one column
-    cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.Cout, 3, 3};
-    cuuint64_t strides[3] = {(cuuint64_t)p.Cin * 2, (cuuint64_t)p.Cout * p.Cin * 2, (cuuint64_t)3 * p.Cout * p.Cin * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)BN, 1, 3};
-    if (!encode(&h.tm_w, 4, w_tap_major, dims, strides, box)) return 2;
-  } else if (up) {
+  if (up) {
     // 16 view-major slices [16][Cout][Cin], four per weight stage
     cuuint64_t dims[3] = {(cuuint64_t)p.Cin, (cuuint64_t)p.Cout, 16};
     cuuint64_t strides[2] = {(cuuint64_t)p.Cin * 2, (cuuint64_t)p.Cout * p.Cin * 2};
@@ -769,7 +658,6 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
   h.N = p.N;
   h.M = p.M;
   h.Cin = p.Cin;
-  h.last_ksteps = ((p.Cin - 1) % 64) / 16 + 1;
   h.gn_stats = nullptr;
   // 256-bit epilogue accesses need 32-byte aligned rows
 #ifdef LTB_HALO_DIAG
@@ -792,56 +680,12 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
   h.relu = p.relu;
   h.halo_y0 = tr ? 0 : -1;
   h.halo_x0 = tr ? 0 : -1;
-  if (up) {
-    // Upsample(nearest 2x) + conv3x3: output phase (a, b) = 2x2 conv over the low-res halo.  Phase a reads halo rows {-1, 0}
-    // (a = 0) or {0, +1} (a = 1); 16 (phase, view) slices, stored view-major so that one instruction per halo view feeds every
-    // phase that reads it (accumulator slots p00, p01, p11, p10 as for ConvT):
-    //   stage 0: view( 0, 0) -> all four slots                                   (N = 4*BN)
-    //   stage 1: view(-1, 0) -> p00,p01 ; view( 0,+1) -> p01,p11                 (N = 2*BN each)
-    //   stage 2: view(+1, 0) -> p11,p10 ; view( 0,-1) -> p00 ; view( 0,-1) -> p10
-    //   stage 3: the four corner views, one slot each
-    // 10 instructions per K step instead of 4 pixels x 9 taps = 36 on the upsampled map (and no upsampled tensor in HBM).
+  if (up || tr) {
+    // accumulator slots p0, p1, p3, p2 (phase index = oy*2 + ox), see FatTable
     const int slot_phase[4] = {0, 1, 3, 2};
     for (int sl = 0; sl < 4; ++sl) {
       h.acc_oy[sl] = p.ph[slot_phase[sl]].ooy;
       h.acc_ox[sl] = p.ph[slot_phase[sl]].oox;
-    }
-    auto view = [](int vy, int vx) { return (vy + 1) * kHaloP + (vx + 1); };
-    struct G { int stage, view, slot0, brow, nslots, first; };
-    const G groups[10] = {{0, view(0, 0), 0, 0, 4, 1},
-                          {1, view(-1, 0), 0, 0, 2, 0}, {1, view(0, 1), 1, 2, 2, 0},
-                          {2, view(1, 0), 2, 0, 2, 0},  {2, view(0, -1), 0, 2, 1, 0}, {2, view(0, -1), 3, 3, 1, 0},
-                          {3, view(-1, -1), 0, 0, 1, 0}, {3, view(-1, 1), 1, 1, 1, 0}, {3, view(1, 1), 2, 2, 1, 0}, {3, view(1, -1), 3, 3, 1, 0}};
-    for (const G& g : groups) {
-      HaloParams::FatMma& f = h.fat[g.stage][h.fat_n[g.stage]++];
-      f.view = g.view;
-      f.dcol = g.slot0 * BN;
-      f.brow = g.brow * BN;
-      f.n = g.nslots * BN;     // BN = 64: at most 256
-      f.first = g.first;
-    }
-  } else if (tr) {
-    // accumulator slots p0, p1, p3, p2 (phase index = oy*2 + ox): slots that share a halo view are adjacent
-    const int slot_phase[4] = {0, 1, 3, 2};
-    for (int sl = 0; sl < 4; ++sl) {
-      h.acc_oy[sl] = p.ph[slot_phase[sl]].ooy;
-      h.acc_ox[sl] = p.ph[slot_phase[sl]].oox;
-    }
-    struct G { int stage, view, slot0, brow, nslots, first; };
-    const G groups[5] = {{0, 0, 0, 0, 3, 1}, {1, 1, 1, 0, 2, 0}, {1, kHaloP + 1, 2, 2, 1, 0}, {2, 0, 3, 2, 1, 1}, {2, kHaloP, 2, 0, 2, 0}};
-    for (const G& g : groups) {
-      int done = 0;
-      while (done < g.nslots) {   // split so that N <= 256
-        int take = g.nslots - done;
-        while (take * BN > 256) --take;
-        HaloParams::FatMma& f = h.fat[g.stage][h.fat_n[g.stage]++];
-        f.view = g.view;
-        f.dcol = (g.slot0 + done) * BN;
-        f.brow = (g.brow + done) * BN;
-        f.n = take * BN;
-        f.first = g.first;
-        done += take;
-      }
     }
   } else {
     h.acc_oy[0] = p.ph[0].ooy;
@@ -856,8 +700,7 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
     return 0;
   }
   h.tiles_x = (p.GW + 7) / 8;
-  h.tile_rows = ys ? 16 * NSUB - 2 : 16 * NSUB;
-  h.tiles_y = (p.GH + h.tile_rows - 1) / h.tile_rows;
+  h.tiles_y = (p.GH + 16 * NSUB - 1) / (16 * NSUB);
   h.total_tiles = h.tiles_x * h.tiles_y * p.N * h.tiles_n;
   return 0;
 }
@@ -866,9 +709,9 @@ template <int BN, int NSUB, int NACC, int TAPS = 9, int RC = 0>
 static cudaError_t launch_cfg(const HaloPlan& pl, int sms, cudaStream_t st) {
   using C = HaloCfg<BN, NSUB, NACC, TAPS, RC>;
   static SmemConfigOnce once;
-  if (cudaError_t e = once.ensure(conv_halo_umma_kernel<BN, NSUB, NACC, TAPS, RC>, C::SMEM_BYTES); e != cudaSuccess) return e;
+  if (cudaError_t e = once.ensure(conv_halo_wgmma_kernel<BN, NSUB, NACC, TAPS, RC>, C::SMEM_BYTES); e != cudaSuccess) return e;
   const int grid = pl.hp.total_tiles < sms ? pl.hp.total_tiles : sms;
-  return launch_kernel_pdl(conv_halo_umma_kernel<BN, NSUB, NACC, TAPS, RC>, dim3(grid), dim3(320), C::SMEM_BYTES, st, pl.hp);
+  return launch_kernel_pdl(conv_halo_wgmma_kernel<BN, NSUB, NACC, TAPS, RC>, dim3(grid), dim3(kHaloThreads), C::SMEM_BYTES, st, pl.hp);
 }
 
 cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
@@ -878,10 +721,9 @@ cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = kSms;
     sms_cached.store(sms);
   }
-  if (pl.YS) return launch_conv_ystack(pl, sms, st);
   if (pl.TAPS == 10) {
     if (pl.NSUB != 1 || pl.NACC != 1) return cudaErrorInvalidValue;
     return pl.BN == 64 ? launch_cfg<64, 1, 1, 10>(pl, sms, st) : (pl.BN == 32 ? launch_cfg<32, 1, 1, 10>(pl, sms, st) : cudaErrorInvalidValue);
@@ -890,7 +732,6 @@ cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
   const int key = pl.BN * 100 + pl.NSUB * 10 + pl.NACC;
   if (pl.TAPS == 1) {
     switch (key) {
-      case 12821: return launch_cfg<128, 2, 1, 1>(pl, sms, st);
       case 12811: return launch_cfg<128, 1, 1, 1>(pl, sms, st);
       case 6421: return launch_cfg<64, 2, 1, 1>(pl, sms, st);
       case 6411: return launch_cfg<64, 1, 1, 1>(pl, sms, st);
@@ -916,7 +757,6 @@ cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
     case 6411: return launch_cfg<64, 1, 1>(pl, sms, st);
     case 3221: return launch_cfg<32, 2, 1>(pl, sms, st);
     case 3211: return launch_cfg<32, 1, 1>(pl, sms, st);
-    case 12814: return launch_cfg<128, 1, 4>(pl, sms, st);
     case 6414: return launch_cfg<64, 1, 4>(pl, sms, st);
     case 3214: return launch_cfg<32, 1, 4>(pl, sms, st);
   }
@@ -924,9 +764,9 @@ cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
 }
 
 // can the epilogue of this plan accumulate GroupNorm statistics of its output?  (power-of-two channels per group >= 4,
-// whole 32-row groups inside one image)
+// whole 16-row groups inside one image)
 bool conv_halo_gn_fusable(const HaloPlan& pl, int cout_total, int groups, int hw) {
-  if (pl.YS || pl.NACC != 1 || groups <= 0 || cout_total % groups) return false;
+  if (pl.NACC != 1 || groups <= 0 || cout_total % groups) return false;
   const int cpg = cout_total / groups;
   if (cpg < 4 || (cpg & (cpg - 1))) return false;
   if (pl.TAPS == 1 && (hw % 128) != 0) return false;

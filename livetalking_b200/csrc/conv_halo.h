@@ -16,29 +16,14 @@ struct alignas(64) HaloParams {
   const __half* res;
   const float* bias;
   int N, M, Cin;  // M: GEMM-mode row count
-  int last_ksteps;  // 16-wide K steps that carry data in the last 64-channel chunk (1..4)
   int OCtot, oc_off, RCtot, rc_off;
   int OH, OW, osy, osx;
   int GH, GW;            // tile-grid extent (= input H, W): tiles may overhang it, rows/columns beyond are masked
   int relu;
   int halo_y0, halo_x0;  // halo origin relative to the tile origin (-1 for pad-1 conv, 0 for ConvT phases)
-  // ConvT only ("fat-N" issue): the nine (sub-pixel phase, tap) weight slices are stored view-major
-  //   stage 0: v00->p0, v00->p1, v00->p3 | stage 1: v01->p1, v01->p3, v11->p3 | stage 2: v10->p3, v10->p2, v00->p2
-  // (vDYDX = halo view, accumulator slots ordered p0,p1,p3,p2), so that ONE tcgen05.mma per halo view feeds every phase that
-  // reads it: N = 3*BN / 2*BN / BN instead of nine N = BN instructions (an M=128 MMA costs ~55 + 0.2*N cycles: the 4 KB A
-  // fetch dominates at small N).  Up to 3 instructions per weight stage (N > 256 is split).
-  struct FatMma {
-    int view;   // halo row offset (dy*10 + dx) of the A view
-    int dcol;   // first accumulator column
-    int brow;   // first weight row inside the stage (rows of 128 B)
-    int n;      // MMA N (multiple of 16, <= 256)
-    int first;  // 1 = overwrite on the first K chunk (first instruction that touches these columns)
-  };
-  int fat_n[4];
-  FatMma fat[4][4];   // ConvT: 3 stages x <= 3; upsample+conv (TAPS = 16): 4 stages x <= 4
+  // output offset of each accumulator slot (sub-pixel phase; slot order p0, p1, p3, p2, see conv_halo.cu FatTable)
   int acc_oy[4], acc_ox[4];
   int tiles_x, tiles_y, tiles_n, total_tiles;
-  int tile_rows;         // output rows per tile: 16*NSUB, or 16*NSUB - 2 for the y-stacked kernel (tiles overlap by two MMA rows)
   // optional fused GroupNorm statistics of the OUTPUT tensor (sum, sum of squares per (image, group)), accumulated by the
   // epilogue from the fp16-rounded values: saves the separate statistics pass of the following GroupNorm
   float* gn_stats;
@@ -59,18 +44,16 @@ struct alignas(64) HaloParams {
 struct HaloPlan {
   HaloParams hp;
   int BN, NSUB, NACC, TAPS;  // TAPS = 9 (3x3 conv / ConvT halo mode) or 1 (TMA GEMM mode: 1x1 conv / linear)
-  int YS;                    // 1: y-stacked narrow-layer kernel (conv_ystack.cu), tm_w is the 4-D (k, n, dx, dy) view
 };
 
 bool conv_halo_supported(const ConvParams& p);
 // w_tap_major: device pointer to the [9][Cout][Cin] copy of the layer's weights (unused in GEMM mode). returns 0 on success.
 int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan* out);
 cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st);
-cudaError_t launch_conv_ystack(const HaloPlan& pl, int sms, cudaStream_t st);   // conv_ystack.cu (called by launch_conv_halo)
 bool conv_halo_gn_fusable(const HaloPlan& pl, int cout_total, int groups, int hw);
 cudaError_t launch_w_tap_major(const __half* w, __half* wt, int cout, int cin, cudaStream_t st, int ntaps = 9);
 // ConvT(k3,s2) weights: phase-major rows [Cout][9][Cin] (pack order of w2l_pack.py / pack_convT_w) -> the view-major slice
-// order the fat-N issue loop expects (see HaloParams::fat)
+// order the fat-N issue loop expects (see conv_halo.cu FatTable)
 cudaError_t launch_w_tap_major_convT(const __half* w, __half* wt, int cout, int cin, cudaStream_t st);
 
 }  // namespace ltb

@@ -1,12 +1,12 @@
 // HuBERT front-end kernels (SURVEY 8 row f4; reference: avatars/ultralight/audio2feature.py:14-56 -> transformers HubertModel,
 // hubert-large-ls960-ft: feat_extract_norm "layer", conv_bias, do_stable_layer_norm).  The transformer layers and conv layers 1-6
-// run on the tcgen05 conv / attention kernels; these are the pieces with no GEMM shape:
+// run on the wgmma conv / attention kernels; these are the pieces with no GEMM shape:
 //   * Wav2Vec2 processor normalisation (zero mean / unit variance over the utterance) fused with conv layer 0 (1 -> 512, k 10, s 5)
 //   * the positional convolution (Conv1d 1024 -> 1024, k 128, pad 64, 16 groups, weight-norm folded) + SamePad trim + GELU + residual
 //   * the window gather of BaseASR._feature2chunks (base_asr.py:91-157) as HubertASR.run_step calls it (hubert.py:42-45)
 #include "ltb_internal.h"
 #include "ops.h"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace ltb {
 

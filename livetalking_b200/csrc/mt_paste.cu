@@ -7,7 +7,7 @@
 // Byte work, bit-exact with OpenCV; one thread per output pixel of the full frame (copy outside the crop box).
 #include "ltb_internal.h"
 #include "ops.h"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace ltb {
 

@@ -7,7 +7,7 @@
 //     (avatars/musetalk/models/unet.py:12-27), VAE post-processing to u8 BGR (avatars/musetalk/models/vae.py:104-107).
 #include "ltb_internal.h"
 #include "ops.h"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace ltb {
 

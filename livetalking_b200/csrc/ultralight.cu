@@ -1,5 +1,5 @@
 // UltraLight path kernels (SURVEY 8 row f4): the pieces of avatars/ultralight/unet.py and avatars/ultralight_avatar.py that are
-// not dense GEMMs.  The pointwise (1x1) and dense 3x3 convolutions of the U-Net run on the tcgen05 conv kernels; here:
+// not dense GEMMs.  The pointwise (1x1) and dense 3x3 convolutions of the U-Net run on the wgmma conv kernels; here:
 //   * depthwise 3x3 + folded BN + ReLU (InvertedResidual's middle conv, unet.py:18-26)            — HBM/L2-bound, fp32 accumulate
 //   * bilinear x2 upsample, align_corners=True (Up.up, unet.py:76) written into a channel slice of the concat buffer
 //   * LightReal.inference_batch's input glue (ultralight_avatar.py:146-160): 168x168 u8 crops -> [B,160,160,16] fp16
@@ -7,7 +7,7 @@
 #include "cv_resize.cuh"
 #include "ltb_internal.h"
 #include "ops.h"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace ltb {
 

@@ -705,7 +705,7 @@ int ltb_set_device(int device) {
   LTB_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   LTB_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return LTB_FAIL(std::string("libltb200 needs an sm_100a GPU (B200); found ") + prop.name);
+  if (prop.major != 9 || prop.minor != 0) return LTB_FAIL(std::string("libltb200 needs an sm_90a GPU (H100); found ") + prop.name);
   return 0;
 }
 

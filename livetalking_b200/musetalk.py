@@ -1,4 +1,4 @@
-"""MuseTalk on the B200 engine: VAE-encode -> audio-conditioned UNet -> VAE-decode -> blend paste-back.
+"""MuseTalk on the H100 engine: VAE-encode -> audio-conditioned UNet -> VAE-decode -> blend paste-back.
 
 The reference only *wraps* these networks (diffusers ``UNet2DConditionModel`` / ``AutoencoderKL``:
 avatars/musetalk/models/unet.py:29-48, vae.py:10-38) and drives them from ``MuseReal.inference_batch``
@@ -129,8 +129,8 @@ class Builder:
 
     GN_GROUPS = 32   # every GroupNorm of the diffusers UNet / VAE uses 32 groups
     # Fusing the GroupNorm statistics into the producing conv's epilogue (ltb_conv_op.gn_stats) is implemented and parity-tested,
-    # but measured SLOWER on B200 (MuseTalk B=8: 15.6 -> 17.6 ms/step): the extra shuffles/atomics make the 0.9 PFLOP/s VAE convs
-    # epilogue-bound, which costs more than the separate statistics pass (1.0 ms) saves.  Off by default.
+    # but off by default: the extra shuffles/atomics load the conv epilogue, and whether that beats the separate statistics pass
+    # has not been measured on H100.
     FUSE_GN_STATS = os.environ.get("LTB_FUSE_GN", "0") == "1"
 
     def __init__(self, ctx: Ctx):
@@ -646,7 +646,7 @@ class MuseTalkBatchSession:
     Whisper features (Bs, 50, 384) or None): group g's latents are gathered from ITS avatar's table (mirror-indexed, outside the
     graph, so any session may occupy any group of any round), its features occupy rows [g*Bs, (g+1)*Bs) of audio_in.
     The reference serves every session with its own B-frame forward (avatars/musetalk_avatar.py:130-152 under app.py:76-100's
-    max_session connections); at batch 8 the UNet is launch-latency bound on a B200 (64 M-tiles per layer), so four sessions per
+    max_session connections); at batch 8 the UNet is launch-latency bound (64 M-tiles per layer), so four sessions per
     launch cost far less than four launches.  `batch` / `infer_slots` make it a mux for plugin.batcher.CrossSessionBatcher."""
 
     def __init__(self, model: MuseTalkModel, lat_hw: int, groups: int, frames_per_session: int, ctx: Optional[Ctx] = None):

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's avatar plugin surface (avatars/base_avatar.py) for the B200 engine.
+"""Host-side mirror of the reference's avatar plugin surface (avatars/base_avatar.py) for the H100 engine.
 
     plugin.base_asr        <-> avatars/audio_features/base_asr.py   (queues, silence synthesis, warm-up)
     plugin.mel_asr         <-> avatars/audio_features/mel.py        (MelASR.run_step, features from the GPU mel kernels)

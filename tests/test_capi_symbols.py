@@ -30,16 +30,16 @@ def test_header_and_binding_agree(built_lib):
         assert hasattr(lib, n), n
 
 
-def test_library_is_sm100a_tensor_core_code(built_lib):
+def test_library_is_sm90a_tensor_core_code(built_lib):
     import shutil
     import subprocess
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", built_lib], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    assert "UTCHMMA" in sass          # tcgen05.mma
-    assert "LDTM" in sass             # tcgen05.ld
+    assert "sm_90a" in sass
+    assert "HGMMA" in sass            # wgmma.mma_async
+    assert "UTMALDG" in sass          # TMA tensor loads
 
 
 def test_version_and_error_string(built_lib):
@@ -65,8 +65,8 @@ def test_header_constants_match_binding():
 
 
 def test_issue_path_has_no_election_loops(built_lib):
-    """Regression guard for the round-1 finding: tcgen05.mma issued from divergent code makes ptxas wrap every UTCHMMA in an
-    ELECT / BRA.U.ANY loop (~100 cycles per MMA).  The halo kernels must contain only the few loops of the TMA producer."""
+    """Regression guard: an MMA issued from divergent code makes ptxas wrap it in an ELECT / BRA.U.ANY loop (~100 cycles per
+    MMA).  The halo kernels must contain only the few loops of the TMA producer."""
     import shutil
     import subprocess
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
@@ -77,10 +77,10 @@ def test_issue_path_has_no_election_loops(built_lib):
         pytest.skip("object file not kept")
     sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True).stdout
     funcs = re.split(r"\n\s*Function : ", sass)[1:]
-    halo = [f for f in funcs if "conv_halo_umma_kernel" in f.split("\n", 1)[0]]
+    halo = [f for f in funcs if "conv_halo_wgmma_kernel" in f.split("\n", 1)[0]]
     assert len(halo) >= 10
     for f in halo:
-        mma = f.count("UTCHMMA")
+        mma = f.count("HGMMA")
         loops = f.count("BRA.U.ANY")
         lines = f.count("\n") // 2
         assert mma >= 4, f.split("\n", 1)[0]

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 implicit-GEMM conv kernel against a plain PyTorch fp32 reference of the same op,
+"""GPU: the wgmma implicit-GEMM conv kernels against a plain PyTorch fp32 reference of the same op,
 called through the C ABI (ltb_conv2d_f16).  Tolerance: fp16 in/out, fp32 accumulate -> |err| <= 2e-2 + 1e-2*|ref|."""
 import numpy as np
 import pytest
@@ -29,21 +29,20 @@ CASES = [
     (8, 8, 8, 512, 512, 3, (1, 1), 1, False, True),      # split-K: M = 512, 72 K blocks, residual through the finalize kernel
     (8, 4, 4, 1280, 640, 3, (1, 1), 1, False, False),    # split-K: M = 128, 180 K blocks
     (2, 8, 8, 256, 512, 3, (2, 2), 1, False, False),     # split-K with stride 2 (M = 32)
-    (16, 16, 16, 768, 384, 3, (2, 2), 1, True, False),   # ConvT with 128-wide N tiles: fat-N issue splits N = 384 into 256 + 128
+    (16, 16, 16, 768, 384, 3, (2, 2), 1, True, False),   # ConvT with 384 outputs: six 64-wide N tiles, fat-N issue up to N = 192
     (16, 32, 32, 384, 384, 3, (1, 1), 1, False, True),   # 384 channels @32x32, batch 16: the cost model picks BN=128, NSUB=1 (3 waves)
     # stride-2 parity-plane TMA path (conv_halo.cu TAPS = 10): four planes loaded with traversal stride 2, nine taps as views
     (2, 64, 64, 80, 32, 3, (2, 2), 1, False, False),     # BN = 32, ragged second K chunk (80 channels)
     (2, 32, 48, 64, 128, 3, (2, 2), 1, False, False),    # 2 N tiles of 64, non-square, output 16 x 24
     (1, 64, 32, 128, 256, 3, (2, 2), 1, False, False),   # 2 K chunks, 4 N tiles
     (3, 40, 36, 64, 64, 3, (2, 2), 1, False, False),     # ragged output 20 x 18: overhanging tile rows / columns
-    # y-stacked narrow-layer kernel (conv_ystack.cu): N = 3*BN per instruction, rows combined in the epilogue.  By default only the
-    # 80->32 geometry takes it (see pick_ystack); test_ystack_all_variants runs every case below with LTB_YSTACK=all in a subprocess
-    (2, 64, 64, 64, 64, 3, (1, 1), 1, False, True),      # BN=64 NSUB=1: 5 overlapping row tiles, residual, streamed weights
-    (5, 256, 64, 64, 64, 3, (1, 1), 1, False, True),     # same, enough tiles for the weights-resident variant (19 x 8 x 5 = 760 tiles)
-    (1, 96, 40, 80, 32, 3, (1, 1), 1, False, False),     # BN=32 NSUB=2: 80 -> 32 (ragged second K chunk), rows cross the sub-tile boundary
-    (3, 128, 128, 32, 32, 3, (1, 1), 1, False, True),    # 32 -> 32 + residual @128: resident weights, 5 row tiles of 30
+    # narrow 3x3 layers on the halo kernel: streamed and resident weights, ragged chunks, overhanging tiles
+    (2, 64, 64, 64, 64, 3, (1, 1), 1, False, True),      # BN=64: residual, streamed weights
+    (5, 256, 64, 64, 64, 3, (1, 1), 1, False, True),     # same, enough tiles for the weights-resident variant
+    (1, 96, 40, 80, 32, 3, (1, 1), 1, False, False),     # BN=32: 80 -> 32 (ragged second K chunk)
+    (3, 128, 128, 32, 32, 3, (1, 1), 1, False, True),    # 32 -> 32 + residual @128: resident weights
     (2, 50, 21, 64, 64, 3, (1, 1), 1, False, False),     # ragged height and width: masked last row tile / column tile
-    (4, 256, 256, 80, 32, 3, (1, 1), 1, False, False),   # the output conv's geometry (2 chunks resident), 9 row tiles
+    (4, 256, 256, 80, 32, 3, (1, 1), 1, False, False),   # the output conv's geometry (2 chunks resident)
 ]
 
 
@@ -118,7 +117,7 @@ HALO_CASES = [
     (2, 27, 16, 64, 64, False, True),       # odd height (audio encoder 27x16)
     (3, 9, 6, 128, 128, False, True),       # odd height and width
     (2, 20, 12, 64, 32, True, False),       # ConvT over an odd-sized map
-    (3, 64, 64, 544, 128, True, False),     # ConvT BN=128: one 512-column accumulator set (single-buffered TMEM), ragged chunk
+    (3, 64, 64, 544, 128, True, False),     # ConvT, 128 outputs in two BN=64 tiles, ragged last K chunk
     (3, 64, 32, 512, 256, True, False),     # ConvT BN=128, two N tiles
 ]
 
@@ -194,15 +193,3 @@ def test_tma_gemm_mode_matches_torch_fp32(case):
     out_g = engine.conv2d_f16(xn, w.numpy(), b.numpy(), relu=False, res=rn, force_path=1).astype(np.float32)
     assert np.abs(out - out_g).max() <= 2e-2
 
-
-def test_ystack_all_variants():
-    """conv_ystack.cu's (64,1) and (32,2) variants incl. resident / streamed weights: the geometry list above, forced with
-    LTB_YSTACK=all (the selector is read once per process, hence the subprocess)."""
-    import os
-    import subprocess
-    import sys
-    env = dict(os.environ, LTB_YSTACK="all")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(root, "tests", "test_gpu_conv.py"), "-q", "-m", "gpu", "-x",
-                        "-k", "matches_torch", "-p", "no:cacheprovider"], env=env, cwd=root, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]

@@ -241,12 +241,12 @@ def test_fused_upsample_conv_matches_interpolate_plus_conv(shape):
     (2, 8, 48, 1024, 1024, 1024, True),     # UNet 32x32 self-attention (d 40 padded to 48): 8 key tiles, 2 passes
     (1, 6, 64, 1500, 1500, 1500, True),     # Whisper-tiny encoder: ragged last query tile and key tile (1500 = 11*128 + 92)
     (3, 8, 80, 256, 64, 50, False),         # UNet cross-attention: 50 valid audio tokens of 64 rows, two K chunks
-    (2, 8, 160, 64, 64, 64, True),          # 8x8 level: three K chunks, single-stage K ring, 512 TMEM columns
+    (2, 8, 160, 64, 64, 64, True),          # 8x8 level: three K chunks, single-stage K ring
     (1, 8, 160, 16, 16, 16, True),          # mid block at 4x4: 16 queries, 16 keys
     (1, 2, 16, 130, 200, 137, False),       # smallest head dim; nothing aligned
 ], ids=["self1024_d48", "whisper1500_d64", "cross50_d80", "self64_d160", "mid16_d160", "ragged_d16"])
 def test_fused_attention_matches_torch(shape):
-    """softmax(scale QK^T)V as ONE tcgen05 kernel (csrc/attn_fused.cu) against plain PyTorch fp32 on the same fp16 inputs.
+    """softmax(scale QK^T)V as ONE wgmma kernel (csrc/attn_fused.cu) against plain PyTorch fp32 on the same fp16 inputs.
     Tolerance: probabilities are rounded to fp16 before the PV product (like the unfused path stored them), fp32 accumulate, fp16 out:
     |err| <= 4e-3 + 1e-2 |ref|."""
     from livetalking_b200 import engine

@@ -44,10 +44,9 @@ def test_mirror_index_and_batch_build():
     assert np.all(b[0, :3, :128] == np.float32(20 / 255.0))
 
 
-def test_musetalk_blend_matches_cv2_and_reference_function():
-    """oracle mt_paste_back vs OpenCV (blendLinear / cvtColor) and, in the build container, vs the reference's own
-    get_image_blending (avatars/musetalk/myutil.py) driven as MuseReal.paste_back_frame does."""
-    cv2 = pytest.importorskip("cv2")
+def blend_case(cv2):
+    """the frame / prediction / boxes / masks of the MuseTalk blend test (also recorded against the reference's own
+    get_image_blending by tests/golden/make_reference_golden.py)"""
     rng = np.random.default_rng(3)
     H, W = 180, 240
     frame = rng.integers(0, 256, (H, W, 3), dtype=np.uint8)
@@ -57,7 +56,18 @@ def test_musetalk_blend_matches_cv2_and_reference_function():
     mh, mw = crop[3] - crop[1], crop[2] - crop[0]
     soft = cv2.GaussianBlur((np.arange(mh)[:, None] > mh // 2).astype(np.float32).repeat(mw, 1) * 255, (0, 0), 7).astype(np.uint8)
     masks = [np.stack([soft] * 3, -1), rng.integers(0, 256, (mh, mw, 3), dtype=np.uint8)]
-    for mask in masks:
+    return frame, pred, bbox, crop, masks
+
+
+def test_musetalk_blend_matches_cv2_and_reference_function(golden_dir):
+    """oracle mt_paste_back vs OpenCV (blendLinear / cvtColor) and vs the output of the reference's own get_image_blending
+    (avatars/musetalk/myutil.py, driven as MuseReal.paste_back_frame does), stored as SHA-256 digests."""
+    import hashlib
+    import json
+    cv2 = pytest.importorskip("cv2")
+    frame, pred, bbox, crop, masks = blend_case(cv2)
+    want_sha = json.load(open(os.path.join(golden_dir, "reference_host_golden.json")))["musetalk_blend_sha256"]
+    for mask, sha in zip(masks, want_sha):
         got = P.mt_paste_back(pred, frame, bbox, mask, crop)
         # direct OpenCV composition
         x1, y1, x2, y2 = bbox
@@ -68,11 +78,4 @@ def test_musetalk_blend_matches_cv2_and_reference_function():
         m = (cv2.cvtColor(mask, cv2.COLOR_BGR2GRAY) / 255).astype(np.float32)
         body[ys:ye, xs:xe] = cv2.blendLinear(large, body[ys:ye, xs:xe], m, 1 - m)
         assert np.array_equal(got, body)
-        ref_path = "/root/reference/avatars/musetalk/myutil.py"
-        if os.path.exists(ref_path):
-            import importlib.util
-            spec = importlib.util.spec_from_file_location("ref_myutil", ref_path)
-            ref = importlib.util.module_from_spec(spec)
-            spec.loader.exec_module(ref)
-            want = ref.get_image_blending(frame.copy(), cv2.resize(pred.astype(np.uint8), (x2 - x1, y2 - y1)), bbox, mask, crop)
-            assert np.array_equal(got, want)
+        assert hashlib.sha256(np.ascontiguousarray(got).tobytes()).hexdigest() == sha

@@ -23,7 +23,7 @@ def test_traffic_from_ncu_reproduces_committed_json(tmp_path):
 
 def test_layer_roofline_table_is_consistent():
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "layer_roofline.py"),
-                        os.path.join(ROOT, "profiles", "r01n_per_op_wav2lip.json"), "1.2876"], capture_output=True, text=True)
+                        os.path.join(ROOT, "profiles", "r01n_per_op_wav2lip.json"), "1.2876", "1404.6", "6541.8"], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
     rows = [l for l in r.stdout.splitlines() if l.startswith("| L")]
     assert len(rows) == 54                                             # 13 audio + 20 face-encoder + 21 decoder conv layers

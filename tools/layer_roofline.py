@@ -1,16 +1,16 @@
 """Per-layer roofline of the wav2lip256 forward (SURVEY.md §8(d): max(flops/peak, bytes/BW) per layer).
 
-    python tools/layer_roofline.py profiles/r01n_per_op_wav2lip.json [forward_ms] > profiles/r01n_layer_roofline.md
+    python tools/layer_roofline.py per_op.json [forward_ms [peak_tflops peak_gbs]] > layer_roofline.md
 
 For every conv op of the B=16 step: algorithmic FLOPs (from the engine's profile pass), algorithmic HBM bytes (fp16 input +
 output (+ residual is the input: counted once) + weights), the time the measured peaks allow
-(1404.6 TFLOP/s, 6541.8 GB/s: MEASURED_PEAKS.json) and the measured eager-event time.  Eager events include a launch gap
+(default: H100 SXM data sheet, 989 TFLOP/s dense fp16 and 3350 GB/s; pass the peaks of the GPU the profile came from) and the measured eager-event time.  Eager events include a launch gap
 per op (their sum is ~25 % above the graph replay), so the last line also gives the whole-forward figure from the live replay.
 """
 import json
 import sys
 
-PEAK_TF, PEAK_GBS = 1404.6, 6541.8
+PEAK_TF, PEAK_GBS = 989.0, 3350.0
 B = 16
 
 
@@ -88,4 +88,6 @@ def main(path, forward_ms=None):
 
 
 if __name__ == "__main__":
+    if len(sys.argv) > 4:
+        PEAK_TF, PEAK_GBS = float(sys.argv[3]), float(sys.argv[4])
     main(sys.argv[1], float(sys.argv[2]) if len(sys.argv) > 2 else None)

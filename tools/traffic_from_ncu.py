@@ -44,7 +44,7 @@ def main(src, dst):
         L = launches[i]
         by = L.get("dram__bytes_read.sum", 0.0) + L.get("dram__bytes_write.sum", 0.0)
         us = L.get("gpu__time_duration.sum", 0.0)
-        is_conv = any(k in L["name"] for k in ("conv_halo_umma", "conv_ystack_umma", "conv_gather_umma", "stem_umma", "splitk_finalize"))
+        is_conv = any(k in L["name"] for k in ("conv_halo_", "conv_ystack_", "conv_gather_", "stem_umma", "splitk_finalize"))
         short = L["name"].split("(")[0].replace("void ", "").replace("ltb::", "")
         pk = per_kernel.setdefault(short, [0, 0.0, 0.0])
         pk[0] += 1
