@@ -408,9 +408,12 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
             }
           }
         }
-        if (p.gn_stats) {
+        // GEMM mode: a warp whose 16 rows all lie at or past M (the second sub-tile of a ragged last tile) has nothing to add, and
+        // its image index would point one table past the end
+        const size_t gn_row0 = (size_t)mt * (128 * NSUB) + sub * 128 + wg * 64 + wq * 16;
+        if (p.gn_stats && (kHaloMode || gn_row0 < (size_t)p.M)) {
           int gimg = img;
-          if (!kHaloMode) gimg = (int)(((size_t)mt * (128 * NSUB) + sub * 128 + wg * 64 + wq * 16) / (size_t)p.gn_hw);
+          if (!kHaloMode) gimg = (int)(gn_row0 / (size_t)p.gn_hw);
           float* sbase = (gn_smem ? gn_acc : p.gn_stats) + (size_t)gimg * p.gn_groups * 2;
 #pragma unroll
           for (int i = 0; i < BN / 8; ++i) {

@@ -35,7 +35,8 @@ __global__ void __launch_bounds__(512) gn_stats_kernel(const __half* __restrict_
   const int n = blockIdx.y;
   const int cpg = C / groups;
   const int vpr = C / 8;
-  if (threadIdx.x < 64) s_sum[threadIdx.x] = s_sq[threadIdx.x] = 0.f;
+  // tiny maps launch a single warp: the table of up to 64 groups is zeroed and flushed in blockDim steps
+  for (int i = threadIdx.x; i < groups; i += blockDim.x) s_sum[i] = s_sq[i] = 0.f;
   __syncthreads();
   const int per = (HW + gridDim.x - 1) / gridDim.x;
   const int p0 = blockIdx.x * per, p1 = min(HW, p0 + per);
@@ -88,9 +89,9 @@ __global__ void __launch_bounds__(512) gn_stats_kernel(const __half* __restrict_
     atomicAdd(&s_sq[g], sb);
   }
   __syncthreads();
-  if (threadIdx.x < groups) {
-    atomicAdd(&stats[((size_t)n * groups + threadIdx.x) * 2 + 0], s_sum[threadIdx.x]);
-    atomicAdd(&stats[((size_t)n * groups + threadIdx.x) * 2 + 1], s_sq[threadIdx.x]);
+  for (int i = threadIdx.x; i < groups; i += blockDim.x) {
+    atomicAdd(&stats[((size_t)n * groups + i) * 2 + 0], s_sum[i]);
+    atomicAdd(&stats[((size_t)n * groups + i) * 2 + 1], s_sq[i]);
   }
 }
 

@@ -128,9 +128,9 @@ class Builder:
     """Emits engine ops for the diffusers building blocks.  Tensors are NHWC fp16 ``DevTensor``s of shape (N,H,W,C)."""
 
     GN_GROUPS = 32   # every GroupNorm of the diffusers UNet / VAE uses 32 groups
-    # Fusing the GroupNorm statistics into the producing conv's epilogue (ltb_conv_op.gn_stats) is implemented and parity-tested,
-    # but off by default: the extra shuffles/atomics load the conv epilogue, and whether that beats the separate statistics pass
-    # has not been measured on H100.
+    # Fusing the GroupNorm statistics into the producing conv's epilogue (ltb_conv_op.gn_stats) is implemented and tested per kernel
+    # path against float64 sums (tests/test_gpu_conv_op.py::test_conv_op_groupnorm_statistics), but off by default: the extra
+    # shuffles/atomics load the conv epilogue, and whether that beats the separate statistics pass has not been measured on H100.
     FUSE_GN_STATS = os.environ.get("LTB_FUSE_GN", "0") == "1"
 
     def __init__(self, ctx: Ctx):
