@@ -211,7 +211,7 @@ static cudaError_t launch_kb(const ConvParams& p, int bn, cudaStream_t st) {
   return cudaErrorInvalidValue;
 }
 
-int conv_gather_pick_bn(const ConvParams& p) {
+static int conv_gather_pick_bn(const ConvParams& p) {
   int bn = 0;
   for (int c : {128, 64, 32, 16})
     if (p.Cout % c == 0) {

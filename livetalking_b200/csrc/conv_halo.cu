@@ -493,7 +493,7 @@ static bool is_convT(const ConvParams& p) {
 }
 
 static bool is_conv3x3_s2(const ConvParams& p) {
-  if (p.nphases != 1 || p.ph[0].ntaps != 9 || p.sy != 2 || p.sx != 2 || p.osy != 1 || p.osx != 1 || p.zbatch > 1) return false;
+  if (p.nphases != 1 || p.ph[0].ntaps != 9 || p.sy != 2 || p.sx != 2 || p.osy != 1 || p.osx != 1) return false;
   for (int t = 0; t < 9; ++t)
     if (p.ph[0].dy[t] != t / 3 - 1 || p.ph[0].dx[t] != t % 3 - 1) return false;
   return p.IH == 2 * p.GH && p.IW == 2 * p.GW && p.OH == p.GH && p.OW == p.GW;
@@ -501,17 +501,18 @@ static bool is_conv3x3_s2(const ConvParams& p) {
 
 static bool is_upconv(const ConvParams& p) {
   return p.upconv == 1 && p.nphases == 4 && p.osy == 2 && p.osx == 2 && p.sy == 1 && p.sx == 1 && p.IH == p.GH && p.IW == p.GW &&
-         p.OH == 2 * p.GH && p.OW == 2 * p.GW && p.zbatch <= 1;
+         p.OH == 2 * p.GH && p.OW == 2 * p.GW;
 }
 
 static bool is_gemm(const ConvParams& p) {
   return p.nphases == 1 && p.ph[0].ntaps == 1 && p.ph[0].dy[0] == 0 && p.ph[0].dx[0] == 0 && p.sy == 1 && p.sx == 1 && p.osy == 1 &&
-         p.osx == 1 && p.IH == p.GH && p.IW == p.GW && p.OH == p.GH && p.OW == p.GW && p.zbatch <= 1;
+         p.osx == 1 && p.IH == p.GH && p.IW == p.GW && p.OH == p.GH && p.OW == p.GW;
 }
 
 static bool pick_cfg(const ConvParams& p, int* BN, int* NSUB, int* NACC);
 
 bool conv_halo_supported(const ConvParams& p) {
+  if (p.zbatch > 1) return false;   // the halo kernel runs one GEMM per launch
   if (is_gemm(p)) {
     // TMA GEMM: K-major rows with 16-byte aligned pitch; worth it from a few M tiles upwards
     return p.Cout % 32 == 0 && p.Cin % 8 == 0 && p.Cin >= 32 && (p.ICtot % 8) == 0 && (p.ic_off % 8) == 0 && (p.Ktot % 8) == 0 &&
@@ -522,11 +523,7 @@ bool conv_halo_supported(const ConvParams& p) {
     // kernel) and a tile carries enough MMAs to hide the four plane loads behind two A stages.  Measured (profiles/r02l_per_op):
     // 64->128 @64->32: 18.5 -> 14.4 us, 128->256 @32->16: 22.5 -> 14.3 us, but 16->32 @256->128: 38.9 -> 64.1 us (nine K=16
     // instructions per 78 KB of zero-padded plane loads: latency bound) -> Cin >= 64 only.
-    static const bool off = [] {
-      const char* e = std::getenv("LTB_NO_S2_TMA");
-      return e && e[0] && e[0] != '0';
-    }();
-    return !off && p.Cout % 32 == 0 && p.Cin >= 64 && (p.ICtot % 8) == 0 && (p.ic_off % 8) == 0 && p.Ktot == 9 * p.Cin && p.GH >= 16 &&
+    return p.Cout % 32 == 0 && p.Cin >= 64 && (p.ICtot % 8) == 0 && (p.ic_off % 8) == 0 && p.Ktot == 9 * p.Cin && p.GH >= 16 &&
            p.GW >= 8 && get_encode() != nullptr;
   }
   if (is_upconv(p))
@@ -662,14 +659,9 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
   h.M = p.M;
   h.Cin = p.Cin;
   h.gn_stats = nullptr;
-  // 256-bit epilogue accesses need 32-byte aligned rows
 #ifdef LTB_HALO_DIAG
   if (const char* e = std::getenv("LTB_HALO_DIAG")) h.dbg = std::atoi(e);
 #endif
-  h.wide_io = ((p.OCtot % 16) == 0 && (p.oc_off % 16) == 0 && (reinterpret_cast<uintptr_t>(p.out) % 32) == 0 &&
-               (!p.res || ((p.RCtot % 16) == 0 && (p.rc_off % 16) == 0 && (reinterpret_cast<uintptr_t>(p.res) % 32) == 0)))
-                  ? 1
-                  : 0;
   h.OCtot = p.OCtot;
   h.oc_off = p.oc_off;
   h.RCtot = p.RCtot;

@@ -28,7 +28,6 @@ struct alignas(64) HaloParams {
   // epilogue from the fp16-rounded values: saves the separate statistics pass of the following GroupNorm
   float* gn_stats;
   int gn_groups, gn_cpg, gn_hw, gn_images;   // gn_images: number of images the statistics table covers (M / gn_hw)
-  int wide_io;  // 1: 32-byte aligned rows -> 256-bit residual loads / output stores
   // optional fused output head (BN == Cout == 32 only): pred[pix][j] = sigmoid(sum_c head_w[j][c] * y[pix][c] + head_b[j]) * 255
   // computed from the fp16-rounded activations in the order of w2l_head_kernel (bit-identical); the activations
   // themselves are then not stored.  wav2lip256 output_block: avatars/wav2lip/models/wav2lip_v2.py:95-97.

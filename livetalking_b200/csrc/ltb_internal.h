@@ -90,7 +90,6 @@ struct SlotDesc {
 // ---- kernel launchers ----
 // splitk_ws: optional zero-initialised fp32 workspace (one per stream) enabling split-K for small-M deep-K layers
 cudaError_t launch_conv_gather(const ConvParams& p, cudaStream_t st, float* splitk_ws = nullptr, size_t splitk_ws_floats = 0);
-int conv_gather_pick_bn(const ConvParams& p);
 
 // wav2lip-specific small kernels (w2l_small.cu)
 // faces u8 [nf,256,256,3] BGR -> padded fp16 [B,262,264,8]: ch0-2 = face/255 with rows >= 128 zeroed, ch3-5 = face/255

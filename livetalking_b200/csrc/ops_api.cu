@@ -9,7 +9,7 @@
 #include <vector>
 
 #include "../../include/ltb200.h"
-#include "conv_halo.h"
+#include "conv_plan.h"
 #include "ltb_internal.h"
 #include "ops.h"
 
@@ -194,68 +194,14 @@ int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d) {
   if (d->KH * d->KW > kMaxTaps) return LTB_FAIL("conv2d: kernel too large");
   pdl_set_enabled(pdl_default());   // the calling thread may have run a w2l profiling pass with PDL off
   if (d->Cout > kZeroBias && !d->bias) return LTB_FAIL("conv2d: Cout too large for the implicit zero bias");
-  ConvParams p;
-  std::memset(&p, 0, sizeof(p));
-  p.in = static_cast<const __half*>(d->in);
-  p.N = d->N;
-  p.IH = d->IH;
-  p.IW = d->IW;
-  p.ICtot = d->ICtot;
-  p.ic_off = d->ic_off;
-  p.Cin = d->Cin;
-  p.sy = d->sy;
-  p.sx = d->sx;
-  p.GH = d->OH;
-  p.GW = d->OW;
-  p.out = static_cast<__half*>(d->out);
-  p.OH = d->OH;
-  p.OW = d->OW;
-  p.OCtot = d->OCtot;
-  p.oc_off = d->oc_off;
-  p.osy = p.osx = 1;
-  p.Cout = d->Cout;
-  p.res = static_cast<const __half*>(d->res);
-  p.RCtot = d->RCtot;
-  p.rc_off = d->rc_off;
-  p.w = static_cast<const __half*>(d->w);
-  p.Ktot = d->Ktot;
-  p.bias = d->bias ? d->bias : c->zero_bias;
-  p.relu = d->relu;
-  p.M = d->N * d->OH * d->OW;
-  p.nphases = 1;
-  p.ph[0].ntaps = d->KH * d->KW;
-  p.ph[0].koff = d->w_koff;
-  for (int kh = 0; kh < d->KH; ++kh)
-    for (int kw = 0; kw < d->KW; ++kw) {
-      p.ph[0].dy[kh * d->KW + kw] = (signed char)(kh - d->pad_t);
-      p.ph[0].dx[kh * d->KW + kw] = (signed char)(kw - d->pad_l);
-    }
-  if (d->upsample2x) {
-    if (d->KH != 3 || d->KW != 3 || d->sy != 1 || d->sx != 1 || d->pad_t != 1 || d->pad_l != 1 || d->OH != 2 * d->IH || d->OW != 2 * d->IW ||
-        d->Ktot != 16 * d->Cin || !d->w_tap || d->zbatch > 1)
-      return LTB_FAIL("conv2d: upsample2x needs a 3x3 s1 p1 conv, OH = 2*IH, OW = 2*IW and the 16-slice weights");
-    // four sub-pixel phases over the low-resolution grid: phase (a, b) reads rows {-1, 0} (a = 0) or {0, +1} (a = 1)
-    p.GH = d->IH;
-    p.GW = d->IW;
-    p.M = d->N * d->IH * d->IW;
-    p.osy = p.osx = 2;
-    p.nphases = 4;
-    p.upconv = 1;
-    for (int a = 0; a < 2; ++a)
-      for (int b = 0; b < 2; ++b) {
-        ConvPhase& ph = p.ph[a * 2 + b];
-        ph.ntaps = 4;
-        ph.koff = (a * 2 + b) * 4 * d->Cin;
-        ph.ooy = a;
-        ph.oox = b;
-        for (int ry = 0; ry < 2; ++ry)
-          for (int rx = 0; rx < 2; ++rx) {
-            ph.dy[ry * 2 + rx] = (signed char)(ry - 1 + a);
-            ph.dx[ry * 2 + rx] = (signed char)(rx - 1 + b);
-          }
-      }
-    if (!conv_halo_supported(p)) return LTB_FAIL("conv2d: upsample2x: geometry not supported by the halo kernel (Cout % 64, Cin % 8)");
-  }
+  if (d->upsample2x && (d->KH != 3 || d->KW != 3 || d->sy != 1 || d->sx != 1 || d->pad_t != 1 || d->pad_l != 1 || d->OH != 2 * d->IH ||
+                        d->OW != 2 * d->IW || d->Ktot != 16 * d->Cin || !d->w_tap || d->zbatch > 1))
+    return LTB_FAIL("conv2d: upsample2x needs a 3x3 s1 p1 conv, OH = 2*IH, OW = 2*IW and the 16-slice weights");
+  ConvParams p = conv_params(d->upsample2x ? ConvMode::Upsample2x : ConvMode::Dense, d->N,
+                             {static_cast<const __half*>(d->in), d->ICtot, d->ic_off}, d->IH, d->IW, d->Cin,
+                             {static_cast<const __half*>(d->out), d->OCtot, d->oc_off}, d->OH, d->OW, d->Cout,
+                             {static_cast<const __half*>(d->res), d->RCtot, d->rc_off}, static_cast<const __half*>(d->w), d->Ktot,
+                             d->w_koff, d->bias ? d->bias : c->zero_bias, d->relu != 0, {d->KH, d->KW, d->sy, d->sx, d->pad_t, d->pad_l});
   p.zbatch = d->zbatch;
   p.zdiv = d->zdiv > 0 ? d->zdiv : 1;
   p.in_zo = d->in_zo;
@@ -264,33 +210,21 @@ int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d) {
   p.w_zi = d->w_zi;
   p.out_zo = d->out_zo;
   p.out_zi = d->out_zi;
-  cudaError_t e;
+  // the fused upsample exists on the halo kernel only
+  const ConvPath path = d->upsample2x ? ConvPath::Halo : d->no_halo ? ConvPath::Gather : ConvPath::Auto;
+  ConvPlan pl;
+  if (conv_plan(p, static_cast<const __half*>(d->w_tap), path, &pl)) return 1;
   const bool want_stats = d->gn_stats != nullptr && d->gn_groups > 0 && d->gn_hw > 0 && (p.M % d->gn_hw) == 0 && d->zbatch <= 1;
-  bool stats_fused = false;
-  const bool one_by_one = (d->KH == 1 && d->KW == 1);
-  if ((d->w_tap || one_by_one) && d->zbatch <= 1 && !d->no_halo && conv_halo_supported(p)) {
-    HaloPlan pl;
-    if (conv_halo_make_plan(p, static_cast<const __half*>(d->w_tap), &pl) != 0) return LTB_FAIL("conv2d: tensor map creation failed");
-    if (want_stats && d->oc_off == 0 && d->OCtot == d->Cout && conv_halo_gn_fusable(pl, d->Cout, d->gn_groups, d->gn_hw)) {
-      // GroupNorm statistics of the output are accumulated by the conv epilogue
-      LTB_CUDA(cudaMemsetAsync(d->gn_stats, 0, (size_t)(p.M / d->gn_hw) * d->gn_groups * 2 * sizeof(float), c->st));
-      pl.hp.gn_stats = static_cast<float*>(d->gn_stats);
-      pl.hp.gn_groups = d->gn_groups;
-      pl.hp.gn_cpg = d->Cout / d->gn_groups;
-      pl.hp.gn_hw = d->gn_hw;
-      pl.hp.gn_images = p.M / d->gn_hw;
-      stats_fused = true;
-    }
-    e = launch_conv_halo(pl, c->st);
-  } else {
-    e = launch_conv_gather(p, c->st, c->splitk_ws, kSplitKWsFloats);
-  }
+  float* stats = static_cast<float*>(d->gn_stats);
+  const bool stats_fused = want_stats && conv_plan_fuse_gn_stats(&pl, stats, d->gn_groups, d->gn_hw);
+  if (stats_fused) LTB_CUDA(cudaMemsetAsync(stats, 0, (size_t)(p.M / d->gn_hw) * d->gn_groups * 2 * sizeof(float), c->st));
+  cudaError_t e = conv_launch(pl, c->st, c->splitk_ws, kSplitKWsFloats);
   if (e != cudaSuccess) return LTB_FAIL(std::string("conv2d launch: ") + cudaGetErrorString(e));
   c->launches += 1;
   if (want_stats && !stats_fused) {
     // fallback: separate statistics pass over the freshly written output
-    e = launch_gn_stats(static_cast<const __half*>(d->out), p.M / d->gn_hw, d->gn_hw, d->Cout, d->OCtot, d->oc_off, d->gn_groups,
-                        static_cast<float*>(d->gn_stats), c->st);
+    e = launch_gn_stats(static_cast<const __half*>(d->out), p.M / d->gn_hw, d->gn_hw, d->Cout, d->OCtot, d->oc_off, d->gn_groups, stats,
+                        c->st);
     if (e != cudaSuccess) return LTB_FAIL(std::string("conv2d gn_stats: ") + cudaGetErrorString(e));
     c->launches += 1;
   }

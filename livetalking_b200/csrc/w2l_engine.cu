@@ -16,7 +16,7 @@
 #include <vector>
 
 #include "../../include/ltb200.h"
-#include "conv_halo.h"
+#include "conv_plan.h"
 #include "ltb_internal.h"
 #include "stem_umma.h"
 
@@ -100,70 +100,6 @@ static void packed_dims(int i, int* rows, int* K) {
   }
 }
 
-// ------------------------------------------------------------------------------------------------ geometry helpers
-static void phases_conv(ConvParams& p, int KH, int KW, int pad, int cin) {
-  p.nphases = 1;
-  ConvPhase& ph = p.ph[0];
-  ph.ntaps = KH * KW;
-  ph.koff = 0;
-  ph.ooy = ph.oox = 0;
-  for (int kh = 0; kh < KH; ++kh)
-    for (int kw = 0; kw < KW; ++kw) {
-      ph.dy[kh * KW + kw] = (signed char)(kh - pad);
-      ph.dx[kh * KW + kw] = (signed char)(kw - pad);
-    }
-  (void)cin;
-}
-
-// ConvTranspose2d(k=3, s=2, p=1, op=1): out[2g+a] gathers (d=0,k=1) for a=0 and (d=0,k=2),(d=+1,k=0) for a=1.
-static const int kTd[2][2] = {{0, 0}, {0, 1}};
-static const int kTk[2][2] = {{1, 0}, {2, 0}};
-static const int kTn[2] = {1, 2};
-static void phases_convT(ConvParams& p, int cin) {
-  p.nphases = 4;
-  int koff = 0;
-  for (int a = 0; a < 2; ++a)
-    for (int b = 0; b < 2; ++b) {
-      ConvPhase& ph = p.ph[a * 2 + b];
-      ph.ntaps = kTn[a] * kTn[b];
-      ph.koff = koff;
-      ph.ooy = a;
-      ph.oox = b;
-      int t = 0;
-      for (int i = 0; i < kTn[a]; ++i)
-        for (int j = 0; j < kTn[b]; ++j, ++t) {
-          ph.dy[t] = (signed char)kTd[a][i];
-          ph.dx[t] = (signed char)kTd[b][j];
-        }
-      koff += ph.ntaps * cin;
-    }
-}
-
-// host-side packing of PyTorch-layout float weights into the kernels' K-major fp16 rows (used by ltb_conv2d_f16;
-// the model path receives rows already packed by livetalking_b200/w2l_pack.py, which follows the same order)
-static void pack_conv_w(const float* w, int cout, int cin, int KH, int KW, std::vector<__half>& out) {
-  out.resize((size_t)cout * KH * KW * cin);
-  for (int co = 0; co < cout; ++co)
-    for (int kh = 0; kh < KH; ++kh)
-      for (int kw = 0; kw < KW; ++kw)
-        for (int ci = 0; ci < cin; ++ci)
-          out[((size_t)co * KH * KW + kh * KW + kw) * cin + ci] = __float2half(w[(((size_t)co * cin + ci) * KH + kh) * KW + kw]);
-}
-static void pack_convT_w(const float* w, int cin, int cout, std::vector<__half>& out) {
-  out.resize((size_t)cout * 9 * cin);
-  for (int co = 0; co < cout; ++co) {
-    size_t k = 0;
-    for (int a = 0; a < 2; ++a)
-      for (int b = 0; b < 2; ++b)
-        for (int i = 0; i < kTn[a]; ++i)
-          for (int j = 0; j < kTn[b]; ++j) {
-            const int kh = kTk[a][i], kw = kTk[b][j];
-            for (int ci = 0; ci < cin; ++ci, ++k)
-              out[(size_t)co * 9 * cin + k] = __float2half(w[(((size_t)ci * cout + co) * 3 + kh) * 3 + kw]);
-          }
-  }
-}
-
 // ------------------------------------------------------------------------------------------------ objects
 struct BlobEntry {
   char name[40];
@@ -212,8 +148,9 @@ struct Tensor {
 struct Op {
   int type;  // 0 = conv (gather kernel), 1 = prep, 2 = audio conv0, 3 = head, 4 = conv (halo kernel), 5 = stem (tensor-core),
              // 6 = mel of the resident PCM chunk (skipped when the host supplies mel windows)
-  ConvParams cp;
-  int halo = -1;    // index into the session's halo plans (type 4)
+  ConvPlan conv;    // types 0 and 4; type 5 keeps only its ConvParams, for the FLOP count
+  __half* audio_out = nullptr;     // type 2
+  const __half* head_in = nullptr;  // type 3
   int branch = 0;   // 1 = audio-encoder branch: runs on the side stream, concurrently with the face encoder
   bool join = false;  // first op that consumes the audio branch's result
 };
@@ -264,7 +201,6 @@ struct ltb_w2l_session {
   SlotDesc* h_slots = nullptr;      // pinned staging for the descriptors
   float* splitk_ws[2] = {nullptr, nullptr};  // one fp32 split-K workspace per stream (main, audio branch)
   std::vector<Op> ops;
-  std::vector<HaloPlan> halo_plans;
   StemParams stem;
   LayerOut louts[kNumLayers];
   cudaGraph_t graph = nullptr;
@@ -343,42 +279,10 @@ static int parse_blob(ltb_w2l_model* m, const uint8_t* host_header, size_t nbyte
   return 0;
 }
 
-// fill the generic part of a ConvParams
-static ConvParams conv_base(const __half* in, int N, int IH, int IW, int ICtot, int ic_off, int Cin, __half* out, int OH,
-                            int OW, int OCtot, int oc_off, int Cout, const __half* w, int Ktot, const float* bias, bool relu) {
-  ConvParams p;
-  std::memset(&p, 0, sizeof(p));
-  p.in = in;
-  p.N = N;
-  p.IH = IH;
-  p.IW = IW;
-  p.ICtot = ICtot;
-  p.ic_off = ic_off;
-  p.Cin = Cin;
-  p.sy = p.sx = 1;
-  p.GH = OH;
-  p.GW = OW;
-  p.out = out;
-  p.OH = OH;
-  p.OW = OW;
-  p.OCtot = OCtot;
-  p.oc_off = oc_off;
-  p.osy = p.osx = 1;
-  p.Cout = Cout;
-  p.w = w;
-  p.Ktot = Ktot;
-  p.bias = bias;
-  p.relu = relu ? 1 : 0;
-  p.M = N * OH * OW;
-  p.nphases = 1;
-  return p;
-}
-
-static int out_dim(int in, int k, int s, int pad) { return (in + 2 * pad - k) / s + 1; }
-
 struct View {
   __half* p;
   int H, W, Ctot, c_off, C;
+  ConvSlice slice() const { return {p, Ctot, c_off}; }
 };
 
 static int build_plan(ltb_w2l_session* s) {
@@ -440,53 +344,33 @@ static int build_plan(ltb_w2l_session* s) {
   auto record = [&](int li, const View& v) {
     s->louts[li] = LayerOut{v.p, v.H, v.W, v.C, v.Ctot, v.c_off};
   };
-  // route a conv to the halo-resident TMA kernel when its geometry allows, else to the generic gather kernel
-  auto push_conv = [&](int li, const ConvParams& p) {
+  const ConvPath path = (s->flags & LTB_SESSION_NO_HALO) ? ConvPath::Gather : ConvPath::Auto;
+  auto push_conv = [&](int li, const ConvParams& p) -> int {
     Op o;
-    o.type = 0;
-    o.cp = p;
-    const bool gemm1x1 = (p.nphases == 1 && p.ph[0].ntaps == 1);
-    if (!(s->flags & LTB_SESSION_NO_HALO) && (m->wt[li] || gemm1x1) && conv_halo_supported(p)) {
-      HaloPlan pl;
-      if (conv_halo_make_plan(p, m->wt[li], &pl) == 0) {
-        o.type = 4;
-        o.halo = (int)s->halo_plans.size();
-        s->halo_plans.push_back(pl);
-      }
-    }
+    if (conv_plan(p, m->wt[li], path, &o.conv)) return LTB_FAIL("plan: layer " + std::to_string(li) + ": " + g_last_error);
+    o.type = o.conv.halo ? 4 : 0;
     s->ops.push_back(o);
+    return 0;
   };
   // regular conv block li: in -> out (+res)
   auto add_conv = [&](int li, const View& in, const View& out, const View* res) -> int {
     const LDef& L = kLayers[li];
     if (in.C != L.cin || out.C != L.cout) return LTB_FAIL("plan: channel mismatch at layer " + std::to_string(li));
-    const int OH = out_dim(in.H, L.k, L.sy, L.pad), OW = out_dim(in.W, L.k, L.sx, L.pad);
+    const int OH = conv_out_dim(in.H, L.k, L.sy, L.pad), OW = conv_out_dim(in.W, L.k, L.sx, L.pad);
     if (OH != out.H || OW != out.W) return LTB_FAIL("plan: spatial mismatch at layer " + std::to_string(li));
-    ConvParams p = conv_base(in.p, B, in.H, in.W, in.Ctot, in.c_off, L.cin, out.p, OH, OW, out.Ctot, out.c_off, L.cout,
-                             m->w[li], L.k * L.k * L.cin, m->bias[li], true);
-    p.sy = L.sy;
-    p.sx = L.sx;
-    phases_conv(p, L.k, L.k, L.pad, L.cin);
-    if (res) {
-      p.res = res->p;
-      p.RCtot = res->Ctot;
-      p.rc_off = res->c_off;
-    }
-    push_conv(li, p);
+    const ConvParams p = conv_params(ConvMode::Dense, B, in.slice(), in.H, in.W, L.cin, out.slice(), OH, OW, L.cout,
+                                     res ? res->slice() : ConvSlice{}, m->w[li], L.k * L.k * L.cin, 0, m->bias[li], true,
+                                     {L.k, L.k, L.sy, L.sx, L.pad, L.pad});
+    if (push_conv(li, p)) return 1;
     record(li, out);
     return 0;
   };
   auto add_convT = [&](int li, const View& in, const View& out) -> int {
     const LDef& L = kLayers[li];
     if (in.C != L.cin || out.C != L.cout || out.H != 2 * in.H) return LTB_FAIL("plan: convT mismatch at layer " + std::to_string(li));
-    ConvParams p = conv_base(in.p, B, in.H, in.W, in.Ctot, in.c_off, L.cin, out.p, out.H, out.W, out.Ctot, out.c_off, L.cout,
-                             m->w[li], 9 * L.cin, m->bias[li], true);
-    p.GH = in.H;
-    p.GW = in.W;
-    p.M = B * in.H * in.W;
-    p.osy = p.osx = 2;
-    phases_convT(p, L.cin);
-    push_conv(li, p);
+    const ConvParams p = conv_params(ConvMode::Transposed, B, in.slice(), in.H, in.W, L.cin, out.slice(), out.H, out.W, L.cout,
+                                     ConvSlice{}, m->w[li], 9 * L.cin, 0, m->bias[li], true);
+    if (push_conv(li, p)) return 1;
     record(li, out);
     return 0;
   };
@@ -494,7 +378,6 @@ static int build_plan(ltb_w2l_session* s) {
   // ---- audio branch first (so the fork precedes the face path): mel of the resident PCM chunk, then audio conv0
   {
     Op o;
-    std::memset(&o.cp, 0, sizeof(o.cp));
     o.type = 6;
     o.branch = 1;
     s->ops.push_back(o);
@@ -503,9 +386,8 @@ static int build_plan(ltb_w2l_session* s) {
   if (new_atmp(80, 16, 32, &a_prev)) return 1;
   {
     Op o;
-    std::memset(&o.cp, 0, sizeof(o.cp));
     o.type = 2;
-    o.cp.out = a_prev.p;
+    o.audio_out = a_prev.p;
     o.branch = 1;
     s->ops.push_back(o);
     record(0, a_prev);
@@ -515,7 +397,7 @@ static int build_plan(ltb_w2l_session* s) {
     int H = 80, W = 16;
     for (int li = 1; li <= 12; ++li) {
       const LDef& L = kLayers[li];
-      const int OH = out_dim(H, L.k, L.sy, L.pad), OW = out_dim(W, L.k, L.sx, L.pad);
+      const int OH = conv_out_dim(H, L.k, L.sy, L.pad), OW = conv_out_dim(W, L.k, L.sx, L.pad);
       View o;
       if (new_atmp(OH, OW, L.cout, &o)) return 1;
       if (add_conv(li, a_prev, o, L.res ? &a_prev : nullptr)) return 1;
@@ -529,7 +411,6 @@ static int build_plan(ltb_w2l_session* s) {
   // ---- prep (faces -> padded 8-channel fp16 image)
   {
     Op o;
-    std::memset(&o.cp, 0, sizeof(o.cp));
     o.type = 1;
     s->ops.push_back(o);
   }
@@ -538,21 +419,17 @@ static int build_plan(ltb_w2l_session* s) {
   // stem (layer 13): 7 row-taps, each K block = 8 consecutive pixels x 8 channels of the padded image
   {
     const View out = cat_skip(7);
-    ConvParams p = conv_base(s->img_pad, B, 262, 264, 8, 0, 64, out.p, 256, 256, out.Ctot, out.c_off, 16, m->w[kStem], 7 * 64,
-                             m->bias[kStem], true);
-    p.nphases = 1;
-    p.ph[0].ntaps = 7;
-    for (int t = 0; t < 7; ++t) {
-      p.ph[0].dy[t] = (signed char)t;
-      p.ph[0].dx[t] = 0;
-    }
-    Op so;
-    so.type = 0;
-    so.cp = p;
+    const ConvParams p = conv_params(ConvMode::Dense, B, {s->img_pad, 8, 0}, 262, 264, 64, out.slice(), 256, 256, 16, ConvSlice{},
+                                     m->w[kStem], 7 * 64, 0, m->bias[kStem], true, {7, 1, 1, 1, 0, 0});
     if (!(s->flags & LTB_SESSION_NO_HALO) && m->wt[kStem] &&
-        stem_make_plan(s->img_pad, B, m->wt[kStem], m->bias[kStem], out.p, out.Ctot, out.c_off, &s->stem) == 0)
+        stem_make_plan(s->img_pad, B, m->wt[kStem], m->bias[kStem], out.p, out.Ctot, out.c_off, &s->stem) == 0) {
+      Op so;
       so.type = 5;
-    s->ops.push_back(so);
+      so.conv.p = p;
+      s->ops.push_back(so);
+    } else if (push_conv(kStem, p)) {
+      return 1;
+    }
     record(kStem, out);
   }
   {
@@ -563,7 +440,7 @@ static int build_plan(ltb_w2l_session* s) {
       View prev = cat_skip(8 - b);  // output of block b-1 lives in cat[7-(b-1)]
       for (int li = first[b]; li <= last[b]; ++li) {
         const LDef& L = kLayers[li];
-        const int OH = out_dim(prev.H, L.k, L.sy, L.pad), OW = out_dim(prev.W, L.k, L.sx, L.pad);
+        const int OH = conv_out_dim(prev.H, L.k, L.sy, L.pad), OW = conv_out_dim(prev.W, L.k, L.sx, L.pad);
         View o;
         if (li == last[b]) {
           o = cat_skip(7 - b);
@@ -585,11 +462,9 @@ static int build_plan(ltb_w2l_session* s) {
     if (new_tmp(4, 4, 512, &t)) return 1;
     {
       const View in = cat_all(0);
-      ConvParams p = conv_base(in.p, B, 1, 1, in.Ctot, 0, 1024, t.p, 1, 1, 16 * 512, 0, 16 * 512, m->w[kConvT4], 1024,
-                               m->bias[kConvT4], true);
-      p.ph[0].ntaps = 1;
-      p.ph[0].dy[0] = p.ph[0].dx[0] = 0;
-      push_conv(kConvT4, p);
+      const ConvParams p = conv_params(ConvMode::Dense, B, {in.p, in.Ctot, 0}, 1, 1, 1024, {t.p, 16 * 512, 0}, 1, 1, 16 * 512,
+                                       ConvSlice{}, m->w[kConvT4], 1024, 0, m->bias[kConvT4], true, {1, 1, 1, 1, 0, 0});
+      if (push_conv(kConvT4, p)) return 1;
       record(kConvT4, t);
     }
     if (add_conv(35, t, cat_dec(1), &t)) return 1;
@@ -617,17 +492,11 @@ static int build_plan(ltb_w2l_session* s) {
   View h;
   if (new_tmp(256, 256, 32, &h)) return 1;
   if (add_conv(53, cat_all(7), h, nullptr)) return 1;
-  if (!keep && s->ops.back().type == 4 && s->halo_plans[s->ops.back().halo].BN == 32) {
-    // fuse the 1x1 head + sigmoid into the epilogue of layer 53 (its 32-channel activations are never stored)
-    HaloParams& hp = s->halo_plans[s->ops.back().halo].hp;
-    hp.head_w = m->head_w;
-    hp.head_b = m->head_b;
-    hp.head_out = s->pred;
-  } else {
+  // fuse the 1x1 head + sigmoid into the epilogue of layer 53 (its 32-channel activations are then never stored)
+  if (keep || !conv_plan_fuse_head(&s->ops.back().conv, m->head_w, m->head_b, s->pred)) {
     Op o;
-    std::memset(&o.cp, 0, sizeof(o.cp));
     o.type = 3;
-    o.cp.in = h.p;
+    o.head_in = h.p;
     s->ops.push_back(o);
   }
   return 0;
@@ -671,11 +540,11 @@ static int run_ops(ltb_w2l_session* s, bool with_mel, cudaEvent_t* events = null
     }
     cudaError_t e = cudaSuccess;
     switch (o.type) {
-      case 0: e = launch_conv_gather(o.cp, st, s->splitk_ws[st == s->st2 ? 1 : 0], kSplitKFloats); break;
+      case 0:
+      case 4: e = conv_launch(o.conv, st, s->splitk_ws[st == s->st2 ? 1 : 0], kSplitKFloats); break;
       case 1: e = launch_w2l_prep_faces(s->a->faces, s->a->n, s->d_index, s->B, s->img_pad, st, s->d_slots); break;
-      case 2: e = launch_w2l_audio_conv0(s->mel, s->m->w0, s->m->bias[0], o.cp.out, s->B, st); break;
-      case 3: e = launch_w2l_head(o.cp.in, s->m->head_w, s->m->head_b, s->pred, s->B * 65536, st); break;
-      case 4: e = launch_conv_halo(s->halo_plans[o.halo], st); break;
+      case 2: e = launch_w2l_audio_conv0(s->mel, s->m->w0, s->m->bias[0], o.audio_out, s->B, st); break;
+      case 3: e = launch_w2l_head(o.head_in, s->m->head_w, s->m->head_b, s->pred, s->B * 65536, st); break;
       case 5: e = launch_stem(s->stem, st); break;
       case 6:
         if (with_mel) e = launch_mel_step(s->pcm, s->pcm_cap, s->B, s->l, s->fps, s->mel_spec, s->mel_mel, s->mel, st);
@@ -1201,7 +1070,8 @@ int ltb_w2l_profile_ops(ltb_w2l_session* s, int index, int max_ops, int* n_ops, 
     if (flops) {
       double f = 0;
       if (o.type == 0 || o.type == 4 || o.type == 5) {
-        for (int p = 0; p < o.cp.nphases; ++p) f += 2.0 * o.cp.M * o.cp.Cout * (double)o.cp.ph[p].ntaps * o.cp.Cin;
+        const ConvParams& cp = o.conv.p;
+        for (int p = 0; p < cp.nphases; ++p) f += 2.0 * cp.M * cp.Cout * (double)cp.ph[p].ntaps * cp.Cin;
       }
       flops[i] = f;
     }
@@ -1302,149 +1172,6 @@ int ltb_w2l_layer_read(ltb_w2l_session* s, int layer, void* out_f16, size_t nbyt
   LTB_CUDA(cudaStreamSynchronize(s->st));
   LTB_CUDA(cudaMemcpy2D(out_f16, (size_t)lo.C * 2, lo.p + lo.c_off, (size_t)lo.Ctot * 2, (size_t)lo.C * 2, rows,
                         cudaMemcpyDeviceToHost));
-  return 0;
-}
-
-static int conv2d_f16_impl(const ltb_conv_desc* d, const void* in_f16, const float* w_f32, const float* bias_f32,
-                           const void* res_f16, void* out_f16, int reps, float* ms_out);
-
-int ltb_conv2d_f16(const ltb_conv_desc* d, const void* in_f16, const float* w_f32, const float* bias_f32,
-                   const void* res_f16, void* out_f16) {
-  return conv2d_f16_impl(d, in_f16, w_f32, bias_f32, res_f16, out_f16, 0, nullptr);
-}
-
-int ltb_conv2d_f16_timed(const ltb_conv_desc* d, const void* in_f16, const float* w_f32, const float* bias_f32,
-                         const void* res_f16, void* out_f16, int reps, float* ms_per_launch) {
-  if (reps < 1 || !ms_per_launch) return LTB_FAIL("conv2d_f16_timed: reps >= 1 and a result pointer are required");
-  return conv2d_f16_impl(d, in_f16, w_f32, bias_f32, res_f16, out_f16, reps, ms_per_launch);
-}
-
-static int conv2d_f16_impl(const ltb_conv_desc* d, const void* in_f16, const float* w_f32, const float* bias_f32,
-                           const void* res_f16, void* out_f16, int reps, float* ms_out) {
-  if (!d || !in_f16 || !w_f32 || !bias_f32 || !out_f16) return LTB_FAIL("null argument");
-  if (d->has_res && !res_f16) return LTB_FAIL("has_res set but res is null");
-  int OH, OW, Ktot;
-  std::vector<__half> wp;
-  if (d->transposed) {
-    if (d->KH != 3 || d->KW != 3) return LTB_FAIL("transposed conv: only k=3,s=2,p=1,op=1");
-    OH = d->IH * 2;
-    OW = d->IW * 2;
-    Ktot = 9 * d->Cin;
-    pack_convT_w(w_f32, d->Cin, d->Cout, wp);
-  } else {
-    if (d->KH * d->KW > kMaxTaps) return LTB_FAIL("kernel too large");
-    OH = out_dim(d->IH, d->KH, d->sy, d->pad);
-    OW = out_dim(d->IW, d->KW, d->sx, d->pad);
-    Ktot = d->KH * d->KW * d->Cin;
-    pack_conv_w(w_f32, d->Cout, d->Cin, d->KH, d->KW, wp);
-  }
-  if (OH <= 0 || OW <= 0) return LTB_FAIL("empty output");
-  const size_t in_b = (size_t)d->N * d->IH * d->IW * d->Cin * 2, out_b = (size_t)d->N * OH * OW * d->Cout * 2;
-  __half *din = nullptr, *dout = nullptr, *dw = nullptr, *dres = nullptr, *dwt = nullptr;
-  float* dbias = nullptr;
-  float* dws = nullptr;
-  int rc = 0;
-  auto cleanup = [&]() {
-    cudaFree(din);
-    cudaFree(dout);
-    cudaFree(dw);
-    cudaFree(dres);
-    cudaFree(dwt);
-    cudaFree(dws);
-    cudaFree(dbias);
-  };
-#define CK(x)                                                             \
-  do {                                                                    \
-    cudaError_t _e = (x);                                                 \
-    if (_e != cudaSuccess) {                                              \
-      rc = LTB_FAIL(std::string(#x) + ": " + cudaGetErrorString(_e));     \
-      cleanup();                                                          \
-      return rc;                                                          \
-    }                                                                     \
-  } while (0)
-  CK(cudaMalloc(&din, in_b));
-  CK(cudaMalloc(&dout, out_b));
-  CK(cudaMalloc(&dw, wp.size() * 2));
-  CK(cudaMalloc(&dbias, (size_t)d->Cout * 4));
-  CK(cudaMemcpy(din, in_f16, in_b, cudaMemcpyHostToDevice));
-  CK(cudaMemcpy(dw, wp.data(), wp.size() * 2, cudaMemcpyHostToDevice));
-  CK(cudaMemcpy(dbias, bias_f32, (size_t)d->Cout * 4, cudaMemcpyHostToDevice));
-  CK(cudaMemset(dout, 0xFF, out_b));  // NaN pattern: unwritten outputs are caught by the test
-  if (d->has_res) {
-    CK(cudaMalloc(&dres, out_b));
-    CK(cudaMemcpy(dres, res_f16, out_b, cudaMemcpyHostToDevice));
-  }
-  ConvParams p = conv_base(din, d->N, d->IH, d->IW, d->Cin, 0, d->Cin, dout, OH, OW, d->Cout, 0, d->Cout, dw, Ktot, dbias,
-                           d->relu != 0);
-  if (d->transposed) {
-    p.GH = d->IH;
-    p.GW = d->IW;
-    p.M = d->N * d->IH * d->IW;
-    p.osy = p.osx = 2;
-    phases_convT(p, d->Cin);
-  } else {
-    p.sy = d->sy;
-    p.sx = d->sx;
-    phases_conv(p, d->KH, d->KW, d->pad, d->Cin);
-  }
-  if (d->has_res) {
-    p.res = dres;
-    p.RCtot = d->Cout;
-    p.rc_off = 0;
-  }
-  const bool can_halo = conv_halo_supported(p);
-  if (d->force_path == 2 && !can_halo) {
-    cleanup();
-    return LTB_FAIL("force_path=2 but this geometry is not supported by the halo kernel");
-  }
-  if (d->force_path != 1 && can_halo) {
-    CK(cudaMalloc(&dwt, wp.size() * 2));
-    if (d->KH == 3)
-      CK(d->transposed ? launch_w_tap_major_convT(dw, dwt, d->Cout, d->Cin, nullptr) : launch_w_tap_major(dw, dwt, d->Cout, d->Cin, nullptr));
-    HaloPlan pl;
-    if (conv_halo_make_plan(p, dwt, &pl) != 0) {
-      cleanup();
-      return LTB_FAIL("halo plan / tensor map creation failed");
-    }
-    CK(launch_conv_halo(pl, nullptr));
-    if (reps > 0) {   // back-to-back launches of the same plan between two events (kernel development aid)
-      cudaEvent_t e0, e1;
-      CK(cudaEventCreate(&e0));
-      CK(cudaEventCreate(&e1));
-      for (int i = 0; i < 3; ++i) CK(launch_conv_halo(pl, nullptr));
-      CK(cudaEventRecord(e0, nullptr));
-      for (int i = 0; i < reps; ++i) CK(launch_conv_halo(pl, nullptr));
-      CK(cudaEventRecord(e1, nullptr));
-      CK(cudaEventSynchronize(e1));
-      float ms = 0.f;
-      CK(cudaEventElapsedTime(&ms, e0, e1));
-      *ms_out = ms / reps;
-      cudaEventDestroy(e0);
-      cudaEventDestroy(e1);
-    }
-  } else {
-    CK(cudaMalloc(&dws, ((size_t)1 << 22) * sizeof(float)));
-    CK(cudaMemset(dws, 0, ((size_t)1 << 22) * sizeof(float)));
-    CK(launch_conv_gather(p, nullptr, dws, (size_t)1 << 22));
-    if (reps > 0) {
-      cudaEvent_t e0, e1;
-      CK(cudaEventCreate(&e0));
-      CK(cudaEventCreate(&e1));
-      CK(cudaEventRecord(e0, nullptr));
-      for (int i = 0; i < reps; ++i) CK(launch_conv_gather(p, nullptr, dws, (size_t)1 << 22));
-      CK(cudaEventRecord(e1, nullptr));
-      CK(cudaEventSynchronize(e1));
-      float ms = 0.f;
-      CK(cudaEventElapsedTime(&ms, e0, e1));
-      *ms_out = ms / reps;
-      cudaEventDestroy(e0);
-      cudaEventDestroy(e1);
-    }
-  }
-  CK(cudaDeviceSynchronize());
-  CK(cudaMemcpy(out_f16, dout, out_b, cudaMemcpyDeviceToHost));
-#undef CK
-  cleanup();
   return 0;
 }
 

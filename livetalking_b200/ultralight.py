@@ -112,7 +112,7 @@ class UltraLightModel:
         ctx.conv(a, self.a3, a3, N=B, IH=32, IW=32, OH=16, OW=16, stride=(2, 2), pad=(1, 1), relu=True)
         a4 = self._ir(b, self.a4, a3)
         a5 = b.new(B, 10, 10, CH[4])
-        ctx.conv(a4, self.a5, a5, N=B, IH=16, IW=16, OH=10, OW=10, stride=(2, 2), pad=(3, 3), relu=True, no_halo=True)
+        ctx.conv(a4, self.a5, a5, N=B, IH=16, IW=16, OH=10, OW=10, stride=(2, 2), pad=(3, 3), relu=True)
         af = self._ir(b, self.a7, self._ir(b, self.a6, a5), view(cat5, CH[4], CH[4]))
         f = self._dc(b, self.fuse, cat5)
         if taps is not None:

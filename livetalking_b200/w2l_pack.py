@@ -63,7 +63,7 @@ def _np(t) -> np.ndarray:
 
 
 # sub-pixel phase taps of ConvTranspose2d(k=3,s=2,p=1,op=1): out[2g+a] = sum over (d, k):
-#   a=0: (d=0,k=1)       a=1: (d=0,k=2), (d=+1,k=0)      (must match phases_convT in csrc/w2l_engine.cu)
+#   a=0: (d=0,k=1)       a=1: (d=0,k=2), (d=+1,k=0)      (must match kTd / kTk in csrc/conv_plan.cu)
 _T_TAPS = {0: [(0, 1)], 1: [(0, 2), (1, 0)]}
 
 
