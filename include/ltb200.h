@@ -183,11 +183,13 @@ int ltb_capture_end(ltb_ctx* c, ltb_graph** out);
 int ltb_graph_launch(ltb_ctx* c, ltb_graph* g);
 int ltb_graph_destroy(ltb_graph* g);
 
+/* stream-ordered device-to-device copy (e.g. a weight bank slot filled from weights already resident on the device) */
+int ltb_d2d(ltb_ctx* c, void* dst_dev, const void* src_dev, size_t bytes);
 /* conv / linear / batched GEMM on the wgmma kernels (nn.Conv2d, nn.Linear, attention Q.K^T and P.V):
  * out[pix, co] = act(sum_{tap,ci} in[pix*s + tap - pad, ic_off+ci] * w[co, w_koff + tap*Cin + ci] + bias[co] (+ res[pix, co]))
  * w: fp16 [Cout][Ktot] (K-major rows); w_tap: optional tap-major copy [9][Cout][Cin] enabling the TMA halo kernel for
  * 3x3 s1 p1; bias may be NULL (zero).  zbatch > 1 runs zbatch independent GEMMs (z = zo*zdiv + zi) with element
- * offsets in_z*, w_z*, out_z* added to the base pointers. */
+ * offsets in_z*, w_z*, out_z* added to the base pointers.  no_halo: 0 = pick the kernel, 1 = gather kernel, 2 = TMA kernel or fail. */
 typedef struct ltb_conv_op {
   const void* in; const void* w; const void* w_tap; const float* bias; const void* res; void* out;
   int N, IH, IW, ICtot, ic_off, Cin;
@@ -204,6 +206,14 @@ typedef struct ltb_conv_op {
    * input is the LOW-resolution map (N, IH, IW), OH = 2*IH, OW = 2*IW; `w` / `w_tap` hold the 16 pre-summed sub-pixel slices
    * ([Cout][16][Cin] phase-major / [16][Cout][Cin] view-major, built by livetalking_b200.ops.ConvWeight.upconv()), Ktot = 16*Cin */
   int upsample2x;
+  /* optional grouped weights (one launch over the networks of several avatars): image n belongs to group n / group_images and
+   * uses bank slot s = group_slot[n / group_images], i.e. weights w + s * w_slot_stride and bias + s * bias_slot_stride (elements;
+   * w_slot_stride * 2 bytes must be a multiple of 16 for the TMA kernel).  group_slot is an int32 DEVICE table read when the
+   * kernel runs (values in [0, slots)), so one captured graph serves any assignment.  NULL = ungrouped.  Grouped ops run the
+   * TMA kernel's GEMM mode (1x1) or the gather kernel; they cannot be combined with zbatch, gn_stats or upsample2x. */
+  const int* group_slot;
+  int group_images, slots;
+  long long w_slot_stride, bias_slot_stride;
 } ltb_conv_op;
 int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d);
 int ltb_op_w_tap_major(ltb_ctx* c, const void* w, void* wt, int cout, int cin);
@@ -236,13 +246,28 @@ int ltb_op_attention(ltb_ctx* c, const void* q, int q_pitch, const void* k, int 
  * [ic_off, ic_off+C)), w_tap fp16 [9][C], bias fp32 [C], pad 1, stride 1|2 -> out (pitch OCtot, offset oc_off). */
 int ltb_op_dwconv3x3(ltb_ctx* c, const void* x, int N, int IH, int IW, int ICtot, int ic_off, int C, const void* w_tap, const float* bias, int stride,
                      int relu, void* out, int OCtot, int oc_off);
+/* grouped form (see ltb_conv_op.group_slot): image n uses w_tap + s * w_slot_stride and bias + s * bias_slot_stride, s = group_slot[n /
+ * group_images] (int32 device table) */
+int ltb_op_dwconv3x3_grouped(ltb_ctx* c, const void* x, int N, int IH, int IW, int ICtot, int ic_off, int C, const void* w_tap, const float* bias,
+                             int stride, int relu, void* out, int OCtot, int oc_off, const int* group_slot, int group_images, long long w_slot_stride,
+                             long long bias_slot_stride);
 /* nn.Upsample(scale_factor=2, mode='bilinear', align_corners=True), unet.py:76, written into a channel slice (torch.cat, unet.py:88) */
 int ltb_op_upsample_bilinear2x(ltb_ctx* c, const void* x, int N, int H, int W, int ICtot, int ic_off, int C, void* out, int OCtot, int oc_off);
 /* LightReal.inference_batch input glue, avatars/ultralight_avatar.py:146-160: faces u8 [nf,168,168,3], frame b = mirror_index(nf,
  * *d_index + b) -> fp16 [B,160,160,16] (ch 0-2 crop/255, ch 3-5 with the filled rectangle (5,5,150,145), ch 6-15 zero) */
 int ltb_op_ul_prep(ltb_ctx* c, const void* faces_u8, int nf, const void* d_index, int B, void* out);
+/* grouped form: image b belongs to group g = b / group_images, whose crops come from groups_dev[g] (a DEVICE table): frame
+ * mirror_index(nf, index + b - g * group_images) of that group's faces */
+typedef struct ltb_ul_prep_group {
+  const void* faces; /* device u8 [nf,168,168,3] */
+  int nf, index;
+} ltb_ul_prep_group;
+int ltb_op_ul_prep_grouped(ltb_ctx* c, const void* groups_dev, int group_images, int B, void* out);
 /* 1x1 conv 32 -> 3 + sigmoid, x 255 (OutConv + F.sigmoid, unet.py:224-225; "* 255." ultralight_avatar.py:168): x fp16 [npix][32] */
 int ltb_op_head_sigmoid255(ltb_ctx* c, const void* x, const float* w3x32, const float* b3, long long npix, float* pred);
+/* grouped form: pixel i of image n = i / hw uses w3x32 + s * w_slot_stride and b3 + s * bias_slot_stride, s = group_slot[n / group_images] */
+int ltb_op_head_sigmoid255_grouped(ltb_ctx* c, const void* x, const float* w3x32, const float* b3, long long npix, float* pred, int hw,
+                                   const int* group_slot, int group_images, long long w_slot_stride, long long bias_slot_stride);
 /* LightReal.paste_back_frame, ultralight_avatar.py:171-184: crop[4:164,4:164] = pred.astype(u8); cv2.resize(crop, bbox) into the
  * frame; coords int32 [nf][4] = (x1,y1,x2,y2); pred f32 [B,160,160,3]; job j < count pastes slot slot0+j into out[j] for frame
  * explicit_idx (>= 0) or mirror_index(nf, index + j).  Bit-exact with OpenCV. */

@@ -26,7 +26,13 @@ class ConvOp(C.Structure):
                                         "rc_off", "KH", "KW", "sy", "sx", "pad_t", "pad_l", "Ktot", "w_koff", "relu", "no_halo",
                                         "zbatch", "zdiv")] +
                 [(n, C.c_longlong) for n in ("in_zo", "in_zi", "w_zo", "w_zi", "out_zo", "out_zi")] +
-                [("gn_stats", C.c_void_p), ("gn_groups", C.c_int), ("gn_hw", C.c_int), ("upsample2x", C.c_int)])
+                [("gn_stats", C.c_void_p), ("gn_groups", C.c_int), ("gn_hw", C.c_int), ("upsample2x", C.c_int)] +
+                [("group_slot", C.c_void_p), ("group_images", C.c_int), ("slots", C.c_int), ("w_slot_stride", C.c_longlong),
+                 ("bias_slot_stride", C.c_longlong)])
+
+
+class UlPrepGroup(C.Structure):
+    _fields_ = [("faces", C.c_void_p), ("nf", C.c_int), ("index", C.c_int)]
 
 
 class MtPasteOp(C.Structure):
@@ -90,6 +96,7 @@ _SIGS = {
     "ltb_h2d": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     "ltb_d2h": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     "ltb_set_i32": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
+    "ltb_d2d": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]),
     "ltb_capture_begin": (C.c_int, [C.c_void_p]),
     "ltb_capture_end": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "ltb_graph_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
@@ -112,10 +119,16 @@ _SIGS = {
                                    C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_int]),
     "ltb_op_dwconv3x3": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                    C.c_int, C.c_void_p, C.c_int, C.c_int]),
+    "ltb_op_dwconv3x3_grouped": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                           C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_longlong,
+                                           C.c_longlong]),
     "ltb_op_upsample_bilinear2x": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                              C.c_int]),
     "ltb_op_ul_prep": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
+    "ltb_op_ul_prep_grouped": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     "ltb_op_head_sigmoid255": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p]),
+    "ltb_op_head_sigmoid255_grouped": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_void_p,
+                                                 C.c_int, C.c_longlong, C.c_longlong]),
     "ltb_op_ul_paste": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                   C.c_int, C.c_int, C.c_int]),
     "ltb_op_hubert_conv0": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),

@@ -40,7 +40,9 @@ __device__ __forceinline__ uint32_t swz_chunk(int row, int j) {
   return (uint32_t)(j ^ ((row >> 2) & 1));
 }
 
-template <int BN, int KB>
+// GRP: grouped weights (ConvParams::group_slot).  A CTA's 128 rows share one weight tile, so M-tiles are enumerated per group
+// (blockIdx.x = group * tiles per group + tile) and rows past the group's end are neither gathered nor written.
+template <int BN, int KB, bool GRP>
 __global__ void __launch_bounds__(kGatherThreads) conv_gather_wgmma_kernel(const __grid_constant__ ConvParams p) {
   using C = GatherCfg<BN, KB>;
   extern __shared__ uint8_t smem_raw[];
@@ -60,7 +62,9 @@ __global__ void __launch_bounds__(kGatherThreads) conv_gather_wgmma_kernel(const
     w_base += zo * p.w_zo + zi * p.w_zi;
     out_base += zo * p.out_zo + zi * p.out_zi;
   }
-  const int m0 = blockIdx.x * 128;
+  const int g_rows = GRP ? p.group_images * p.GH * p.GW : 0, g_tiles = (g_rows + 127) / 128;
+  const int group = GRP ? (int)blockIdx.x / g_tiles : 0;
+  const int m0 = GRP ? group * g_rows + ((int)blockIdx.x - group * g_tiles) * 128 : blockIdx.x * 128;
   const int n0 = blockIdx.y * BN;
   const int cpt = p.Cin / KB;  // K chunks per tap
   int it_begin = 0, kiters = ph.ntaps * cpt;
@@ -72,6 +76,15 @@ __global__ void __launch_bounds__(kGatherThreads) conv_gather_wgmma_kernel(const
   // PDL: everything below touches activations
   pdl_launch_dependents();
   pdl_wait();
+  const float* bias_g = nullptr;
+  if constexpr (GRP) {   // the slot table is written by the stream before this kernel: read it after the wait
+    const int slot = p.group_slot[group];
+    w_base += slot * p.w_slot_stride;
+    bias_g = p.bias + slot * p.bias_slot_stride;
+  }
+  // the ungrouped instantiation reads the parameters directly (same code as before grouping existed)
+  const float* const bias = GRP ? bias_g : p.bias;
+  const int M = GRP ? (group + 1) * g_rows : p.M;
 
   // per gathered row: input coordinates of tap (0,0) and the element offset of that pixel (+ this thread's 16-byte K chunk);
   // per K iteration only one uniform tap offset is added
@@ -83,7 +96,7 @@ __global__ void __launch_bounds__(kGatherThreads) conv_gather_wgmma_kernel(const
 #pragma unroll
   for (int i = 0; i < C::RPT; ++i) {
     const int m = m0 + r0 + i * C::RSTEP;
-    if (m < p.M) {
+    if (m < M) {
       const int b = m / gsz;
       const int rem = m - b * gsz;
       const int gy = rem / p.GW;
@@ -154,7 +167,7 @@ __global__ void __launch_bounds__(kGatherThreads) conv_gather_wgmma_kernel(const
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const int m = m0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * hh;
-    if (m >= p.M) continue;
+    if (m >= M) continue;
     if (p.ksplit > 1) {
       // split-K: this CTA's fp32 partial goes to its own slice ws[split][m][co] (plain stores, no atomics)
       float* wrow = p.ws + ((size_t)blockIdx.z * p.M + m) * p.Cout + n0;
@@ -173,7 +186,7 @@ __global__ void __launch_bounds__(kGatherThreads) conv_gather_wgmma_kernel(const
 #pragma unroll
     for (int i = 0; i < BN / 8; ++i) {
       const int c = 8 * i + cq;
-      const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c));
+      const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + n0 + c));
       float x = acc[4 * i + 2 * hh] + bb.x, y = acc[4 * i + 2 * hh + 1] + bb.y;
       if (rptr) {
         const float2 rf = __half22float2(__ldcg(reinterpret_cast<const __half2*>(rptr + c)));
@@ -191,13 +204,19 @@ __global__ void __launch_bounds__(kGatherThreads) conv_gather_wgmma_kernel(const
   }
 }
 
-template <int BN, int KB>
-static cudaError_t launch_one(const ConvParams& p, cudaStream_t st) {
+template <int BN, int KB, bool GRP>
+static cudaError_t launch_grp(const ConvParams& p, cudaStream_t st) {
   using C = GatherCfg<BN, KB>;
   static SmemConfigOnce once;
-  if (cudaError_t e = once.ensure(conv_gather_wgmma_kernel<BN, KB>, C::SMEM_BYTES); e != cudaSuccess) return e;
-  dim3 grid((p.M + 127) / 128, p.Cout / BN, p.ksplit > 1 ? p.ksplit : p.nphases * (p.zbatch > 1 ? p.zbatch : 1));
-  return launch_kernel_pdl(conv_gather_wgmma_kernel<BN, KB>, grid, dim3(kGatherThreads), C::SMEM_BYTES, st, p);
+  if (cudaError_t e = once.ensure(conv_gather_wgmma_kernel<BN, KB, GRP>, C::SMEM_BYTES); e != cudaSuccess) return e;
+  const int mt = GRP ? (p.N / p.group_images) * ((p.group_images * p.GH * p.GW + 127) / 128) : (p.M + 127) / 128;
+  dim3 grid(mt, p.Cout / BN, p.ksplit > 1 ? p.ksplit : p.nphases * (p.zbatch > 1 ? p.zbatch : 1));
+  return launch_kernel_pdl(conv_gather_wgmma_kernel<BN, KB, GRP>, grid, dim3(kGatherThreads), C::SMEM_BYTES, st, p);
+}
+
+template <int BN, int KB>
+static cudaError_t launch_one(const ConvParams& p, cudaStream_t st) {
+  return p.group_slot ? launch_grp<BN, KB, true>(p, st) : launch_grp<BN, KB, false>(p, st);
 }
 
 template <int KB>
@@ -279,7 +298,7 @@ cudaError_t launch_conv_gather(const ConvParams& p_in, cudaStream_t st, float* s
   p.ws = nullptr;
   const int kiters = p.ph[0].ntaps * (p.Cin / kb);
   const long mt = (p.M + 127) / 128;
-  if (splitk_ws && p.nphases == 1 && p.zbatch <= 1 && p.osy == 1 && p.osx == 1 && p.GH == p.OH && p.GW == p.OW && kiters >= 32 && mt <= 8) {
+  if (splitk_ws && !p.group_slot && p.nphases == 1 && p.zbatch <= 1 && p.osy == 1 && p.osx == 1 && p.GH == p.OH && p.GW == p.OW && kiters >= 32 && mt <= 8) {
     int bn2 = 0;
     for (int c : {128, 64, 32, 16})
       if (p.Cout % c == 0) {

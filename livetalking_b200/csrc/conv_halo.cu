@@ -112,8 +112,10 @@ __device__ __forceinline__ void fat_issue(float (&acc)[R], int j, int k, uint32_
       ...);
 }
 
-template <int BN, int NSUB, int NACC, int TAPS, int RC>
+// GRP: grouped GEMM mode (TAPS == 1 only): per-group M-tiles and weight slots, see HaloParams::group_slot
+template <int BN, int NSUB, int NACC, int TAPS, int RC, bool GRP>
 __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const __grid_constant__ HaloParams p) {
+  static_assert(!GRP || TAPS == 1, "grouped weights exist in GEMM mode only");
   using C = HaloCfg<BN, NSUB, NACC, TAPS, RC>;
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t a_full[C::A_STAGES], a_empty[C::A_STAGES];
@@ -173,6 +175,12 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
         const int nt = t / tiles_m;
         int mt = t - nt * tiles_m;
         int img = 0, y0 = 0, x0 = 0;
+        int g_row = 0, g_slot = 0;   // grouped: first A row of the tile and the group's weight slot
+        if constexpr (GRP) {
+          const int g = mt / p.group_tiles;
+          g_row = g * p.group_rows + (mt - g * p.group_tiles) * (128 * NSUB);
+          g_slot = p.group_slot[g];
+        }
         if (kHaloMode) {
           img = mt / (p.tiles_x * p.tiles_y);
           mt -= img * (p.tiles_x * p.tiles_y);
@@ -194,6 +202,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
                 tma_load_4d(a_smem + as * C::A_BYTES + pl * C::PLANE_BYTES, &p.tm_in, smem_u32(&a_full[as]), c * 64,
                             2 * (x0 + 1) - (pl & 1), 2 * (y0 + 1) - (pl >> 1), img);
             } else if (kHaloMode) tma_load_4d(a_smem + as * C::A_BYTES, &p.tm_in, smem_u32(&a_full[as]), c * 64, x0, y0, img);
+            else if constexpr (GRP) tma_load_2d(a_smem + as * C::A_BYTES, &p.tm_in, smem_u32(&a_full[as]), c * 64, g_row);
             else tma_load_2d(a_smem + as * C::A_BYTES, &p.tm_in, smem_u32(&a_full[as]), c * 64, mt * (128 * NSUB));
           }
           ++ai;
@@ -208,6 +217,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
             }
             mbar_arrive_expect_tx(smem_u32(&b_full[bs]), C::B_BYTES);
             if (kHaloMode) tma_load_3d(b_smem + bs * C::B_BYTES, &p.tm_w, smem_u32(&b_full[bs]), c * 64, nt * BN, j * C::TG);
+            else if constexpr (GRP) tma_load_3d(b_smem + bs * C::B_BYTES, &p.tm_w, smem_u32(&b_full[bs]), c * 64, nt * BN, g_slot);
             else tma_load_2d(b_smem + bs * C::B_BYTES, &p.tm_w, smem_u32(&b_full[bs]), c * 64, nt * BN);
             ++bi;
           }
@@ -319,11 +329,17 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
         tx = mt - ty * p.tiles_x;
       }
       const int n0 = nt * BN;
+      const float* bias = p.bias;
+      int g_tile = 0;   // grouped: this tile's group; its rows [g_tile * group_rows, (g_tile + 1) * group_rows) are the only ones written
+      if constexpr (GRP) {
+        g_tile = mt / p.group_tiles;
+        bias += p.group_slot[g_tile] * p.bias_slot_stride;
+      }
       const bool has_res = (p.res != nullptr) && !LTB_DIAG(1);
       const bool head = kHeadOk && p.head_out != nullptr;
       float2 bb[BN / 8];
 #pragma unroll
-      for (int i = 0; i < BN / 8; ++i) bb[i] = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * i + cq));
+      for (int i = 0; i < BN / 8; ++i) bb[i] = __ldg(reinterpret_cast<const float2*>(bias + n0 + 8 * i + cq));
       const __half2 hmax = __floats2half2_rn(65504.f, 65504.f);
       const __half2 hlo = p.relu ? __floats2half2_rn(0.f, 0.f) : __floats2half2_rn(-65504.f, -65504.f);
 #pragma unroll
@@ -343,6 +359,11 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
               const int gy = ty * (16 * NSUB) + sub * 16 + wg * 8 + (r >> 3), gx = tx * 8 + (r & 7);
               opix = ((size_t)img * p.OH + gy * p.osy + p.acc_oy[sl]) * p.OW + gx * p.osx + p.acc_ox[sl];
               row_ok = gy < p.GH && gx < p.GW;   // tiles may overhang small / odd-sized maps
+            } else if constexpr (GRP) {
+              // rows past the group's end belong to the next group, computed here with the wrong weights: never written
+              const int lrow = (mt - g_tile * p.group_tiles) * (128 * NSUB) + sub * 128 + wg * 64 + r;
+              opix = (size_t)g_tile * p.group_rows + lrow;
+              row_ok = lrow < p.group_rows;
             } else {
               opix = (size_t)mt * (128 * NSUB) + sub * 128 + wg * 64 + r;   // GEMM mode: output row index
               row_ok = opix < (size_t)p.M;
@@ -513,6 +534,9 @@ static bool pick_cfg(const ConvParams& p, int* BN, int* NSUB, int* NACC);
 
 bool conv_halo_supported(const ConvParams& p) {
   if (p.zbatch > 1) return false;   // the halo kernel runs one GEMM per launch
+  // grouped weights: GEMM mode only (the weight map's slot stride must be 16-byte aligned); 3x3, stride-2, ConvT and upsample
+  // layers go to the gather kernel
+  if (p.group_slot && (!is_gemm(p) || (p.w_slot_stride * 2) % 16 != 0)) return false;
   if (is_gemm(p)) {
     // TMA GEMM: K-major rows with 16-byte aligned pitch; worth it from a few M tiles upwards
     return p.Cout % 32 == 0 && p.Cin % 8 == 0 && p.Cin >= 32 && (p.ICtot % 8) == 0 && (p.ic_off % 8) == 0 && (p.Ktot % 8) == 0 &&
@@ -607,6 +631,7 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
   if (!conv_halo_supported(p)) return 1;
   HaloParams& h = out->hp;
   std::memset(&h, 0, sizeof(h));
+  out->grouped = false;
   int BN, NSUB, NACC;
   if (!pick_cfg(p, &BN, &NSUB, &NACC)) return 1;
   out->BN = BN;
@@ -623,10 +648,11 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
     cuuint64_t strides[1] = {(cuuint64_t)p.ICtot * 2};
     cuuint32_t box[2] = {64, (cuuint32_t)(128 * NSUB)};
     if (!encode(&h.tm_in, 2, p.in + p.ic_off, dims, strides, box)) return 2;
-    cuuint64_t wdims[2] = {(cuuint64_t)p.Cin, (cuuint64_t)p.Cout};
-    cuuint64_t wstrides[1] = {(cuuint64_t)p.Ktot * 2};
-    cuuint32_t wbox[2] = {64, (cuuint32_t)BN};
-    if (!encode(&h.tm_w, 2, p.w + p.ph[0].koff, wdims, wstrides, wbox)) return 2;
+    // grouped: 3-D (K, Cout, slot) over the whole bank, one slot per box
+    cuuint64_t wdims[3] = {(cuuint64_t)p.Cin, (cuuint64_t)p.Cout, (cuuint64_t)p.slots};
+    cuuint64_t wstrides[2] = {(cuuint64_t)p.Ktot * 2, (cuuint64_t)p.w_slot_stride * 2};
+    cuuint32_t wbox[3] = {64, (cuuint32_t)BN, 1};
+    if (!encode(&h.tm_w, p.group_slot ? 3 : 2, p.w + p.ph[0].koff, wdims, wstrides, wbox)) return 2;
   } else
   // input: 4-D (C, W, H, N) view of the NHWC channel slice
   {
@@ -690,6 +716,14 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
   if (gemm) {
     h.halo_y0 = h.halo_x0 = 0;
     h.tiles_x = (p.M + 128 * NSUB - 1) / (128 * NSUB);
+    if (p.group_slot) {
+      out->grouped = true;
+      h.group_slot = p.group_slot;
+      h.group_rows = p.group_images * p.GH * p.GW;
+      h.group_tiles = (h.group_rows + 128 * NSUB - 1) / (128 * NSUB);
+      h.bias_slot_stride = p.bias_slot_stride;
+      h.tiles_x = (p.N / p.group_images) * h.group_tiles;
+    }
     h.tiles_y = 1;
     h.total_tiles = h.tiles_x * h.tiles_n;
     return 0;
@@ -700,13 +734,13 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
   return 0;
 }
 
-template <int BN, int NSUB, int NACC, int TAPS = 9, int RC = 0>
+template <int BN, int NSUB, int NACC, int TAPS = 9, int RC = 0, bool GRP = false>
 static cudaError_t launch_cfg(const HaloPlan& pl, int sms, cudaStream_t st) {
   using C = HaloCfg<BN, NSUB, NACC, TAPS, RC>;
   static SmemConfigOnce once;
-  if (cudaError_t e = once.ensure(conv_halo_wgmma_kernel<BN, NSUB, NACC, TAPS, RC>, C::SMEM_BYTES); e != cudaSuccess) return e;
+  if (cudaError_t e = once.ensure(conv_halo_wgmma_kernel<BN, NSUB, NACC, TAPS, RC, GRP>, C::SMEM_BYTES); e != cudaSuccess) return e;
   const int grid = pl.hp.total_tiles < sms ? pl.hp.total_tiles : sms;
-  return launch_kernel_pdl(conv_halo_wgmma_kernel<BN, NSUB, NACC, TAPS, RC>, dim3(grid), dim3(kHaloThreads), C::SMEM_BYTES, st, pl.hp);
+  return launch_kernel_pdl(conv_halo_wgmma_kernel<BN, NSUB, NACC, TAPS, RC, GRP>, dim3(grid), dim3(kHaloThreads), C::SMEM_BYTES, st, pl.hp);
 }
 
 cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
@@ -725,6 +759,16 @@ cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
   }
   if (pl.TAPS == 16) return (pl.BN == 64 && pl.NSUB == 1 && pl.NACC == 4) ? launch_cfg<64, 1, 4, 16>(pl, sms, st) : cudaErrorInvalidValue;
   const int key = pl.BN * 100 + pl.NSUB * 10 + pl.NACC;
+  if (pl.TAPS == 1 && pl.grouped) {
+    switch (key) {
+      case 12811: return launch_cfg<128, 1, 1, 1, 0, true>(pl, sms, st);
+      case 6421: return launch_cfg<64, 2, 1, 1, 0, true>(pl, sms, st);
+      case 6411: return launch_cfg<64, 1, 1, 1, 0, true>(pl, sms, st);
+      case 3221: return launch_cfg<32, 2, 1, 1, 0, true>(pl, sms, st);
+      case 3211: return launch_cfg<32, 1, 1, 1, 0, true>(pl, sms, st);
+    }
+    return cudaErrorInvalidValue;
+  }
   if (pl.TAPS == 1) {
     switch (key) {
       case 12811: return launch_cfg<128, 1, 1, 1>(pl, sms, st);

@@ -34,6 +34,11 @@ struct alignas(64) HaloParams {
   const float* head_w;
   const float* head_b;
   float* head_out;
+  // grouped GEMM mode (ConvParams::group_slot): M-tiles are enumerated per group of group_rows rows, tiles_x = groups *
+  // group_tiles; the weight map is 3-D (k, n, slot) over the bank and the bias of slot s starts at bias + s * bias_slot_stride
+  const int* group_slot;
+  int group_rows, group_tiles;
+  long long bias_slot_stride;
 #ifdef LTB_HALO_DIAG
   int dbg;      // diagnostic build only (tools/diag_halo.py): bit0 no epilogue global I/O, bit1 no epilogue at all,
                 // bit2 no MMAs, bit3 no A loads, bit4 no B loads.  Never compiled into libltb200.so.
@@ -43,6 +48,7 @@ struct alignas(64) HaloParams {
 struct HaloPlan {
   HaloParams hp;
   int BN, NSUB, NACC, TAPS;  // TAPS = 9 (3x3 conv / ConvT halo mode) or 1 (TMA GEMM mode: 1x1 conv / linear)
+  bool grouped;              // GEMM mode with per-group weight slots
 };
 
 bool conv_halo_supported(const ConvParams& p);

@@ -55,6 +55,13 @@ struct ConvParams {
   // 2x2 conv over the LOW-resolution input with pre-summed taps (16 weight slices [Cout][16][Cin], see ops.py
   // ConvWeight.upconv).  Halo kernel only (no gather fallback).
   int upconv;
+  // optional grouped weights (cross-session batching of networks that differ per avatar): image n belongs to group
+  // n / group_images and uses the weights / bias of bank slot group_slot[n / group_images] (read on the device, so one captured
+  // graph serves any assignment), i.e. w + slot * w_slot_stride and bias + slot * bias_slot_stride (elements).  The bank holds
+  // `slots` slots.  group_slot == nullptr: ungrouped.
+  const int* group_slot;
+  int group_images, slots;
+  long long w_slot_stride, bias_slot_stride;
 };
 
 }  // namespace ltb

@@ -89,6 +89,11 @@ ConvParams conv_params(ConvMode mode, int N, ConvSlice in, int IH, int IW, int C
 int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan* out) {
   out->p = p;
   out->halo = false;
+  if (p.group_slot) {
+    if (p.group_images < 1 || p.N % p.group_images || p.slots < 1 || p.w_slot_stride < 0 || p.bias_slot_stride < 0)
+      return LTB_FAIL("conv: grouped weights need N divisible by group_images >= 1, slots >= 1 and non-negative slot strides");
+    if (p.zbatch > 1 || p.upconv) return LTB_FAIL("conv: grouped weights cannot be combined with zbatch or the fused upsample");
+  }
   if (path == ConvPath::Gather) return 0;
   const bool gemm = p.nphases == 1 && p.ph[0].ntaps == 1;   // the halo kernel's GEMM mode reads the K-major rows
   if (!((w_tap || gemm) && conv_halo_supported(p))) {
@@ -108,7 +113,7 @@ cudaError_t conv_launch(const ConvPlan& pl, cudaStream_t st, float* splitk_ws, s
 
 bool conv_plan_fuse_gn_stats(ConvPlan* pl, float* stats, int groups, int hw) {
   const ConvParams& p = pl->p;
-  if (!pl->halo || p.oc_off != 0 || p.OCtot != p.Cout || !conv_halo_gn_fusable(pl->hp, p.Cout, groups, hw)) return false;
+  if (!pl->halo || pl->hp.grouped || p.oc_off != 0 || p.OCtot != p.Cout || !conv_halo_gn_fusable(pl->hp, p.Cout, groups, hw)) return false;
   HaloParams& h = pl->hp.hp;
   h.gn_stats = stats;
   h.gn_groups = groups;
@@ -119,7 +124,7 @@ bool conv_plan_fuse_gn_stats(ConvPlan* pl, float* stats, int groups, int hw) {
 }
 
 bool conv_plan_fuse_head(ConvPlan* pl, const float* w, const float* b, float* out) {
-  if (!pl->halo || pl->hp.BN != 32 || pl->p.Cout != 32) return false;
+  if (!pl->halo || pl->hp.grouped || pl->hp.BN != 32 || pl->p.Cout != 32) return false;
   pl->hp.hp.head_w = w;
   pl->hp.hp.head_b = b;
   pl->hp.hp.head_out = out;

@@ -40,7 +40,8 @@ struct ConvPlan {
 };
 
 // w_tap: device copy of the weights in the halo kernel's tap-major layout (see launch_w_tap_major*); null if there is none.
-// Returns 0, or 1 with the reason set as the last error.
+// Grouped ops (p.group_slot) run on the halo kernel's GEMM mode or on the gather kernel, never with zbatch, split-K, the fused
+// upsample or an epilogue fusion.  Returns 0, or 1 with the reason set as the last error.
 int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan* out);
 // splitk_ws: zero-initialised fp32 workspace of ws_floats floats for the gather kernel's split-K (one per stream)
 cudaError_t conv_launch(const ConvPlan& pl, cudaStream_t st, float* splitk_ws, size_t ws_floats);

@@ -27,8 +27,24 @@ bool attn_fused_supported(int d, int q_pitch, int kv_pitch, int n_pad);
 cudaError_t launch_attn_fused(const __half* q, int q_pitch, const __half* k, int kv_pitch, int kv_rows, const __half* vt, int n_pad, int B, int H,
                               int nq, int valid, int d, float scale, __half* out, int out_pitch, cudaStream_t st);
 // ---- UltraLight / HuBERT (ultralight.cu, hubert.cu)
+// grouped weights of the per-image ops: image n uses w + s * w_stride and bias + s * b_stride, s = slot[n / images] (device table)
+struct WeightGroups {
+  const int* slot;
+  int images;
+  long long w_stride, b_stride;
+};
+// grp == nullptr: ungrouped
 cudaError_t launch_dwconv3x3(const __half* x, int N, int IH, int IW, int ICtot, int ic_off, int C, const __half* w, const float* bias, int stride,
-                             int relu, __half* out, int OCtot, int oc_off, cudaStream_t st);
+                             int relu, __half* out, int OCtot, int oc_off, cudaStream_t st, const WeightGroups* grp = nullptr);
+// per-group crop source of launch_ul_prep_grouped (layout of ltb_ul_prep_group)
+struct UlPrepGroup {
+  const uint8_t* faces;
+  int nf, index;
+};
+cudaError_t launch_ul_prep_grouped(const UlPrepGroup* groups, int group_images, int B, __half* out, cudaStream_t st);
+// 32 -> 3 head + sigmoid * 255 (w2l_small.cu); grouped: hw pixels per image, hw % 256 == 0
+cudaError_t launch_head_grouped(const __half* x, const float* w3x32, const float* b3, float* pred, int npix, int hw, const WeightGroups& grp,
+                                cudaStream_t st);
 cudaError_t launch_upsample_bilinear2x(const __half* x, int N, int H, int W, int ICtot, int ic_off, int C, __half* out, int OCtot, int oc_off,
                                        cudaStream_t st);
 cudaError_t launch_ul_prep(const uint8_t* faces, int nf, const int* d_index, int B, __half* out, cudaStream_t st);

@@ -136,6 +136,12 @@ int ltb_d2h(ltb_ctx* c, void* dst_host, const void* src_dev, size_t bytes, int s
   if (sync) LTB_CUDA(cudaStreamSynchronize(c->st));
   return 0;
 }
+int ltb_d2d(ltb_ctx* c, void* dst_dev, const void* src_dev, size_t bytes) {
+  if (!c || !dst_dev || !src_dev) return LTB_FAIL("d2d: null argument");
+  LTB_CTX_ENTER(c);
+  LTB_CUDA(cudaMemcpyAsync(dst_dev, src_dev, bytes, cudaMemcpyDeviceToDevice, c->st));
+  return 0;
+}
 int ltb_set_i32(ltb_ctx* c, void* dptr, int value) {
   if (!c || !dptr) return LTB_FAIL("null argument");
   LTB_CTX_ENTER(c);
@@ -210,8 +216,16 @@ int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d) {
   p.w_zi = d->w_zi;
   p.out_zo = d->out_zo;
   p.out_zi = d->out_zi;
+  if (d->group_slot) {
+    if (d->gn_stats) return LTB_FAIL("conv2d: grouped weights cannot produce GroupNorm statistics");
+    p.group_slot = static_cast<const int*>(d->group_slot);
+    p.group_images = d->group_images;
+    p.slots = d->slots;
+    p.w_slot_stride = d->w_slot_stride;
+    p.bias_slot_stride = d->bias_slot_stride;
+  }
   // the fused upsample exists on the halo kernel only
-  const ConvPath path = d->upsample2x ? ConvPath::Halo : d->no_halo ? ConvPath::Gather : ConvPath::Auto;
+  const ConvPath path = d->upsample2x ? ConvPath::Halo : d->no_halo == 1 ? ConvPath::Gather : d->no_halo == 2 ? ConvPath::Halo : ConvPath::Auto;
   ConvPlan pl;
   if (conv_plan(p, static_cast<const __half*>(d->w_tap), path, &pl)) return 1;
   const bool want_stats = d->gn_stats != nullptr && d->gn_groups > 0 && d->gn_hw > 0 && (p.M % d->gn_hw) == 0 && d->zbatch <= 1;
@@ -341,6 +355,20 @@ int ltb_op_dwconv3x3(ltb_ctx* c, const void* x, int N, int IH, int IW, int ICtot
   c->launches += 1;
   return 0;
 }
+int ltb_op_dwconv3x3_grouped(ltb_ctx* c, const void* x, int N, int IH, int IW, int ICtot, int ic_off, int C, const void* w_tap, const float* bias,
+                             int stride, int relu, void* out, int OCtot, int oc_off, const int* group_slot, int group_images, long long w_slot_stride,
+                             long long bias_slot_stride) {
+  if (!c || !x || !w_tap || !bias || !out || !group_slot) return LTB_FAIL("dwconv3x3_grouped: null argument");
+  LTB_CTX_ENTER(c);
+  const WeightGroups grp{group_slot, group_images, w_slot_stride, bias_slot_stride};
+  cudaError_t e = launch_dwconv3x3(static_cast<const __half*>(x), N, IH, IW, ICtot, ic_off, C, static_cast<const __half*>(w_tap), bias, stride, relu,
+                                   static_cast<__half*>(out), OCtot, oc_off, c->st, &grp);
+  if (e != cudaSuccess)
+    return LTB_FAIL(std::string("dwconv3x3_grouped (C, pitches, offsets, w stride % 8 == 0; bias stride % 4 == 0; N % group_images == 0): ") +
+                    cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
 int ltb_op_upsample_bilinear2x(ltb_ctx* c, const void* x, int N, int H, int W, int ICtot, int ic_off, int C, void* out, int OCtot, int oc_off) {
   if (!c || !x || !out) return LTB_FAIL("upsample_bilinear2x: null argument");
   LTB_CTX_ENTER(c);
@@ -354,6 +382,25 @@ int ltb_op_ul_prep(ltb_ctx* c, const void* faces_u8, int nf, const void* d_index
   LTB_CTX_ENTER(c);
   cudaError_t e = launch_ul_prep(static_cast<const uint8_t*>(faces_u8), nf, static_cast<const int*>(d_index), B, static_cast<__half*>(out), c->st);
   if (e != cudaSuccess) return LTB_FAIL(std::string("ul_prep: ") + cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
+int ltb_op_ul_prep_grouped(ltb_ctx* c, const void* groups_dev, int group_images, int B, void* out) {
+  static_assert(sizeof(UlPrepGroup) == sizeof(ltb_ul_prep_group), "ltb_ul_prep_group layout");
+  if (!c || !groups_dev || !out || B < 1) return LTB_FAIL("ul_prep_grouped: bad argument");
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_ul_prep_grouped(static_cast<const UlPrepGroup*>(groups_dev), group_images, B, static_cast<__half*>(out), c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("ul_prep_grouped (B % group_images == 0): ") + cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
+int ltb_op_head_sigmoid255_grouped(ltb_ctx* c, const void* x, const float* w3x32, const float* b3, long long npix, float* pred, int hw,
+                                   const int* group_slot, int group_images, long long w_slot_stride, long long bias_slot_stride) {
+  if (!c || !x || !w3x32 || !b3 || !pred || !group_slot) return LTB_FAIL("head_sigmoid255_grouped: null argument");
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_head_grouped(static_cast<const __half*>(x), w3x32, b3, pred, (int)npix, hw,
+                                      WeightGroups{group_slot, group_images, w_slot_stride, bias_slot_stride}, c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("head_sigmoid255_grouped (hw % 256 == 0, whole groups): ") + cudaGetErrorString(e));
   c->launches += 1;
   return 0;
 }

@@ -14,9 +14,11 @@ namespace ltb {
 // ------------------------------------------------------------------------------------------------ depthwise 3x3
 // x [N,IH,IW] pixels of ICtot halves (channels [ic_off, ic_off+C)), w tap-major [9][C] fp16 (BN folded), bias fp32 [C];
 // out [N,OH,OW] pixels of OCtot halves.  pad 1, stride s.  One thread = 8 channels of one output pixel.
+// GRP: per-image weight slots (WeightGroups)
+template <bool GRP>
 __global__ void __launch_bounds__(256) dwconv3x3_kernel(const __half* __restrict__ x, int N, int IH, int IW, int ICtot, int ic_off, int C,
                                                         const __half* __restrict__ w, const float* __restrict__ bias, int stride, int relu,
-                                                        __half* __restrict__ out, int OH, int OW, int OCtot, int oc_off) {
+                                                        __half* __restrict__ out, int OH, int OW, int OCtot, int oc_off, const WeightGroups grp) {
   pdl_launch_dependents();   // a PDL-launched successor (the conv kernels) may start its prologue now; it waits before reading
   const int cg = C >> 3;
   const size_t total = (size_t)N * OH * OW * cg;
@@ -24,9 +26,16 @@ __global__ void __launch_bounds__(256) dwconv3x3_kernel(const __half* __restrict
     const int c8 = (int)(i % cg) * 8;
     const size_t pix = i / cg;
     const int ox = (int)(pix % OW), oy = (int)((pix / OW) % OH), n = (int)(pix / ((size_t)OW * OH));
+    const __half* wn = w;
+    const float* bn = bias;
+    if constexpr (GRP) {
+      const int s = grp.slot[n / grp.images];
+      wn += s * grp.w_stride;
+      bn += s * grp.b_stride;
+    }
     float acc[8];
     {
-      const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + c8)), b1 = __ldg(reinterpret_cast<const float4*>(bias + c8 + 4));
+      const float4 b0 = __ldg(reinterpret_cast<const float4*>(bn + c8)), b1 = __ldg(reinterpret_cast<const float4*>(bn + c8 + 4));
       acc[0] = b0.x, acc[1] = b0.y, acc[2] = b0.z, acc[3] = b0.w, acc[4] = b1.x, acc[5] = b1.y, acc[6] = b1.z, acc[7] = b1.w;
     }
 #pragma unroll
@@ -38,7 +47,7 @@ __global__ void __launch_bounds__(256) dwconv3x3_kernel(const __half* __restrict
         const int ix = ox * stride + kx - 1;
         if (ix < 0 || ix >= IW) continue;
         const uint4 xv = __ldg(reinterpret_cast<const uint4*>(x + (((size_t)n * IH + iy) * IW + ix) * ICtot + ic_off + c8));
-        const uint4 wv = __ldg(reinterpret_cast<const uint4*>(w + (size_t)(ky * 3 + kx) * C + c8));
+        const uint4 wv = __ldg(reinterpret_cast<const uint4*>(wn + (size_t)(ky * 3 + kx) * C + c8));
         const __half2* xh = reinterpret_cast<const __half2*>(&xv);
         const __half2* wh = reinterpret_cast<const __half2*>(&wv);
 #pragma unroll
@@ -62,13 +71,19 @@ __global__ void __launch_bounds__(256) dwconv3x3_kernel(const __half* __restrict
 }
 
 cudaError_t launch_dwconv3x3(const __half* x, int N, int IH, int IW, int ICtot, int ic_off, int C, const __half* w, const float* bias, int stride,
-                             int relu, __half* out, int OCtot, int oc_off, cudaStream_t st) {
+                             int relu, __half* out, int OCtot, int oc_off, cudaStream_t st, const WeightGroups* grp) {
   if (C % 8 || ICtot % 8 || ic_off % 8 || OCtot % 8 || oc_off % 8 || (stride != 1 && stride != 2)) return cudaErrorInvalidValue;
+  // 16-byte weight / bias loads in every slot
+  if (grp && (grp->images < 1 || N % grp->images || grp->w_stride % 8 || grp->b_stride % 4)) return cudaErrorInvalidValue;
   const int OH = (IH + 2 - 3) / stride + 1, OW = (IW + 2 - 3) / stride + 1;
   const size_t total = (size_t)N * OH * OW * (C / 8);
   int blocks = (int)((total + 255) / 256);
   if (blocks > 148 * 16) blocks = 148 * 16;
-  return launch_kernel_plain(dwconv3x3_kernel, dim3(blocks), dim3(256), 0, st, x, N, IH, IW, ICtot, ic_off, C, w, bias, stride, relu, out, OH, OW, OCtot, oc_off);
+  if (grp)
+    return launch_kernel_plain(dwconv3x3_kernel<true>, dim3(blocks), dim3(256), 0, st, x, N, IH, IW, ICtot, ic_off, C, w, bias, stride, relu, out, OH, OW,
+                               OCtot, oc_off, *grp);
+  return launch_kernel_plain(dwconv3x3_kernel<false>, dim3(blocks), dim3(256), 0, st, x, N, IH, IW, ICtot, ic_off, C, w, bias, stride, relu, out, OH,
+                             OW, OCtot, oc_off, WeightGroups{});
 }
 
 // ------------------------------------------------------------------------------------------------ bilinear x2, align_corners=True
@@ -118,14 +133,24 @@ cudaError_t launch_upsample_bilinear2x(const __half* x, int N, int H, int W, int
 // ------------------------------------------------------------------------------------------------ LightReal input glue
 // faces u8 [nf,168,168,3] BGR -> [B,160,160,16] fp16: ch 0-2 = centre crop [4:164,4:164] / 255, ch 3-5 = the same with the filled
 // cv2.rectangle((5,5,150,145)) = columns [5,154], rows [5,149] zeroed, ch 6-15 = 0 (K padding of the first 1x1 conv).
+// GRP: image b takes its crop from groups[b / group_images] (faces, nf, first index) instead of (faces, nf, *d_index)
+template <bool GRP>
 __global__ void __launch_bounds__(256) ul_prep_kernel(const uint8_t* __restrict__ faces, int nf, const int* __restrict__ d_index, int B,
-                                                      __half* __restrict__ out) {
+                                                      __half* __restrict__ out, const UlPrepGroup* __restrict__ groups, int group_images) {
   pdl_launch_dependents();   // a PDL-launched successor (the conv kernels) may start its prologue now; it waits before reading
   const int total = B * 160 * 160;
   const int i = blockIdx.x * 256 + threadIdx.x;
   if (i >= total) return;
   const int x = i % 160, y = (i / 160) % 160, b = i / 25600;
-  const int idx = mirror_index_p(nf, *d_index + b);
+  int idx;
+  if constexpr (GRP) {
+    const int g = b / group_images;
+    const UlPrepGroup gd = groups[g];
+    faces = gd.faces;
+    idx = mirror_index_p(gd.nf, gd.index + b - g * group_images);
+  } else {
+    idx = mirror_index_p(nf, *d_index + b);
+  }
   const uint8_t* p = faces + (((size_t)idx * 168 + (y + 4)) * 168 + (x + 4)) * 3;
   const bool masked = (x >= 5 && x <= 154 && y >= 5 && y <= 149);
   uint4 lo = make_uint4(0, 0, 0, 0), hi = make_uint4(0, 0, 0, 0);
@@ -142,7 +167,14 @@ __global__ void __launch_bounds__(256) ul_prep_kernel(const uint8_t* __restrict_
 }
 
 cudaError_t launch_ul_prep(const uint8_t* faces, int nf, const int* d_index, int B, __half* out, cudaStream_t st) {
-  return launch_kernel_plain(ul_prep_kernel, dim3((B * 25600 + 255) / 256), dim3(256), 0, st, faces, nf, d_index, B, out);
+  return launch_kernel_plain(ul_prep_kernel<false>, dim3((B * 25600 + 255) / 256), dim3(256), 0, st, faces, nf, d_index, B, out,
+                             (const UlPrepGroup*)nullptr, 0);
+}
+
+cudaError_t launch_ul_prep_grouped(const UlPrepGroup* groups, int group_images, int B, __half* out, cudaStream_t st) {
+  if (group_images < 1 || B % group_images) return cudaErrorInvalidValue;
+  return launch_kernel_plain(ul_prep_kernel<true>, dim3((B * 25600 + 255) / 256), dim3(256), 0, st, (const uint8_t*)nullptr, 0, (const int*)nullptr,
+                             B, out, groups, group_images);
 }
 
 // ------------------------------------------------------------------------------------------------ LightReal.paste_back_frame

@@ -6,6 +6,7 @@
 //   head        : output_block.1 Conv2d(32,3,1) + Sigmoid (wav2lip_v2.py:90-91) and the "* 255" of
 //                 wav2lip_avatar.py:138, emitting pred in the reference layout (B,256,256,3) f32 BGR.
 #include "ltb_internal.h"
+#include "ops.h"
 
 namespace ltb {
 
@@ -96,10 +97,18 @@ cudaError_t launch_w2l_audio_conv0(const float* mel, const float* w9x32, const f
   return cudaGetLastError();
 }
 
+// GRP: the block's image (hw % 256 == 0, so a block never straddles two) reads the weights of its group's slot
+template <bool GRP>
 __global__ void __launch_bounds__(256) w2l_head_kernel(const __half* __restrict__ x, const float* __restrict__ w,
-                                                       const float* __restrict__ b, float* __restrict__ pred, int npix) {
+                                                       const float* __restrict__ b, float* __restrict__ pred, int npix, int hw,
+                                                       const WeightGroups grp) {
   __shared__ float sw[96];
   __shared__ float sb[3];
+  if constexpr (GRP) {
+    const int s = grp.slot[(int)((size_t)blockIdx.x * 256 / hw) / grp.images];
+    w += s * grp.w_stride;
+    b += s * grp.b_stride;
+  }
   if (threadIdx.x < 96) sw[threadIdx.x] = w[threadIdx.x];
   if (threadIdx.x < 3) sb[threadIdx.x] = b[threadIdx.x];
   __syncthreads();
@@ -130,7 +139,14 @@ __global__ void __launch_bounds__(256) w2l_head_kernel(const __half* __restrict_
 }
 
 cudaError_t launch_w2l_head(const __half* x, const float* w3x32, const float* b3, float* pred, int npix, cudaStream_t st) {
-  w2l_head_kernel<<<(npix + 255) / 256, 256, 0, st>>>(x, w3x32, b3, pred, npix);
+  w2l_head_kernel<false><<<(npix + 255) / 256, 256, 0, st>>>(x, w3x32, b3, pred, npix, 0, WeightGroups{});
+  return cudaGetLastError();
+}
+
+cudaError_t launch_head_grouped(const __half* x, const float* w3x32, const float* b3, float* pred, int npix, int hw, const WeightGroups& grp,
+                                cudaStream_t st) {
+  if (hw <= 0 || hw % 256 || npix % hw || grp.images < 1 || (npix / hw) % grp.images) return cudaErrorInvalidValue;
+  w2l_head_kernel<true><<<(npix + 255) / 256, 256, 0, st>>>(x, w3x32, b3, pred, npix, hw, grp);
   return cudaGetLastError();
 }
 

@@ -12,7 +12,7 @@ from typing import Optional, Sequence
 import numpy as np
 
 from . import _capi
-from ._capi import ConvOp, MtPasteOp, check, lib
+from ._capi import ConvOp, MtPasteOp, UlPrepGroup, check, lib
 
 
 class DevTensor:
@@ -107,6 +107,10 @@ class Ctx:
         self.free(tmp)
         return out
 
+    def d2d(self, dst_ptr: int, src_ptr: int, nbytes: int):
+        """Stream-ordered device-to-device copy."""
+        check(lib().ltb_d2d(self._h, C.c_void_p(dst_ptr), C.c_void_p(src_ptr), int(nbytes)))
+
     def set_i32(self, t: DevTensor, value: int):
         check(lib().ltb_set_i32(self._h, C.c_void_p(t.ptr), int(value)))
 
@@ -147,12 +151,15 @@ class Ctx:
              pad=(0, 0), res: Optional[DevTensor] = None, relu: bool = False, cin: Optional[int] = None, no_halo: bool = False,
              zbatch: int = 0, zdiv: int = 1, in_z=(0, 0), w_z=(0, 0), out_z=(0, 0), w_ptr: Optional[int] = None,
              ktot: Optional[int] = None, cout: Optional[int] = None, in_ptr: Optional[int] = None, out_ptr: Optional[int] = None,
-             gn_stats: Optional[DevTensor] = None, gn_groups: int = 0, gn_hw: int = 0, upsample2x: bool = False):
+             gn_stats: Optional[DevTensor] = None, gn_groups: int = 0, gn_hw: int = 0, upsample2x: bool = False,
+             bias_ptr: Optional[int] = None, group: Optional[tuple] = None):
+        """group = (slot table int32 DevTensor, images per group, slots, w slot stride, bias slot stride): grouped weights
+        (ltb_conv_op.group_slot) read from w_ptr / bias_ptr.  no_halo: False / True, or 2 to require the TMA kernel."""
         d = ConvOp()
         d.in_ = in_ptr if in_ptr is not None else x.ptr
         d.w = w_ptr if w_ptr is not None else w.w.ptr
         d.w_tap = (w.w_tap.ptr if (w is not None and w.w_tap is not None and w_ptr is None) else None)
-        d.bias = (w.bias.ptr if (w is not None and w.bias is not None) else None)
+        d.bias = bias_ptr if bias_ptr is not None else (w.bias.ptr if (w is not None and w.bias is not None) else None)
         d.res = res.ptr if res is not None else None
         d.out = out_ptr if out_ptr is not None else out.ptr
         d.N, d.IH, d.IW = N, IH, IW
@@ -175,6 +182,9 @@ class Ctx:
         d.out_zo, d.out_zi = out_z
         d.gn_stats = gn_stats.ptr if gn_stats is not None else None
         d.gn_groups, d.gn_hw = gn_groups, gn_hw
+        if group is not None:
+            table, d.group_images, d.slots, d.w_slot_stride, d.bias_slot_stride = group
+            d.group_slot = table.ptr
         if upsample2x:          # fused nearest-2x upsample + 3x3 conv: the 16-slice weights of ConvWeight.upconv()
             up = w.upconv(self)
             d.w, d.w_tap, d.Ktot, d.upsample2x = up[0].ptr, up[1].ptr, 16 * w.cin, 1
@@ -221,7 +231,15 @@ class Ctx:
                                      heads, nq, valid, d, scale, C.c_void_p(out.ptr), out.pitch))
 
     # ---- UltraLight / HuBERT ops (SURVEY 8 row f4)
-    def dwconv3x3(self, x: DevTensor, N: int, IH: int, IW: int, w_tap: DevTensor, bias: DevTensor, stride: int, relu: bool, out: DevTensor):
+    def dwconv3x3(self, x: DevTensor, N: int, IH: int, IW: int, w_tap: DevTensor, bias: DevTensor, stride: int, relu: bool, out: DevTensor,
+                  group: Optional[tuple] = None):
+        """group = (slot table int32 DevTensor, images per group, w slot stride, bias slot stride): grouped weights."""
+        if group is not None:
+            table, images, ws, bs = group
+            check(lib().ltb_op_dwconv3x3_grouped(self._h, C.c_void_p(x.ptr), N, IH, IW, x.pitch, x.c_off, x.C, C.c_void_p(w_tap.ptr),
+                                                 C.c_void_p(bias.ptr), stride, int(relu), C.c_void_p(out.ptr), out.pitch, out.c_off,
+                                                 C.c_void_p(table.ptr), images, ws, bs))
+            return
         check(lib().ltb_op_dwconv3x3(self._h, C.c_void_p(x.ptr), N, IH, IW, x.pitch, x.c_off, x.C, C.c_void_p(w_tap.ptr), C.c_void_p(bias.ptr),
                                      stride, int(relu), C.c_void_p(out.ptr), out.pitch, out.c_off))
 
@@ -232,7 +250,18 @@ class Ctx:
     def ul_prep(self, faces_u8: DevTensor, nf: int, d_index: DevTensor, B: int, out: DevTensor):
         check(lib().ltb_op_ul_prep(self._h, C.c_void_p(faces_u8.ptr), nf, C.c_void_p(d_index.ptr), B, C.c_void_p(out.ptr)))
 
-    def head_sigmoid255(self, x: DevTensor, w3x32: DevTensor, b3: DevTensor, npix: int, pred: DevTensor):
+    def ul_prep_grouped(self, groups: DevTensor, group_images: int, B: int, out: DevTensor):
+        """groups: device table of ltb_ul_prep_group (faces pointer, nf, first index) per group (see ul_prep_table)."""
+        check(lib().ltb_op_ul_prep_grouped(self._h, C.c_void_p(groups.ptr), group_images, B, C.c_void_p(out.ptr)))
+
+    def head_sigmoid255(self, x: DevTensor, w3x32: DevTensor, b3: DevTensor, npix: int, pred: DevTensor, group: Optional[tuple] = None,
+                        hw: int = 0):
+        """group = (slot table, images per group, w slot stride, bias slot stride) with hw pixels per image: grouped weights."""
+        if group is not None:
+            table, images, ws, bs = group
+            check(lib().ltb_op_head_sigmoid255_grouped(self._h, C.c_void_p(x.ptr), C.c_void_p(w3x32.ptr), C.c_void_p(b3.ptr), npix,
+                                                       C.c_void_p(pred.ptr), hw, C.c_void_p(table.ptr), images, ws, bs))
+            return
         check(lib().ltb_op_head_sigmoid255(self._h, C.c_void_p(x.ptr), C.c_void_p(w3x32.ptr), C.c_void_p(b3.ptr), npix, C.c_void_p(pred.ptr)))
 
     def ul_paste(self, frames: DevTensor, faces: DevTensor, coords: DevTensor, pred: DevTensor, out: DevTensor, nf: int, H: int, W: int,
@@ -290,6 +319,14 @@ class Ctx:
             self.close()
         except Exception:
             pass
+
+
+def ul_prep_table(groups) -> np.ndarray:
+    """[(faces DevTensor, nf, first index), ...] -> the bytes of an ltb_ul_prep_group table (upload with Ctx.h2d)."""
+    t = (UlPrepGroup * len(groups))()
+    for g, (faces, nf, index) in enumerate(groups):
+        t[g].faces, t[g].nf, t[g].index = faces.ptr, int(nf), int(index)
+    return np.frombuffer(bytes(t), np.uint8)
 
 
 class ConvWeight:

@@ -8,19 +8,25 @@ and the class registered as ``("avatar", "ultralight")``.  ``LightReal`` keeps t
 
 Default (fused) mode: ``inference_batch`` runs prep + U-Net + paste-back on the device and returns B ``EngineFrame`` tokens that
 already hold the composited frames; ``paste_back_frame`` hands the matching one out.  ``opt.ltb_return_pred = True`` restores the
-reference's exact data flow (float32 (B,160,160,3) predictions x 255, pasted per frame from the host)."""
+reference's exact data flow (float32 (B,160,160,3) predictions x 255, pasted per frame from the host).
+
+Cross-session mode (``opt.ltb_cross_session`` / ``LTB_CROSS_SESSION=1``): ``inference_batch`` submits one group request to a shared
+``UltraLightBatchSession`` (``LTB_UL_GROUPS`` sessions per launch, default 4, with a bank of twice as many avatar networks); the
+session keeps its own HuBERT extractor and render threads and only a paste-back context of its own."""
 from __future__ import annotations
 
 import glob
 import os
 import pickle
+import threading
 
 import numpy as np
 
 from .. import engine
 from ..hubert import HubertEncoder, HubertFeatures
 from ..ops import Ctx
-from ..ultralight import FACE, UltraLightAvatar, UltraLightModel, UltraLightSession
+from ..ultralight import FACE, UltraLightAvatar, UltraLightBatchSession, UltraLightModel, UltraLightSession
+from .batcher import CrossSessionBatcher
 from .hubert_asr import HubertASR
 
 try:
@@ -93,6 +99,25 @@ def warm_up(batch_size, avatar, modelres):
     logger.info("warmup model... (engine sessions warm up at creation)")
 
 
+_BATCHER_LOCK = threading.Lock()
+
+
+def shared_batcher(audio: EngineAudio, template: UltraLightModel, frames_per_session: int, return_pred: bool) -> CrossSessionBatcher:
+    """Cross-session mode: one scheduler per (HuBERT model, session batch size), created by the first session that asks.  Its mux is
+    an UltraLightBatchSession of LTB_UL_GROUPS groups whose graph takes its shapes from `template` (every UltraLight network has the
+    same layout) and whose bank holds 2 x groups avatar networks."""
+    with _BATCHER_LOCK:
+        table = getattr(audio, "_ltb_batchers", None)
+        if table is None:
+            table = audio._ltb_batchers = {}
+        key = (int(frames_per_session), bool(return_pred))
+        if key not in table:
+            groups = int(os.environ.get("LTB_UL_GROUPS", "4"))
+            mux = UltraLightBatchSession(template, groups, frames_per_session, slots=2 * groups, return_pred=return_pred)
+            table[key] = CrossSessionBatcher(mux, float(os.environ.get("LTB_MUX_WAIT_MS", "4")))
+        return table[key]
+
+
 @register("avatar", "ultralight")
 class LightReal(BaseAvatar):
     def __init__(self, opt, model, avatar):
@@ -104,15 +129,18 @@ class LightReal(BaseAvatar):
             raise RuntimeError("LightReal needs the payload of livetalking_b200.plugin.ultralight_avatar.load_avatar / make_avatar")
         self._engine_avatar = eng_avatar
         self._return_pred = bool(getattr(opt, "ltb_return_pred", False))
-        # every session owns its stream + scratch (two: U-Net graph, HuBERT graph); weights / avatar assets are shared
-        self.engine_session = UltraLightSession(eng_avatar, self.batch_size)
+        cross = bool(getattr(opt, "ltb_cross_session", False)) or os.environ.get("LTB_CROSS_SESSION", "0") == "1"
+        self._batcher = shared_batcher(audio_processor, eng_avatar.model, self.batch_size, self._return_pred) if cross else None
+        # every session owns its stream + scratch (two: U-Net graph, HuBERT graph); weights / avatar assets are shared.
+        # Cross-session mode: the session keeps only a paste-back context, its U-Net pass runs in the shared batch.
+        self.engine_session = UltraLightSession(eng_avatar, self.batch_size, paste_only=cross)
         self.audio_processor = HubertFeatures(audio_processor.encoder, self.batch_size, opt.l, opt.r)
         self.asr = HubertASR(opt, self, self.audio_processor, audio_feat_length=[4, 4])
         self.asr.warm_up()
         # page-locked output ring for the fused mode (a D2H into pageable memory runs at a few GB/s, pinned at PCIe speed); a buffer is
         # reused after `ring` more batches: res_frame_queue holds at most 2 batches (base_avatar.py:86) + one produced + one pasted
         self._ring, self._ring_pos = [], 0
-        if not self._return_pred:
+        if not self._return_pred and not cross:
             try:
                 shape = (self.batch_size, eng_avatar.H, eng_avatar.W, 3)
                 self._ring = [engine.PinnedBuffer(shape, np.uint8) for _ in range(max(4, int(os.environ.get("LTB_PIN_RING", "4"))))]
@@ -156,6 +184,12 @@ class LightReal(BaseAvatar):
 
     def inference_batch(self, index, audiofeat_batch):
         feats = self._features(audiofeat_batch)
+        if self._batcher is not None:                                                  # one group request of the shared cross-session batch
+            out = self._batcher.submit([(self._engine_avatar, index, feats)])[0]
+            if self._return_pred:
+                return out
+            length = len(self.face_list_cycle)
+            return [EngineFrame(out[i], mirror_index(length, index + i)) for i in range(self.batch_size)]
         if self._return_pred:
             return self.engine_session.infer(index, feats, want_pred=True)          # float32 (B,160,160,3), as the reference
         frames = self.engine_session.infer_paste(index, feats, out=self._next_out())   # (B,H,W,3) uint8: one engine round, one D2H

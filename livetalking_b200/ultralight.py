@@ -6,15 +6,19 @@ The network is MobileNet-style: every InvertedResidual is 1x1 conv -> depthwise 
 (unet.py:7-37).  BatchNorm (eval) is folded into the preceding convolution at load time; the 1x1 convs (97 % of the FLOPs) and the
 two dense stride-2 3x3 convs of the audio branch run on the tcgen05 implicit-GEMM kernels, the depthwise convs / bilinear
 upsampling / input glue / paste-back on the HBM-bound kernels of csrc/ultralight.cu.  ``torch.cat`` never copies: producers write
-straight into channel slices of the concat buffers.  One CUDA graph per (session, batch size)."""
+straight into channel slices of the concat buffers.  One CUDA graph per (session, batch size).
+
+Cross-session batching (``UltraLightBatchSession``): the network belongs to the avatar, so a batch of several sessions runs every
+layer as a *grouped* op — the weights of up to S avatars are stacked slot by slot in an ``UltraLightBank`` and image n of the
+batch reads slot ``group_slot[n // Bs]`` from a device table, so one captured graph serves any assignment of avatars to groups."""
 from __future__ import annotations
 
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
 from .musetalk import Builder, _Replay, _ceil16, _np
-from .ops import ConvWeight, Ctx, DevTensor
+from .ops import ConvWeight, Ctx, DevTensor, ul_prep_table
 
 CH = [32, 64, 128, 256, 512]          # unet.py:188
 FACE, CROP, INSET = 160, 168, 4       # network input side, stored crop side, crop[4:164] (ultralight_avatar.py:148)
@@ -70,51 +74,71 @@ class UltraLightModel:
         self.head_b = ctx.upload(_np(sd["outc.conv.bias"]).astype(np.float32))
         ctx.sync()
 
+    def blocks(self) -> List[_IR]:
+        return [self.a1, self.a2, self.a4, self.a6, self.a7, *self.fuse, self.inc, *(k for d in self.down for k in d),
+                *(k for u in self.up for k in u)]
+
+    def weight_tensors(self) -> List[DevTensor]:
+        """Every device weight tensor the forward reads, in a fixed order (the slot layout of UltraLightBank)."""
+        ts = []
+        for blk in self.blocks():
+            ts += [blk.pw1.w, blk.pw1.bias, blk.dw_w, blk.dw_b, blk.pw2.w, blk.pw2.bias]
+        return ts + [self.a3.w, self.a3.bias, self.a5.w, self.a5.bias, self.head_w, self.head_b]
+
     # ---- emitters (ops go to the builder's ctx = the session's stream; weights are read-only)
     @staticmethod
-    def _ir(b: Builder, blk: _IR, x: DevTensor, out: Optional[DevTensor] = None) -> DevTensor:
+    def _ir(b: Builder, blk: _IR, x: DevTensor, out: Optional[DevTensor] = None, grp: Optional["_Grouping"] = None) -> DevTensor:
         ctx = b.ctx
         N, H, W, _ = x.shape
         rows = N * H * W
         h1 = b.new(N, H, W, blk.hid_p)
-        ctx.conv(x, blk.pw1, h1, N=1, IH=1, IW=rows, OH=1, OW=rows, relu=True)
         OH, OW = (H - 1) // blk.stride + 1, (W - 1) // blk.stride + 1
         h2 = b.new(N, OH, OW, blk.hid_p)
-        ctx.dwconv3x3(h1, N, H, W, blk.dw_w, blk.dw_b, blk.stride, True, h2)
         if out is None:
             out = b.new(N, OH, OW, blk.oup)
         orow = N * OH * OW
-        ctx.conv(h2, blk.pw2, out, N=1, IH=1, IW=orow, OH=1, OW=orow, res=x if blk.res else None)
+        res = x if blk.res else None
+        if grp is None:
+            ctx.conv(x, blk.pw1, h1, N=1, IH=1, IW=rows, OH=1, OW=rows, relu=True)
+            ctx.dwconv3x3(h1, N, H, W, blk.dw_w, blk.dw_b, blk.stride, True, h2)
+            ctx.conv(h2, blk.pw2, out, N=1, IH=1, IW=orow, OH=1, OW=orow, res=res)
+        else:   # grouped: N = images, so that image n maps to group n // Bs
+            ctx.conv(x, blk.pw1, h1, N=N, IH=H, IW=W, OH=H, OW=W, relu=True, **grp.conv(blk.pw1))
+            ctx.dwconv3x3(h1, N, H, W, *grp.dw(blk.dw_w, blk.dw_b), blk.stride, True, h2, group=grp.dw_group(blk.dw_w, blk.dw_b))
+            ctx.conv(h2, blk.pw2, out, N=N, IH=OH, IW=OW, OH=OH, OW=OW, res=res, **grp.conv(blk.pw2))
         return out
 
-    def _dc(self, b: Builder, blks: List[_IR], x: DevTensor, out: Optional[DevTensor] = None) -> DevTensor:
+    def _dc(self, b: Builder, blks: List[_IR], x: DevTensor, out: Optional[DevTensor] = None, grp: Optional["_Grouping"] = None) -> DevTensor:
         for i, blk in enumerate(blks):
-            x = self._ir(b, blk, x, out if i == len(blks) - 1 else None)
+            x = self._ir(b, blk, x, out if i == len(blks) - 1 else None, grp)
         return x
 
-    def emit(self, b: Builder, img16: DevTensor, audio16: DevTensor, pred: DevTensor, taps: Optional[dict] = None):
+    def emit(self, b: Builder, img16: DevTensor, audio16: DevTensor, pred: DevTensor, taps: Optional[dict] = None,
+             grp: Optional["_Grouping"] = None):
         """img16 (B,160,160,16) fp16 NHWC (6 real channels), audio16 (B,32,32,16) -> pred f32 (B,160,160,3) = sigmoid x 255.
-        Model.forward, unet.py:208-226."""
+        Model.forward, unet.py:208-226.  grp: grouped form — every op reads the weights of its image's bank slot (this model only
+        supplies the shapes)."""
         ctx = b.ctx
+        g_conv = (lambda cw: grp.conv(cw)) if grp is not None else (lambda cw: {})   # noqa: E731
         B = img16.shape[0]
         view = lambda buf, c0, c: DevTensor(buf.ptr, buf.shape[:3] + (c,), pitch=buf.shape[3], c_off=c0)  # noqa: E731
         # concat buffers: [upsampled | skip] (torch.cat([x1, x2]), unet.py:88) and [x5 | audio] (unet.py:217)
         cat = [b.new(B, FACE >> i, FACE >> i, 2 * CH[i]) for i in range(4)]                  # up4..up1 inputs at 160, 80, 40, 20
         cat5 = b.new(B, 10, 10, 2 * CH[4])
         skips = [view(cat[i], CH[i], CH[i]) for i in range(4)]                              # x1..x4 live in the second half
-        x = self._ir(b, self.inc, img16, skips[0])
+        x = self._ir(b, self.inc, img16, skips[0], grp)
         for i in range(3):
-            x = self._dc(b, self.down[i], x, skips[i + 1])
-        x5 = self._dc(b, self.down[3], x, view(cat5, 0, CH[4]))
+            x = self._dc(b, self.down[i], x, skips[i + 1], grp)
+        x5 = self._dc(b, self.down[3], x, view(cat5, 0, CH[4]), grp)
         # audio branch, AudioConvHubert.forward (unet.py:164-181)
-        a = self._ir(b, self.a2, self._ir(b, self.a1, audio16))
+        a = self._ir(b, self.a2, self._ir(b, self.a1, audio16, None, grp), None, grp)
         a3 = b.new(B, 16, 16, CH[3])
-        ctx.conv(a, self.a3, a3, N=B, IH=32, IW=32, OH=16, OW=16, stride=(2, 2), pad=(1, 1), relu=True)
-        a4 = self._ir(b, self.a4, a3)
+        ctx.conv(a, self.a3, a3, N=B, IH=32, IW=32, OH=16, OW=16, stride=(2, 2), pad=(1, 1), relu=True, **g_conv(self.a3))
+        a4 = self._ir(b, self.a4, a3, None, grp)
         a5 = b.new(B, 10, 10, CH[4])
-        ctx.conv(a4, self.a5, a5, N=B, IH=16, IW=16, OH=10, OW=10, stride=(2, 2), pad=(3, 3), relu=True)
-        af = self._ir(b, self.a7, self._ir(b, self.a6, a5), view(cat5, CH[4], CH[4]))
-        f = self._dc(b, self.fuse, cat5)
+        ctx.conv(a4, self.a5, a5, N=B, IH=16, IW=16, OH=10, OW=10, stride=(2, 2), pad=(3, 3), relu=True, **g_conv(self.a5))
+        af = self._ir(b, self.a7, self._ir(b, self.a6, a5, None, grp), view(cat5, CH[4], CH[4]), grp)
+        f = self._dc(b, self.fuse, cat5, None, grp)
         if taps is not None:
             taps.update(x5=x5, audio=af, fuse=f)
         # Up.forward x 4 (unet.py:81-90): sizes are exact doubles, so the F.pad is a no-op
@@ -122,10 +146,14 @@ class UltraLightModel:
             lvl = 3 - i
             H = FACE >> (lvl + 1)
             ctx.upsample_bilinear2x(f, B, H, H, view(cat[lvl], 0, CH[lvl]))
-            f = self._dc(b, self.up[i], cat[lvl])
+            f = self._dc(b, self.up[i], cat[lvl], None, grp)
             if taps is not None:
                 taps[f"u{i + 1}"] = f
-        ctx.head_sigmoid255(f, self.head_w, self.head_b, B * FACE * FACE, pred)
+        if grp is None:
+            ctx.head_sigmoid255(f, self.head_w, self.head_b, B * FACE * FACE, pred)
+        else:
+            ctx.head_sigmoid255(f, *grp.dw(self.head_w, self.head_b), B * FACE * FACE, pred, group=grp.dw_group(self.head_w, self.head_b),
+                                hw=FACE * FACE)
         return pred
 
 
@@ -147,12 +175,81 @@ class UltraLightAvatar:
         self.frames, self.faces, self.coords = ctx.upload(frames), ctx.upload(faces), ctx.upload(self.coords_host)
 
 
+class UltraLightBank:
+    """The weights of up to ``slots`` UltraLight networks, stacked slot by slot: one device buffer (slots, *shape) per weight tensor
+    of ``UltraLightModel.weight_tensors()``.  ``slot_of(model)`` loads a network on a miss (stream-ordered device-to-device copies from
+    its resident weights) into a free slot or the least recently used one.  Used by one dispatcher thread only: no lock."""
+
+    def __init__(self, ctx: Ctx, template: UltraLightModel, slots: int):
+        self.ctx, self.slots = ctx, int(slots)
+        if self.slots < 1:
+            raise ValueError("UltraLightBank needs at least one slot")
+        ts = template.weight_tensors()
+        self._layout = [(t.shape, t.dtype) for t in ts]
+        self._index = {id(t): i for i, t in enumerate(ts)}
+        self._bufs = [ctx.alloc((self.slots,) + t.shape, t.dtype, zero=True) for t in ts]
+        self.nbytes = sum(b.nbytes for b in self._bufs)
+        self._model: List[Optional[UltraLightModel]] = [None] * self.slots
+        self._used = [0] * self.slots                   # tick of the last slot_of() that returned the slot; 0 = never
+        self._tick = 0
+        self.loads = 0
+
+    def stacked(self, t: DevTensor) -> DevTensor:
+        """The bank buffer (slots, *t.shape) of the template tensor t."""
+        return self._bufs[self._index[id(t)]]
+
+    def slot_of(self, model: UltraLightModel, keep: Sequence[int] = ()) -> int:
+        """Slot holding `model`'s weights; on a miss the network is loaded into an empty slot or, failing that, the least recently
+        used slot not listed in `keep` (the slots the current batch already uses)."""
+        self._tick += 1
+        for s, m in enumerate(self._model):
+            if m is model:
+                self._used[s] = self._tick
+                return s
+        free = [s for s in range(self.slots) if s not in keep]
+        if not free:
+            raise RuntimeError(f"UltraLightBank: all {self.slots} slots are in use by this batch")
+        s = min(free, key=lambda k: self._used[k])
+        ts = model.weight_tensors()
+        if [(t.shape, t.dtype) for t in ts] != self._layout:
+            raise ValueError("UltraLightBank: the network's weight shapes differ from the bank's")
+        for t, buf in zip(ts, self._bufs):
+            self.ctx.d2d(buf.ptr + s * t.nbytes, t.ptr, t.nbytes)
+        self._model[s], self._used[s] = model, self._tick
+        self.loads += 1
+        return s
+
+
+class _Grouping:
+    """Arguments of the grouped ops: weights from `bank`, image n uses slot table[n // images]."""
+
+    def __init__(self, bank: UltraLightBank, table: DevTensor, images: int):
+        self.bank, self.table, self.images = bank, table, int(images)
+
+    def conv(self, cw: ConvWeight) -> dict:
+        w, b = self.bank.stacked(cw.w), self.bank.stacked(cw.bias)
+        return dict(w_ptr=w.ptr, bias_ptr=b.ptr, group=(self.table, self.images, self.bank.slots, cw.cout * cw.ktot, cw.cout))
+
+    def dw(self, w: DevTensor, b: DevTensor):
+        return self.bank.stacked(w), self.bank.stacked(b)
+
+    def dw_group(self, w: DevTensor, b: DevTensor) -> tuple:
+        return (self.table, self.images, int(np.prod(w.shape)), int(np.prod(b.shape)))
+
+
 class UltraLightSession:
     """One avatar stream at a fixed batch size: captured prep + U-Net + head graph, paste-back buffers."""
 
-    def __init__(self, avatar: UltraLightAvatar, batch: int, keep_taps: bool = False, ctx: Optional[Ctx] = None):
+    def __init__(self, avatar: UltraLightAvatar, batch: int, keep_taps: bool = False, ctx: Optional[Ctx] = None, paste_only: bool = False):
+        """paste_only: no network graph and no activation arena — only paste_pred() works (cross-session mode: this session's
+        U-Net pass runs in a shared UltraLightBatchSession)."""
         self.avatar, self.B = avatar, int(batch)
         self._own_ctx = ctx is None
+        self._paste_ctx = None
+        self.graph = None
+        if paste_only:
+            self.ctx, self._own_ctx = None, False
+            return
         ctx = self.ctx = Ctx() if ctx is None else ctx
         B = self.B
         self.builder = Builder(ctx)
@@ -179,6 +276,8 @@ class UltraLightSession:
     # ---- LightReal.inference_batch (ultralight_avatar.py:141-169)
     def infer_async(self, index: int, audio_feats: Optional[np.ndarray] = None):
         """audio_feats: (B, 16, 1024) float (the HubertASR windows) or None when audio16 is already resident."""
+        if self.graph is None:
+            raise RuntimeError("UltraLightSession: paste-only (or closed) session has no network graph")
         if audio_feats is not None:
             a = np.asarray(audio_feats, np.float32)
             if a.shape != (self.B, 16, 1024):
@@ -241,6 +340,129 @@ class UltraLightSession:
         if self._paste_ctx is not None:
             self._paste_ctx.close()
             self._paste_ctx = None
+        if self._own_ctx and self.ctx is not None:
+            self.ctx.close()
+        self.ctx = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class UltraLightBatchSession:
+    """Cross-session batching for UltraLight: up to G sessions x Bs frames run as ONE captured prep + U-Net + head graph of batch
+    G*Bs.  A *group request* is (UltraLightAvatar, first frame index, HuBERT features (Bs, 16, 1024) or None = resident).  Each
+    avatar brings its own network: the graph's ops are grouped, group g reads the weights of bank slot group_slot[g] and its crops
+    from its own avatar (a per-group prep descriptor), both device tables written before every launch.  Groups beyond the
+    requests of a call keep their last slot and a blank crop source; their output is discarded.  `batch` / `infer_slots` make it a
+    mux for plugin.batcher.CrossSessionBatcher; infer_groups returns composited frames, or float32 predictions with return_pred."""
+
+    def __init__(self, template: UltraLightModel, groups: int, frames_per_session: int, slots: Optional[int] = None,
+                 return_pred: bool = False, ctx: Optional[Ctx] = None):
+        self.G, self.Bs, self.return_pred = int(groups), int(frames_per_session), bool(return_pred)
+        self.batch = self.G                                  # CrossSessionBatcher: requests per engine call
+        self.B = B = self.G * self.Bs
+        self._own_ctx = ctx is None
+        ctx = self.ctx = Ctx() if ctx is None else ctx
+        self.bank = UltraLightBank(ctx, template, slots if slots is not None else 2 * self.G)
+        if self.bank.slots < self.G:
+            raise ValueError(f"the bank needs at least {self.G} slots")
+        self.builder = Builder(ctx)
+        self.d_slot = ctx.alloc((self.G,), np.int32, zero=True)
+        self._slot_host = np.zeros(self.G, np.int32)
+        self._blank = ctx.alloc((1, CROP, CROP, 3), np.uint8, zero=True)      # crop source of the groups a call leaves empty
+        self._prep = [(self._blank, 1, 0)] * self.G
+        self.d_prep = ctx.upload(ul_prep_table(self._prep))
+        self.audio16 = ctx.alloc((B, 32, 32, 16), np.float16, zero=True)
+        self.img16 = ctx.alloc((B, FACE, FACE, 16), np.float16, zero=True)
+        self.pred = ctx.alloc((B, FACE, FACE, 3), np.float32, zero=True)
+        self._audio_host = np.zeros((B, 1024, 16), np.float16)
+        self._frames_out: Dict[tuple, DevTensor] = {}
+        grp = _Grouping(self.bank, self.d_slot, self.Bs)
+
+        def emit():
+            ctx.ul_prep_grouped(self.d_prep, self.Bs, B, self.img16)
+            template.emit(self.builder, self.img16, self.audio16, self.pred, None, grp)
+
+        emit()
+        ctx.sync()
+        temps, self.builder.temps = self.builder.temps, []
+        self.builder.new = _Replay(temps)
+        with ctx.capture() as cap:
+            emit()
+        self.graph = cap.graph
+
+    def _check(self, requests):
+        if not 1 <= len(requests) <= self.G:
+            raise ValueError(f"1..{self.G} group requests per call, got {len(requests)}")
+
+    def infer_async(self, requests: Sequence[tuple]):
+        """requests[g] = (UltraLightAvatar, first frame index, features (Bs,16,1024) | None = resident in audio16 rows of group g)."""
+        self._check(requests)
+        ctx, Bs = self.ctx, self.Bs
+        keep: List[int] = []
+        stage = False
+        for g, (av, index, feats) in enumerate(requests):
+            s = self.bank.slot_of(av.model, keep)
+            keep.append(s)
+            self._slot_host[g] = s
+            self._prep[g] = (av.faces, av.n, int(index))
+            if feats is not None:
+                a = np.asarray(feats, np.float32)
+                if a.shape != (Bs, 16, 1024):
+                    raise ValueError(f"group features must be ({Bs},16,1024), got {a.shape}")
+                self._audio_host[g * Bs:(g + 1) * Bs] = a.transpose(0, 2, 1)
+                stage = True
+        for g in range(len(requests), self.G):
+            self._prep[g] = (self._blank, 1, 0)
+        ctx.h2d(self.d_slot, self._slot_host, sync=False)
+        ctx.h2d(self.d_prep, ul_prep_table(self._prep), sync=False)
+        if stage:
+            n = len(requests) * Bs
+            ctx.h2d(self.audio16, self._audio_host[:n], sync=False)
+        self.graph.launch()
+
+    def _out(self, g: int, av: UltraLightAvatar) -> DevTensor:
+        key = (g, av.H, av.W)
+        if key not in self._frames_out:
+            self._frames_out[key] = self.ctx.alloc((self.Bs, av.H, av.W, 3), np.uint8, zero=True)
+        return self._frames_out[key]
+
+    def paste_async(self, requests: Sequence[tuple]) -> List[DevTensor]:
+        """Paste-back of every group's predictions into its own avatar's frames (LightReal.paste_back_frame x Bs per group)."""
+        self._check(requests)
+        outs = []
+        for g, (av, index, _f) in enumerate(requests):
+            out = self._out(g, av)
+            self.ctx.ul_paste(av.frames, av.faces, av.coords, self.pred, out, av.n, av.H, av.W, int(index), -1, g * self.Bs, self.Bs)
+            outs.append(out)
+        return outs
+
+    def step_async(self, requests: Sequence[tuple]):
+        self.infer_async(requests)
+        self.paste_async(requests)
+
+    def infer_groups(self, requests: Sequence[tuple]) -> List[np.ndarray]:
+        """-> per request its (Bs, H, W, 3) uint8 composited frames, or with return_pred its float32 (Bs, 160, 160, 3) predictions
+        (what LightReal.inference_batch returns for that session)."""
+        with self.ctx.lock:
+            self.infer_async(requests)
+            if self.return_pred:
+                n = len(requests) * self.Bs
+                pred = self.ctx.download(DevTensor(self.pred.ptr, (n, FACE, FACE, 3), np.float32))
+                return [pred[g * self.Bs:(g + 1) * self.Bs] for g in range(len(requests))]
+            outs = [self.ctx.download(t, sync=False) for t in self.paste_async(requests)]
+            self.ctx.sync()
+            return outs
+
+    infer_slots = infer_groups
+
+    def close(self):
+        if getattr(self, "graph", None) is not None:
+            self.graph.close()
+            self.graph = None
         if self._own_ctx and self.ctx is not None:
             self.ctx.close()
         self.ctx = None
