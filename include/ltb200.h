@@ -214,8 +214,22 @@ typedef struct ltb_conv_op {
   const int* group_slot;
   int group_images, slots;
   long long w_slot_stride, bias_slot_stride;
+  /* 1: ConvTranspose2d(k3, s2, p1, output_padding 1) as four sub-pixel phases over the input grid: KH = KW = 3, OH = 2*IH,
+   * OW = 2*IW, Ktot = 9*Cin (stride and padding fields are not read).  Each weight row holds the taps of phase (0,0), (0,1),
+   * (1,0), (1,1) in turn (the packing of ltb_conv2d_f16); `w_tap`, if given, the same nine [Cout][Cin] slices of `w` in the
+   * order 0, 1, 5, 2, 6, 8, 7, 4, 3 for the TMA kernel. */
+  int transposed;
 } ltb_conv_op;
 int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d);
+/* test hook (like ltb_conv2d_f16): the kernel instance ltb_op_conv2d would run for *d on this device, found by the same
+ * argument checks and planning; nothing is launched.  kernel: 0 = cp.async gather kernel conv_gather_wgmma_kernel<bn, kb,
+ * grouped>, 1 = TMA kernel conv_halo_wgmma_kernel<bn, nsub, nacc, taps, resident_chunks, grouped> (taps: 9 = 3x3 / ConvT,
+ * 10 = stride-2 parity planes, 16 = fused upsample, 1 = GEMM mode).  ksplit > 1: the gather kernel splits K that many ways
+ * and a finalize kernel sums the slices.  Fields that do not apply to the kernel are 0. */
+typedef struct ltb_conv_variant {
+  int kernel, taps, bn, nsub, nacc, resident_chunks, kb, ksplit, grouped;
+} ltb_conv_variant;
+int ltb_op_conv2d_plan(ltb_ctx* c, const ltb_conv_op* d, ltb_conv_variant* out);
 int ltb_op_w_tap_major(ltb_ctx* c, const void* w, void* wt, int cout, int cin);
 /* torch.nn.GroupNorm (+ optional SiLU) on an NHWC channel slice; fp32 statistics */
 int ltb_op_groupnorm(ltb_ctx* c, const void* x, int N, int HW, int C, int Ctot, int c_off, int groups, float eps, const float* gamma,

@@ -28,7 +28,11 @@ class ConvOp(C.Structure):
                 [(n, C.c_longlong) for n in ("in_zo", "in_zi", "w_zo", "w_zi", "out_zo", "out_zi")] +
                 [("gn_stats", C.c_void_p), ("gn_groups", C.c_int), ("gn_hw", C.c_int), ("upsample2x", C.c_int)] +
                 [("group_slot", C.c_void_p), ("group_images", C.c_int), ("slots", C.c_int), ("w_slot_stride", C.c_longlong),
-                 ("bias_slot_stride", C.c_longlong)])
+                 ("bias_slot_stride", C.c_longlong), ("transposed", C.c_int)])
+
+
+class ConvVariant(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ("kernel", "taps", "bn", "nsub", "nacc", "resident_chunks", "kb", "ksplit", "grouped")]
 
 
 class UlPrepGroup(C.Structure):
@@ -102,6 +106,7 @@ _SIGS = {
     "ltb_graph_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
     "ltb_graph_destroy": (C.c_int, [C.c_void_p]),
     "ltb_op_conv2d": (C.c_int, [C.c_void_p, C.POINTER(ConvOp)]),
+    "ltb_op_conv2d_plan": (C.c_int, [C.c_void_p, C.POINTER(ConvOp), C.POINTER(ConvVariant)]),
     "ltb_op_w_tap_major": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "ltb_op_groupnorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                    C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int]),

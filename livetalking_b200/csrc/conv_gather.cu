@@ -283,22 +283,20 @@ __global__ void __launch_bounds__(256) splitk_finalize_kernel(const float* __res
   }
 }
 
-cudaError_t launch_conv_gather(const ConvParams& p_in, cudaStream_t st, float* splitk_ws, size_t splitk_ws_floats) {
-  ConvParams p = p_in;
+bool conv_gather_pick(const ConvParams& p, bool have_ws, size_t splitk_ws_floats, int* bn_out, int* kb_out, int* ksplit_out) {
   if (p.Cout % 16 != 0 || p.Cin % 16 != 0 || (p.ICtot % 8) || (p.OCtot % 8) || (p.ic_off % 8) || (p.oc_off % 8) ||
       (p.Ktot % 8) || p.nphases < 1 || p.nphases > kMaxPhases)
-    return cudaErrorInvalidValue;
-  if (p.res && ((p.RCtot % 8) || (p.rc_off % 8))) return cudaErrorInvalidValue;
+    return false;
+  if (p.res && ((p.RCtot % 8) || (p.rc_off % 8))) return false;
   int bn = conv_gather_pick_bn(p);
-  if (!bn) return cudaErrorInvalidValue;
+  if (!bn) return false;
   const int kb = (p.Cin % 64 == 0) ? 64 : (p.Cin % 32 == 0) ? 32 : 16;
   // split-K for small-M, deep-K layers (1x1..8x8 maps with 512..2560 channels): they are weight-streaming bound and a
   // handful of CTAs walking thousands of K blocks serially is latency-bound.
-  p.ksplit = 0;
-  p.ws = nullptr;
+  int ksplit = 0;
   const int kiters = p.ph[0].ntaps * (p.Cin / kb);
   const long mt = (p.M + 127) / 128;
-  if (splitk_ws && !p.group_slot && p.nphases == 1 && p.zbatch <= 1 && p.osy == 1 && p.osx == 1 && p.GH == p.OH && p.GW == p.OW && kiters >= 32 && mt <= 8) {
+  if (have_ws && !p.group_slot && p.nphases == 1 && p.zbatch <= 1 && p.osy == 1 && p.osx == 1 && p.GH == p.OH && p.GW == p.OW && kiters >= 32 && mt <= 8) {
     int bn2 = 0;
     for (int c : {128, 64, 32, 16})
       if (p.Cout % c == 0) {
@@ -313,13 +311,22 @@ cudaError_t launch_conv_gather(const ConvParams& p_in, cudaStream_t st, float* s
       while (ks >= 2 && (size_t)ks * p.M * p.Cout > splitk_ws_floats) --ks;
       if (ks >= 2) {
         const int per = (kiters + ks - 1) / ks;
-        ks = (kiters + per - 1) / per;  // no empty splits
-        p.ksplit = ks;
-        p.ws = splitk_ws;
+        ksplit = (kiters + per - 1) / per;  // no empty splits
         bn = bn2;
       }
     }
   }
+  *bn_out = bn;
+  *kb_out = kb;
+  *ksplit_out = ksplit;
+  return true;
+}
+
+cudaError_t launch_conv_gather(const ConvParams& p_in, cudaStream_t st, float* splitk_ws, size_t splitk_ws_floats) {
+  ConvParams p = p_in;
+  int bn, kb;
+  if (!conv_gather_pick(p, splitk_ws != nullptr, splitk_ws_floats, &bn, &kb, &p.ksplit)) return cudaErrorInvalidValue;
+  p.ws = p.ksplit > 1 ? splitk_ws : nullptr;
   cudaError_t e;
   if (kb == 64) e = launch_kb<64>(p, bn, st);
   else if (kb == 32) e = launch_kb<32>(p, bn, st);

@@ -743,7 +743,7 @@ static cudaError_t launch_cfg(const HaloPlan& pl, int sms, cudaStream_t st) {
   return launch_kernel_pdl(conv_halo_wgmma_kernel<BN, NSUB, NACC, TAPS, RC, GRP>, dim3(grid), dim3(kHaloThreads), C::SMEM_BYTES, st, pl.hp);
 }
 
-cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
+int conv_halo_sms() {
   static std::atomic<int> sms_cached{0};
   int sms = sms_cached.load();
   if (!sms) {
@@ -753,6 +753,22 @@ cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
     if (sms <= 0) sms = kSms;
     sms_cached.store(sms);
   }
+  return sms;
+}
+
+// weights-resident variants: 3x3 / ConvT layers with a single N tile, at least two tiles per SM and one or two K chunks of
+// weights (the variants that fit next to the halo ring)
+int conv_halo_resident_chunks(const HaloPlan& pl, int sms) {
+  if (pl.TAPS != 9 || pl.hp.tiles_n != 1 || pl.hp.total_tiles < 2 * sms) return 0;
+  const int key = pl.BN * 100 + pl.NSUB * 10 + pl.NACC;
+  const int chunks = (pl.hp.Cin + 63) / 64;
+  if (chunks == 1 && (key == 6421 || key == 3221 || key == 6414 || key == 3214)) return 1;
+  if (chunks == 2 && (key == 3221 || key == 6414 || key == 3214)) return 2;
+  return 0;
+}
+
+cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
+  const int sms = conv_halo_sms();
   if (pl.TAPS == 10) {
     if (pl.NSUB != 1 || pl.NACC != 1) return cudaErrorInvalidValue;
     return pl.BN == 64 ? launch_cfg<64, 1, 1, 10>(pl, sms, st) : (pl.BN == 32 ? launch_cfg<32, 1, 1, 10>(pl, sms, st) : cudaErrorInvalidValue);
@@ -780,14 +796,14 @@ cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
     return cudaErrorInvalidValue;
   }
   // weights-resident variants (single N tile, whole weight set in shared memory)
-  if (pl.hp.tiles_n == 1 && pl.hp.total_tiles >= 2 * sms) {
-    const int chunks = (pl.hp.Cin + 63) / 64;
-    if (key == 6421 && chunks == 1) return launch_cfg<64, 2, 1, 9, 1>(pl, sms, st);
-    if (key == 3221 && chunks == 1) return launch_cfg<32, 2, 1, 9, 1>(pl, sms, st);
-    if (key == 3221 && chunks == 2) return launch_cfg<32, 2, 1, 9, 2>(pl, sms, st);
-    if (key == 6414 && chunks == 2) return launch_cfg<64, 1, 4, 9, 2>(pl, sms, st);
-    if (key == 6414 && chunks == 1) return launch_cfg<64, 1, 4, 9, 1>(pl, sms, st);
-    if (key == 3214 && chunks <= 2) return chunks == 1 ? launch_cfg<32, 1, 4, 9, 1>(pl, sms, st) : launch_cfg<32, 1, 4, 9, 2>(pl, sms, st);
+  switch (conv_halo_resident_chunks(pl, sms) * 100000 + key) {
+    case 106421: return launch_cfg<64, 2, 1, 9, 1>(pl, sms, st);
+    case 103221: return launch_cfg<32, 2, 1, 9, 1>(pl, sms, st);
+    case 203221: return launch_cfg<32, 2, 1, 9, 2>(pl, sms, st);
+    case 206414: return launch_cfg<64, 1, 4, 9, 2>(pl, sms, st);
+    case 106414: return launch_cfg<64, 1, 4, 9, 1>(pl, sms, st);
+    case 103214: return launch_cfg<32, 1, 4, 9, 1>(pl, sms, st);
+    case 203214: return launch_cfg<32, 1, 4, 9, 2>(pl, sms, st);
   }
   switch (key) {
     case 12821: return launch_cfg<128, 2, 1>(pl, sms, st);

@@ -55,6 +55,10 @@ bool conv_halo_supported(const ConvParams& p);
 // w_tap_major: device pointer to the [9][Cout][Cin] copy of the layer's weights (unused in GEMM mode). returns 0 on success.
 int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan* out);
 cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st);
+// SM count of the current device (read once), the width of the persistent grid launch_conv_halo sizes
+int conv_halo_sms();
+// K chunks of weights the variant launch_conv_halo runs for pl on `sms` SMs keeps resident (template argument RC); 0: streamed
+int conv_halo_resident_chunks(const HaloPlan& pl, int sms);
 bool conv_halo_gn_fusable(const HaloPlan& pl, int cout_total, int groups, int hw);
 cudaError_t launch_w_tap_major(const __half* w, __half* wt, int cout, int cin, cudaStream_t st, int ntaps = 9);
 // ConvT(k3,s2) weights: phase-major rows [Cout][9][Cin] (pack order of w2l_pack.py / pack_convT_w) -> the view-major slice

@@ -111,6 +111,24 @@ cudaError_t conv_launch(const ConvPlan& pl, cudaStream_t st, float* splitk_ws, s
   return pl.halo ? launch_conv_halo(pl.hp, st) : launch_conv_gather(pl.p, st, splitk_ws, ws_floats);
 }
 
+bool conv_plan_variant(const ConvPlan& pl, bool have_ws, size_t ws_floats, ltb_conv_variant* out) {
+  std::memset(out, 0, sizeof(*out));
+  out->grouped = pl.p.group_slot != nullptr;
+  if (pl.halo) {
+    out->kernel = 1;
+    out->taps = pl.hp.TAPS;
+    out->bn = pl.hp.BN;
+    out->nsub = pl.hp.NSUB;
+    out->nacc = pl.hp.NACC;
+    out->resident_chunks = conv_halo_resident_chunks(pl.hp, conv_halo_sms());
+    return true;
+  }
+  int ksplit = 0;
+  if (!conv_gather_pick(pl.p, have_ws, ws_floats, &out->bn, &out->kb, &ksplit)) return false;
+  out->ksplit = ksplit > 1 ? ksplit : 1;
+  return true;
+}
+
 bool conv_plan_fuse_gn_stats(ConvPlan* pl, float* stats, int groups, int hw) {
   const ConvParams& p = pl->p;
   if (!pl->halo || pl->hp.grouped || p.oc_off != 0 || p.OCtot != p.Cout || !conv_halo_gn_fusable(pl->hp, p.Cout, groups, hw)) return false;

@@ -5,6 +5,8 @@
 
 #include "conv_halo.h"
 
+struct ltb_conv_variant;   // include/ltb200.h
+
 namespace ltb {
 
 // channels [off, off + C) of an NHWC fp16 tensor whose pixels are Ctot elements apart
@@ -45,6 +47,8 @@ struct ConvPlan {
 int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan* out);
 // splitk_ws: zero-initialised fp32 workspace of ws_floats floats for the gather kernel's split-K (one per stream)
 cudaError_t conv_launch(const ConvPlan& pl, cudaStream_t st, float* splitk_ws, size_t ws_floats);
+// the kernel instance conv_launch runs for pl with (have_ws) or without a split-K workspace; false if no instance can run it
+bool conv_plan_variant(const ConvPlan& pl, bool have_ws, size_t ws_floats, ltb_conv_variant* out);
 
 // Epilogue fusions; each returns false, leaving the plan unchanged, when the plan cannot take it.
 // GroupNorm statistics (sum, sum of squares per (image, group)) of the output, hw pixels per image: `stats` must be zeroed

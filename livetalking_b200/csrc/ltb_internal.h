@@ -90,6 +90,9 @@ struct SlotDesc {
 // ---- kernel launchers ----
 // splitk_ws: optional zero-initialised fp32 workspace (one per stream) enabling split-K for small-M deep-K layers
 cudaError_t launch_conv_gather(const ConvParams& p, cudaStream_t st, float* splitk_ws = nullptr, size_t splitk_ws_floats = 0);
+// the variant launch_conv_gather runs for p (have_ws: a split-K workspace of splitk_ws_floats floats is passed): N tile width,
+// K chunk width and split-K factor (0: none); false if the kernel cannot run p
+bool conv_gather_pick(const ConvParams& p, bool have_ws, size_t splitk_ws_floats, int* bn, int* kb, int* ksplit);
 
 // wav2lip-specific small kernels (w2l_small.cu)
 // faces u8 [nf,256,256,3] BGR -> padded fp16 [B,262,264,8]: ch0-2 = face/255 with rows >= 128 zeroed, ch3-5 = face/255

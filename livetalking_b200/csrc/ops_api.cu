@@ -193,17 +193,23 @@ int ltb_graph_destroy(ltb_graph* g) {
   return 0;
 }
 
+}  // extern "C"
+
 // ---- ops ----------------------------------------------------------------------------------------
-int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d) {
-  if (!c || !d || !d->in || !d->w || !d->out) return LTB_FAIL("conv2d: null argument");
-  LTB_CTX_ENTER(c);
+
+// argument checks and planning of ltb_op_conv2d, shared with ltb_op_conv2d_plan.  Returns 0, or 1 with the reason set.
+static int conv2d_plan(ltb_ctx* c, const ltb_conv_op* d, ConvPlan* pl) {
+  if (!d->in || !d->w || !d->out) return LTB_FAIL("conv2d: null argument");
   if (d->KH * d->KW > kMaxTaps) return LTB_FAIL("conv2d: kernel too large");
-  pdl_set_enabled(pdl_default());   // the calling thread may have run a w2l profiling pass with PDL off
   if (d->Cout > kZeroBias && !d->bias) return LTB_FAIL("conv2d: Cout too large for the implicit zero bias");
   if (d->upsample2x && (d->KH != 3 || d->KW != 3 || d->sy != 1 || d->sx != 1 || d->pad_t != 1 || d->pad_l != 1 || d->OH != 2 * d->IH ||
                         d->OW != 2 * d->IW || d->Ktot != 16 * d->Cin || !d->w_tap || d->zbatch > 1))
     return LTB_FAIL("conv2d: upsample2x needs a 3x3 s1 p1 conv, OH = 2*IH, OW = 2*IW and the 16-slice weights");
-  ConvParams p = conv_params(d->upsample2x ? ConvMode::Upsample2x : ConvMode::Dense, d->N,
+  if (d->transposed && (d->upsample2x || d->KH != 3 || d->KW != 3 || d->OH != 2 * d->IH || d->OW != 2 * d->IW || d->Ktot != 9 * d->Cin ||
+                        d->zbatch > 1))
+    return LTB_FAIL("conv2d: transposed needs a 3x3 kernel, OH = 2*IH, OW = 2*IW, Ktot = 9*Cin and no upsample2x or zbatch");
+  const ConvMode mode = d->upsample2x ? ConvMode::Upsample2x : d->transposed ? ConvMode::Transposed : ConvMode::Dense;
+  ConvParams p = conv_params(mode, d->N,
                              {static_cast<const __half*>(d->in), d->ICtot, d->ic_off}, d->IH, d->IW, d->Cin,
                              {static_cast<const __half*>(d->out), d->OCtot, d->oc_off}, d->OH, d->OW, d->Cout,
                              {static_cast<const __half*>(d->res), d->RCtot, d->rc_off}, static_cast<const __half*>(d->w), d->Ktot,
@@ -226,8 +232,18 @@ int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d) {
   }
   // the fused upsample exists on the halo kernel only
   const ConvPath path = d->upsample2x ? ConvPath::Halo : d->no_halo == 1 ? ConvPath::Gather : d->no_halo == 2 ? ConvPath::Halo : ConvPath::Auto;
+  return conv_plan(p, static_cast<const __half*>(d->w_tap), path, pl);
+}
+
+extern "C" {
+
+int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d) {
+  if (!c || !d) return LTB_FAIL("conv2d: null argument");
+  LTB_CTX_ENTER(c);
   ConvPlan pl;
-  if (conv_plan(p, static_cast<const __half*>(d->w_tap), path, &pl)) return 1;
+  if (conv2d_plan(c, d, &pl)) return 1;
+  pdl_set_enabled(pdl_default());   // the calling thread may have run a w2l profiling pass with PDL off
+  const ConvParams& p = pl.p;
   const bool want_stats = d->gn_stats != nullptr && d->gn_groups > 0 && d->gn_hw > 0 && (p.M % d->gn_hw) == 0 && d->zbatch <= 1;
   float* stats = static_cast<float*>(d->gn_stats);
   const bool stats_fused = want_stats && conv_plan_fuse_gn_stats(&pl, stats, d->gn_groups, d->gn_hw);
@@ -242,6 +258,15 @@ int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d) {
     if (e != cudaSuccess) return LTB_FAIL(std::string("conv2d gn_stats: ") + cudaGetErrorString(e));
     c->launches += 1;
   }
+  return 0;
+}
+
+int ltb_op_conv2d_plan(ltb_ctx* c, const ltb_conv_op* d, ltb_conv_variant* out) {
+  if (!c || !d || !out) return LTB_FAIL("conv2d_plan: null argument");
+  LTB_CTX_ENTER(c);
+  ConvPlan pl;
+  if (conv2d_plan(c, d, &pl)) return 1;
+  if (!conv_plan_variant(pl, c->splitk_ws != nullptr, kSplitKWsFloats, out)) return LTB_FAIL("conv2d_plan: no kernel instance runs this geometry");
   return 0;
 }
 

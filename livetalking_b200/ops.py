@@ -147,14 +147,25 @@ class Ctx:
         holder.graph = Graph(self, h)
 
     # ---- ops
-    def conv(self, x: DevTensor, w: "ConvWeight", out: DevTensor, *, N: int, IH: int, IW: int, OH: int, OW: int, stride=(1, 1),
-             pad=(0, 0), res: Optional[DevTensor] = None, relu: bool = False, cin: Optional[int] = None, no_halo: bool = False,
-             zbatch: int = 0, zdiv: int = 1, in_z=(0, 0), w_z=(0, 0), out_z=(0, 0), w_ptr: Optional[int] = None,
-             ktot: Optional[int] = None, cout: Optional[int] = None, in_ptr: Optional[int] = None, out_ptr: Optional[int] = None,
-             gn_stats: Optional[DevTensor] = None, gn_groups: int = 0, gn_hw: int = 0, upsample2x: bool = False,
-             bias_ptr: Optional[int] = None, group: Optional[tuple] = None):
+    def conv(self, x: DevTensor, w: "ConvWeight", out: DevTensor, **kw):
+        """One ltb_op_conv2d; keywords as _conv_op."""
+        check(lib().ltb_op_conv2d(self._h, C.byref(self._conv_op(x, w, out, **kw))))
+
+    def conv_plan(self, x: DevTensor, w: "ConvWeight", out: DevTensor, **kw) -> dict:
+        """The kernel instance conv(x, w, out, **kw) would run (ltb_op_conv2d_plan, a test hook): the ltb_conv_variant fields."""
+        v = _capi.ConvVariant()
+        check(lib().ltb_op_conv2d_plan(self._h, C.byref(self._conv_op(x, w, out, **kw)), C.byref(v)))
+        return {n: getattr(v, n) for n, _ in v._fields_}
+
+    def _conv_op(self, x: DevTensor, w: "ConvWeight", out: DevTensor, *, N: int, IH: int, IW: int, OH: int, OW: int, stride=(1, 1),
+                 pad=(0, 0), res: Optional[DevTensor] = None, relu: bool = False, cin: Optional[int] = None, no_halo: bool = False,
+                 zbatch: int = 0, zdiv: int = 1, in_z=(0, 0), w_z=(0, 0), out_z=(0, 0), w_ptr: Optional[int] = None,
+                 ktot: Optional[int] = None, cout: Optional[int] = None, in_ptr: Optional[int] = None, out_ptr: Optional[int] = None,
+                 gn_stats: Optional[DevTensor] = None, gn_groups: int = 0, gn_hw: int = 0, upsample2x: bool = False,
+                 bias_ptr: Optional[int] = None, group: Optional[tuple] = None, transposed: bool = False) -> ConvOp:
         """group = (slot table int32 DevTensor, images per group, slots, w slot stride, bias slot stride): grouped weights
-        (ltb_conv_op.group_slot) read from w_ptr / bias_ptr.  no_halo: False / True, or 2 to require the TMA kernel."""
+        (ltb_conv_op.group_slot) read from w_ptr / bias_ptr.  no_halo: False / True, or 2 to require the TMA kernel.
+        transposed: ConvTranspose2d(k3, s2, p1, op1); w.w / w.w_tap hold the weight layouts of ltb_conv_op.transposed."""
         d = ConvOp()
         d.in_ = in_ptr if in_ptr is not None else x.ptr
         d.w = w_ptr if w_ptr is not None else w.w.ptr
@@ -188,7 +199,8 @@ class Ctx:
         if upsample2x:          # fused nearest-2x upsample + 3x3 conv: the 16-slice weights of ConvWeight.upconv()
             up = w.upconv(self)
             d.w, d.w_tap, d.Ktot, d.upsample2x = up[0].ptr, up[1].ptr, 16 * w.cin, 1
-        check(lib().ltb_op_conv2d(self._h, C.byref(d)))
+        d.transposed = int(transposed)
+        return d
 
     def groupnorm(self, x: DevTensor, N: int, HW: int, groups: int, eps: float, gamma: DevTensor, beta: DevTensor, silu: bool,
                   out: DevTensor):

@@ -9,10 +9,10 @@ pytestmark = pytest.mark.gpu
 
 CASES = [
     # N, H, W, Cin, Cout, k, (sy,sx), pad, transposed, res
-    (2, 16, 16, 64, 64, 3, (1, 1), 1, False, True),      # KB=64 BN=64, residual
-    (1, 12, 10, 32, 32, 3, (1, 1), 1, False, True),      # KB=32, ragged M (120 rows)
+    (2, 16, 16, 64, 64, 3, (1, 1), 1, False, True),      # halo BN=32, residual
+    (1, 12, 10, 32, 32, 3, (1, 1), 1, False, True),      # halo BN=32, overhanging tile (120 pixels)
     (2, 20, 20, 16, 32, 3, (2, 2), 1, False, False),     # KB=16, stride 2
-    (1, 12, 10, 128, 256, 3, (2, 2), 1, False, False),   # stride 2, 2 N tiles
+    (1, 12, 10, 128, 256, 3, (2, 2), 1, False, False),   # stride 2, 8 N tiles of 32
     (3, 80, 16, 32, 64, 3, (3, 1), 1, False, False),     # audio encoder stride (3,1)
     (3, 27, 16, 64, 128, 3, (3, 3), 1, False, False),    # audio encoder stride 3
     (3, 9, 6, 128, 256, 3, (3, 2), 1, False, False),     # audio encoder stride (3,2)
@@ -22,11 +22,11 @@ CASES = [
     (1, 5, 7, 64, 32, 3, (2, 2), 1, True, False),        # ConvT phases, ragged
     (2, 8, 8, 160, 64, 3, (2, 2), 1, True, False),       # ConvT KB=32
     (2, 4, 4, 1024, 512, 3, (2, 2), 1, True, False),     # ConvT deep K
-    (1, 16, 16, 384, 384, 3, (1, 1), 1, False, True),    # 3 N tiles of 128
-    (1, 24, 24, 80, 32, 3, (1, 1), 1, False, False),     # head conv: KB=16, 5 chunks per tap
+    (1, 16, 16, 384, 384, 3, (1, 1), 1, False, True),    # 12 N tiles of 32
+    (1, 24, 24, 80, 32, 3, (1, 1), 1, False, False),     # head conv: halo BN=32, ragged second K chunk
     (1, 64, 64, 64, 64, 3, (1, 1), 1, False, True),      # many M tiles
     (1, 32, 32, 320, 128, 3, (2, 2), 1, True, False),    # ConvT 320 -> 128
-    (8, 8, 8, 512, 512, 3, (1, 1), 1, False, True),      # split-K: M = 512, 72 K blocks, residual through the finalize kernel
+    (8, 8, 8, 512, 512, 3, (1, 1), 1, False, True),      # M = 512, 8 K chunks: halo BN=32 over overhanging tiles, residual
     (8, 4, 4, 1280, 640, 3, (1, 1), 1, False, False),    # split-K: M = 128, 180 K blocks
     (2, 8, 8, 256, 512, 3, (2, 2), 1, False, False),     # split-K with stride 2 (M = 32)
     (16, 16, 16, 768, 384, 3, (2, 2), 1, True, False),   # ConvT with 384 outputs: six 64-wide N tiles, fat-N issue up to N = 192
@@ -37,10 +37,10 @@ CASES = [
     (1, 64, 32, 128, 256, 3, (2, 2), 1, False, False),   # 2 K chunks, 4 N tiles
     (3, 40, 36, 64, 64, 3, (2, 2), 1, False, False),     # ragged output 20 x 18: overhanging tile rows / columns
     # narrow 3x3 layers on the halo kernel: streamed and resident weights, ragged chunks, overhanging tiles
-    (2, 64, 64, 64, 64, 3, (1, 1), 1, False, True),      # BN=64: residual, streamed weights
-    (5, 256, 64, 64, 64, 3, (1, 1), 1, False, True),     # same, enough tiles for the weights-resident variant
+    (2, 64, 64, 64, 64, 3, (1, 1), 1, False, True),      # BN=32: residual, streamed weights
+    (5, 256, 64, 64, 64, 3, (1, 1), 1, False, True),     # enough tiles for the weights-resident variant (BN=64, NSUB=2)
     (1, 96, 40, 80, 32, 3, (1, 1), 1, False, False),     # BN=32: 80 -> 32 (ragged second K chunk)
-    (3, 128, 128, 32, 32, 3, (1, 1), 1, False, True),    # 32 -> 32 + residual @128: resident weights
+    (3, 128, 128, 32, 32, 3, (1, 1), 1, False, True),    # 32 -> 32 + residual @128: BN=32, NSUB=2, streamed (192 tiles)
     (2, 50, 21, 64, 64, 3, (1, 1), 1, False, False),     # ragged height and width: masked last row tile / column tile
     (4, 256, 256, 80, 32, 3, (1, 1), 1, False, False),   # the output conv's geometry (2 chunks resident)
 ]
@@ -98,18 +98,18 @@ def test_conv_no_relu_negative_outputs():
 HALO_CASES = [
     # N, H, W, Cin, Cout, transposed, res
     (1, 16, 16, 64, 64, False, True),       # NSUB=1
-    (1, 64, 64, 64, 64, False, True),       # NSUB=2, BN=64
+    (1, 64, 64, 64, 64, False, True),       # NSUB=1, BN=32
     (2, 32, 32, 128, 128, False, True),     # 2 chunks
-    (1, 32, 16, 256, 384, False, False),    # 3 N tiles, 4 chunks
+    (1, 32, 16, 256, 384, False, False),    # 12 N tiles, 4 chunks
     (1, 32, 32, 80, 32, False, False),      # Cin=80: second chunk zero-filled beyond channel 80
     (2, 32, 8, 32, 32, False, True),        # Cin=32: half a chunk
-    (16, 16, 16, 512, 512, False, True),    # deep K, many tiles, persistent loop
+    (16, 16, 16, 512, 512, False, True),    # deep K, BN=128: 128 tiles
     (3, 48, 24, 64, 128, False, False),     # non power-of-two tiling
     (1, 16, 16, 64, 64, True, False),       # ConvT, 4 accumulators
     (2, 32, 32, 160, 64, True, False),      # ConvT Cin=160 (2.5 chunks)
     (1, 16, 8, 128, 32, True, False),       # ConvT BN=32
     (1, 32, 32, 320, 128, True, False),     # ConvT 320->128
-    (1, 128, 128, 64, 64, False, True),     # many tiles per CTA
+    (1, 128, 128, 64, 64, False, True),     # BN=64, NSUB=1: 128 tiles
     (16, 8, 8, 512, 512, False, True),      # map smaller than a tile: overhanging rows masked (w2l L28/L37)
     (16, 4, 4, 512, 512, False, True),      # 4x4 map: rows and columns masked (w2l L30/L35)
     (4, 4, 4, 1024, 512, True, False),      # ConvT 4x4 -> 8x8 (w2l L36)
@@ -118,7 +118,7 @@ HALO_CASES = [
     (3, 9, 6, 128, 128, False, True),       # odd height and width
     (2, 20, 12, 64, 32, True, False),       # ConvT over an odd-sized map
     (3, 64, 64, 544, 128, True, False),     # ConvT, 128 outputs in two BN=64 tiles, ragged last K chunk
-    (3, 64, 32, 512, 256, True, False),     # ConvT BN=128, two N tiles
+    (3, 64, 32, 512, 256, True, False),     # ConvT BN=64, four N tiles
 ]
 
 
