@@ -10,10 +10,13 @@
 // L2->SM operand traffic for A by 6.4x; weights are streamed 3 taps at a time and amortised over NSUB stacked 128-pixel
 // sub-tiles (M = 128 * NSUB per CTA).
 //
-// Roles (288 threads): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer.  Consumer warpgroup g owns pixel rows
-// [8g, 8g+8) of every 16-row sub-tile (64 MMA rows), issues its own wgmma into register accumulators and runs the epilogue
-// (+bias (+residual) -> ReLU -> fp16 NHWC channel slice) straight from the accumulator fragments.  Persistent CTAs: the
-// producer runs ahead across tiles, so the loads of tile i+1 overlap the epilogue of tile i.
+// Roles (384 threads): warps 0-7 = two consumer warpgroups, warpgroup 2 = TMA producer (one elected thread issues every
+// load).  The producer warpgroup gives its registers to the consumers (setmaxnreg 40 / 232), so the accumulators and the
+// epilogue of the widest tiles fit without spills.  Consumer warpgroup g owns pixel rows [8g, 8g+8) of every 16-row sub-tile
+// (64 MMA rows), issues its own wgmma into register accumulators and runs the epilogue (+bias (+residual) -> ReLU -> fp16
+// NHWC channel slice) straight from the accumulator fragments: the four lanes of a row swap their channel pairs so that each
+// lane stores (and reads the residual of) 8 consecutive channels with one 16-byte access.  Persistent CTAs: the producer
+// runs ahead across tiles, so the loads of tile i+1 overlap the epilogue of tile i.
 #include <cuda.h>
 
 #include <atomic>
@@ -34,7 +37,8 @@
 namespace ltb {
 
 constexpr int kHaloP = 10;  // halo row pitch in pixels (8 + 2)
-constexpr int kHaloThreads = 288;
+constexpr int kHaloThreads = 384;
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;   // 128 x 40 + 256 x 232 <= 64 K registers per SM
 constexpr int kSms = 132;   // H100 SXM: tile-count heuristics; launches read the device's own SM count
 
 // TAPS = 9: 3x3 conv / sub-pixel ConvT over a (16*NSUB+2) x 10 pixel halo.
@@ -105,11 +109,34 @@ __device__ __forceinline__ void fat_issue(float (&acc)[R], int j, int k, uint32_
   (
       [&] {
         constexpr FatMma g = FatTable<TAPS>::g[G];
-        if (j == g.stage)
+        if (j == g.stage) {
           wgmma_ss_at<g.nslots * BN, g.slot0 * BN>(acc, wgmma_lohi(a_lo0 + g.view * 8u + k * 2u, a_hi),
                                                    wgmma_lohi(b_lo0 + g.brow * BN * 8u + k * 2u, b_hi), 1u);
+          // groups of different N overlap in accumulator columns and must not be in flight together
+          wgmma_commit();
+          wgmma_wait<0>();
+        }
       }(),
       ...);
+}
+
+// 4 x 4 transpose of 32-bit words across the four lanes of a quad (lane q's word j <-> lane j's word q), two xor-shuffle
+// rounds.  Applied to the four channel-pair words of four 8-column blocks of one accumulator row, it turns "every lane holds
+// channels 8i + 2q (+1) of blocks i" into "lane q holds all 8 channels of block q"; it is its own inverse.
+__device__ __forceinline__ void quad_transpose(uint32_t (&x)[4], int lane) {
+  const bool b2 = lane & 2, b1 = lane & 1;
+  uint32_t s0 = __shfl_xor_sync(0xffffffffu, b2 ? x[0] : x[2], 2);
+  uint32_t s1 = __shfl_xor_sync(0xffffffffu, b2 ? x[1] : x[3], 2);
+  x[0] = b2 ? s0 : x[0];
+  x[1] = b2 ? s1 : x[1];
+  x[2] = b2 ? x[2] : s0;
+  x[3] = b2 ? x[3] : s1;
+  s0 = __shfl_xor_sync(0xffffffffu, b1 ? x[0] : x[1], 1);
+  s1 = __shfl_xor_sync(0xffffffffu, b1 ? x[2] : x[3], 1);
+  x[0] = b1 ? s0 : x[0];
+  x[2] = b1 ? s1 : x[2];
+  x[1] = b1 ? x[1] : s0;
+  x[3] = b1 ? x[3] : s1;
 }
 
 // GRP: grouped GEMM mode (TAPS == 1 only): per-group M-tiles and weight slots, see HaloParams::group_slot
@@ -167,9 +194,10 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
   }
   pdl_wait();
 
-  if (warp == 8) {
+  if (warp >= 8) {
     // =============================================================== TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == 8 && lane == 0) {
       uint32_t ai = 0, bi = 0;  // running stage counters
       for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
         const int nt = t / tiles_m;
@@ -226,6 +254,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
     }
   } else {
     // =============================================================== consumers: wgmma + epilogue
+    setmaxnreg_inc<kConsumerRegs>();
     const int wg = warp >> 2, wq = warp & 3;
     const int cq = 2 * (lane & 3);
     constexpr uint32_t kAHi = wgmma_hi_128b(C::P * 128);   // SBO = halo pitch (1280 B) / 1024 B in GEMM mode
@@ -368,28 +397,46 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
               opix = (size_t)mt * (128 * NSUB) + sub * 128 + wg * 64 + r;   // GEMM mode: output row index
               row_ok = opix < (size_t)p.M;
             }
-            __half* optr = p.out + opix * p.OCtot + p.oc_off + n0;
-            const __half* rptr = has_res ? p.res + opix * p.RCtot + p.rc_off + n0 : nullptr;
-            __half2 oh[BN / 8];
+            // block 4m + (lane & 3) of this row: 8 channels, 16-byte aligned (conv_halo_supported)
+            const size_t ocol = n0 + 8 * (lane & 3);
+            uint4* optr = reinterpret_cast<uint4*>(p.out + opix * p.OCtot + p.oc_off + ocol);
+            const uint4* rptr = has_res ? reinterpret_cast<const uint4*>(p.res + opix * p.RCtot + p.rc_off + ocol) : nullptr;
+            __half2 oh[BN / 8];   // the row's values in accumulator order (lane holds channels 8i + cq (+1))
 #pragma unroll
-            for (int i = 0; i < BN / 8; ++i) {
-              const float f0 = acc[sub][sl * BN / 2 + 4 * i + 2 * hh] + bb[i].x;
-              const float f1 = acc[sub][sl * BN / 2 + 4 * i + 2 * hh + 1] + bb[i].y;
-              uint32_t w;
-              if (!has_res && p.relu) {
-                w = f32x2_to_f16x2_sat_relu(f0, f1);
-              } else {
-                w = f32x2_to_f16x2_sat(f0, f1);
-                if (has_res && row_ok) {
-                  const __half2 rh = __ldcg(reinterpret_cast<const __half2*>(rptr + 8 * i + cq));
-                  __half2 o = *reinterpret_cast<__half2*>(&w);
-                  o = __hmin2(__hmax2(__hadd2(o, rh), hlo), hmax);
-                  w = *reinterpret_cast<uint32_t*>(&o);
+            for (int m = 0; m < BN / 32; ++m) {
+              uint32_t v[4];
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const int i = 4 * m + j;
+                const float f0 = acc[sub][sl * BN / 2 + 4 * i + 2 * hh] + bb[i].x;
+                const float f1 = acc[sub][sl * BN / 2 + 4 * i + 2 * hh + 1] + bb[i].y;
+                v[j] = (!has_res && p.relu) ? f32x2_to_f16x2_sat_relu(f0, f1) : f32x2_to_f16x2_sat(f0, f1);
+                oh[i] = *reinterpret_cast<const __half2*>(&v[j]);
+              }
+              if (!head || has_res) {
+                quad_transpose(v, lane);
+                if (has_res) {
+                  uint4 r4 = make_uint4(0u, 0u, 0u, 0u);
+                  if (row_ok) r4 = __ldcg(rptr + 4 * m);
+                  const uint32_t rv[4] = {r4.x, r4.y, r4.z, r4.w};
+#pragma unroll
+                  for (int j = 0; j < 4; ++j) {
+                    __half2 o = *reinterpret_cast<const __half2*>(&v[j]);
+                    o = __hmin2(__hmax2(__hadd2(o, *reinterpret_cast<const __half2*>(&rv[j])), hlo), hmax);
+                    v[j] = *reinterpret_cast<const uint32_t*>(&o);
+                  }
+                }
+                if (row_ok && !head && !LTB_DIAG(1)) optr[4 * m] = make_uint4(v[0], v[1], v[2], v[3]);
+                if (has_res && (p.gn_stats || head)) {   // the statistics and the head read the sums in accumulator order
+                  quad_transpose(v, lane);
+#pragma unroll
+                  for (int j = 0; j < 4; ++j) oh[4 * m + j] = *reinterpret_cast<const __half2*>(&v[j]);
                 }
               }
-              oh[i] = *reinterpret_cast<__half2*>(&w);
-              if (row_ok && !head && !LTB_DIAG(1)) *reinterpret_cast<__half2*>(optr + 8 * i + cq) = oh[i];
-              if (p.gn_stats && row_ok) {
+            }
+            if (p.gn_stats && row_ok) {
+#pragma unroll
+              for (int i = 0; i < BN / 8; ++i) {
                 const float2 f = __half22float2(oh[i]);
                 gs[i] += f.x + f.y;
                 gq[i] += f.x * f.x + f.y * f.y;
@@ -534,6 +581,9 @@ static bool pick_cfg(const ConvParams& p, int* BN, int* NSUB, int* NACC);
 
 bool conv_halo_supported(const ConvParams& p) {
   if (p.zbatch > 1) return false;   // the halo kernel runs one GEMM per launch
+  // the epilogue writes the output (and reads the residual) 8 channels per 16-byte access
+  if ((p.OCtot % 8) || (p.oc_off % 8) || (reinterpret_cast<uintptr_t>(p.out) % 16)) return false;
+  if (p.res && ((p.RCtot % 8) || (p.rc_off % 8) || (reinterpret_cast<uintptr_t>(p.res) % 16))) return false;
   // grouped weights: GEMM mode only (the weight map's slot stride must be 16-byte aligned); 3x3, stride-2, ConvT and upsample
   // layers go to the gather kernel
   if (p.group_slot && (!is_gemm(p) || (p.w_slot_stride * 2) % 16 != 0)) return false;

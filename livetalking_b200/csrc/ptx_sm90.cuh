@@ -307,6 +307,17 @@ __device__ __forceinline__ uint32_t f32x2_to_f16x2_sat_relu(float lo, float hi) 
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
+// Warpgroup register reallocation: every thread of the warpgroup executes it; the kernel's register count (from
+// __launch_bounds__) must be the per-thread budget the warpgroups trade within.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(

@@ -26,6 +26,8 @@ def main():
         ("L41 ConvT 768->384 @16", 16, 16, 768, 384, True, False),
         ("L42 conv 384->384 @32 res", 16, 32, 384, 384, False, True),
         ("L45 conv 256->256 @64 res", 16, 64, 256, 256, False, True),
+        ("L48 conv 128->128 @128 res", 16, 128, 128, 128, False, True),
+        ("L51 conv 64->64 @256 res", 16, 256, 64, 64, False, True),
         ("L39 conv 512->512 @16 res", 16, 16, 512, 512, False, True),
         ("L25 conv 256->256 @16 res", 16, 16, 256, 256, False, True),
         ("L28 conv 512->512 @8 res", 16, 8, 512, 512, False, True),
