@@ -225,9 +225,10 @@ int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d);
  * argument checks and planning; nothing is launched.  kernel: 0 = cp.async gather kernel conv_gather_wgmma_kernel<bn, kb,
  * grouped>, 1 = TMA kernel conv_halo_wgmma_kernel<bn, nsub, nacc, taps, resident_chunks, grouped> (taps: 9 = 3x3 / ConvT,
  * 10 = stride-2 parity planes, 16 = fused upsample, 1 = GEMM mode).  ksplit > 1: the gather kernel splits K that many ways
- * and a finalize kernel sums the slices.  Fields that do not apply to the kernel are 0. */
+ * and a finalize kernel sums the slices.  res_halo = 1: the TMA kernel adds the residual from its shared-memory halo tiles
+ * (res is the input slice itself) instead of reading res from global memory.  Fields that do not apply to the kernel are 0. */
 typedef struct ltb_conv_variant {
-  int kernel, taps, bn, nsub, nacc, resident_chunks, kb, ksplit, grouped;
+  int kernel, taps, bn, nsub, nacc, resident_chunks, kb, ksplit, grouped, res_halo;
 } ltb_conv_variant;
 int ltb_op_conv2d_plan(ltb_ctx* c, const ltb_conv_op* d, ltb_conv_variant* out);
 int ltb_op_w_tap_major(ltb_ctx* c, const void* w, void* wt, int cout, int cin);

@@ -32,7 +32,7 @@ class ConvOp(C.Structure):
 
 
 class ConvVariant(C.Structure):
-    _fields_ = [(n, C.c_int) for n in ("kernel", "taps", "bn", "nsub", "nacc", "resident_chunks", "kb", "ksplit", "grouped")]
+    _fields_ = [(n, C.c_int) for n in ("kernel", "taps", "bn", "nsub", "nacc", "resident_chunks", "kb", "ksplit", "grouped", "res_halo")]
 
 
 class UlPrepGroup(C.Structure):

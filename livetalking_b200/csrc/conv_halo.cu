@@ -15,8 +15,10 @@
 // epilogue of the widest tiles fit without spills.  Consumer warpgroup g owns pixel rows [8g, 8g+8) of every 16-row sub-tile
 // (64 MMA rows), issues its own wgmma into register accumulators and runs the epilogue (+bias (+residual) -> ReLU -> fp16
 // NHWC channel slice) straight from the accumulator fragments: the four lanes of a row swap their channel pairs so that each
-// lane stores (and reads the residual of) 8 consecutive channels with one 16-byte access.  Persistent CTAs: the producer
-// runs ahead across tiles, so the loads of tile i+1 overlap the epilogue of tile i.
+// lane stores (and reads the residual of) 8 consecutive channels with one 16-byte access.  A conv whose residual is its own
+// input (HaloParams::res_halo) takes it from the halo instead: the consumers ldmatrix the centre view of the chunks holding
+// the tile's channels while they hold those stages, and add it in accumulator order.  Persistent CTAs: the producer runs
+// ahead across tiles, so the loads of tile i+1 overlap the epilogue of tile i.
 #include <cuda.h>
 
 #include <atomic>
@@ -138,6 +140,11 @@ __device__ __forceinline__ void quad_transpose(uint32_t (&x)[4], int lane) {
   x[1] = b1 ? x[1] : s0;
   x[3] = b1 ? x[3] : s1;
 }
+
+// Instances that can take the residual from the halo (HaloParams::res_halo): 3x3 stride-1 convs with one accumulator slot.
+// <128, 2, 1> is left out: its 128 accumulator floats, 64 residual words and the epilogue's GroupNorm partial sums do not fit
+// the 232 consumer registers without spills, so it keeps reading the residual from global memory.
+constexpr bool halo_res_smem_ok(int BN, int NSUB, int NACC, int TAPS) { return TAPS == 9 && NACC == 1 && BN * NSUB <= 128; }
 
 // GRP: grouped GEMM mode (TAPS == 1 only): per-group M-tiles and weight slots, see HaloParams::group_slot
 template <int BN, int NSUB, int NACC, int TAPS, int RC, bool GRP>
@@ -262,6 +269,13 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
     // this warpgroup's first MMA row inside a sub-tile / plane: pixel row 8*wg (halo modes), row 64*wg (GEMM mode)
     constexpr uint32_t kRowsPerSub = C::HALO ? 16u * C::P : 128u;
     const uint32_t wg_off = (uint32_t)wg * (C::HALO ? 8u * C::P : 64u) * 8u;   // in 16-byte descriptor units
+    // residual from the halo (p.res_halo): output channels [n0, n0 + BN) of a 3x3 conv whose residual is its own input are the
+    // centre view (dy = dx = 1) of the halo stages of K chunks n0/64 (and n0/64 + 1 for BN = 128).  ldmatrix.x4 reads
+    // matrices (row half hh, channel block i) = (0, i), (1, i), (0, i+1), (1, i+1): lanes 8k..8k+7 address rows 0..7 of matrix k,
+    // and each lane receives its accumulator-fragment words rh[sub][hh][i] (row lane/4 + 8hh, channels 8i + cq (+1)).
+    constexpr bool kResHalo = halo_res_smem_ok(BN, NSUB, NACC, TAPS);
+    const int res_row = (8 * wg + 2 * wq + ((lane >> 3) & 1) + 1) * C::P + (lane & 7) + 1;   // halo row of MMA row (r % 8 = lane % 8)
+    const int res_kb = lane >> 4;
     if (RC) mbar_wait(smem_u32(&b_full[0]), 0);
     uint32_t ai = 0, bi = 0;
     for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
@@ -270,12 +284,33 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
       for (int s = 0; s < NSUB; ++s)
 #pragma unroll
         for (int i = 0; i < C::ACOLS / 2; ++i) acc[s][i] = 0.f;
+      uint32_t rh[NSUB][2][BN / 8];
+      const int n0_res = (t / tiles_m) * BN;
+      const int c_res = (kResHalo && p.res_halo) ? n0_res / 64 : chunks;   // chunks: no chunk holds it
+      const int cb_res = (BN == 32) ? (n0_res & 63) >> 3 : 0;              // first 8-channel block of the tile in its chunk
       uint32_t pend_as = 0, pend_bs = 0;   // stages of the previous chunk (LAG mode), released once its wgmma group retired
       bool pend = false;
 #pragma unroll 1
       for (int c = 0; c < chunks; ++c) {
         const uint32_t as = ai % C::A_STAGES;
         mbar_wait(smem_u32(&a_full[as]), (ai / C::A_STAGES) & 1u);
+        if constexpr (kResHalo) {
+          // read here, while this warp still holds the stage (it is handed back after this chunk's MMAs, or the next chunk's)
+          if (c == c_res || (BN == 128 && c == c_res + 1)) {
+            const bool hi = BN == 128 && c != c_res;
+            const uint32_t rbase = a_smem + as * C::A_BYTES + res_row * 128;
+#pragma unroll
+            for (int s = 0; s < NSUB; ++s)
+#pragma unroll
+              for (int i = 0; i < BN / 8; i += 2) {
+                if (BN == 128 && (i >= 8) != hi) continue;
+                // 128B swizzle on a 1024-aligned stage: 16-byte chunk (channel / 8) XOR (halo row & 7); 16 * P rows per sub-tile
+                // keep the row's phase
+                const uint32_t chunk16 = (uint32_t)(((cb_res + i + res_kb) & 7) ^ (res_row & 7));
+                ldmatrix_x4(rh[s][0][i], rh[s][1][i], rh[s][0][i + 1], rh[s][1][i + 1], rbase + s * (16 * C::P * 128) + chunk16 * 16);
+              }
+          }
+        }
         const uint32_t a_lo0 = wgmma_lo(a_smem + as * C::A_BYTES) + wg_off;
         const uint32_t bs0 = bi % C::B_STAGES;
         // 3x3 / GEMM layers: unrolled (a data-dependent branch around wgmma makes ptxas serialise the wgmma pipeline).  Sub-pixel
@@ -365,12 +400,19 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
         bias += p.group_slot[g_tile] * p.bias_slot_stride;
       }
       const bool has_res = (p.res != nullptr) && !LTB_DIAG(1);
+      const bool res_smem = kResHalo && has_res && p.res_halo;   // residual in rh, added in accumulator order
+      const bool res_gmem = has_res && !res_smem;                // residual read from p.res after the quad transpose
       const bool head = kHeadOk && p.head_out != nullptr;
       float2 bb[BN / 8];
 #pragma unroll
       for (int i = 0; i < BN / 8; ++i) bb[i] = __ldg(reinterpret_cast<const float2*>(bias + n0 + 8 * i + cq));
       const __half2 hmax = __floats2half2_rn(65504.f, 65504.f);
       const __half2 hlo = p.relu ? __floats2half2_rn(0.f, 0.f) : __floats2half2_rn(-65504.f, -65504.f);
+      // (conv + bias) + residual, clamped: the same fp16 operation on either residual path
+      auto add_res = [&](uint32_t v, uint32_t r) {
+        const __half2 o = __hmin2(__hmax2(__hadd2(*reinterpret_cast<const __half2*>(&v), *reinterpret_cast<const __half2*>(&r)), hlo), hmax);
+        return *reinterpret_cast<const uint32_t*>(&o);
+      };
 #pragma unroll
       for (int sub = 0; sub < NSUB; ++sub) {
         // GroupNorm partial sums of this warp's 16 rows, per 8-column block
@@ -400,7 +442,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
             // block 4m + (lane & 3) of this row: 8 channels, 16-byte aligned (conv_halo_supported)
             const size_t ocol = n0 + 8 * (lane & 3);
             uint4* optr = reinterpret_cast<uint4*>(p.out + opix * p.OCtot + p.oc_off + ocol);
-            const uint4* rptr = has_res ? reinterpret_cast<const uint4*>(p.res + opix * p.RCtot + p.rc_off + ocol) : nullptr;
+            const uint4* rptr = res_gmem ? reinterpret_cast<const uint4*>(p.res + opix * p.RCtot + p.rc_off + ocol) : nullptr;
             __half2 oh[BN / 8];   // the row's values in accumulator order (lane holds channels 8i + cq (+1))
 #pragma unroll
             for (int m = 0; m < BN / 32; ++m) {
@@ -411,23 +453,21 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
                 const float f0 = acc[sub][sl * BN / 2 + 4 * i + 2 * hh] + bb[i].x;
                 const float f1 = acc[sub][sl * BN / 2 + 4 * i + 2 * hh + 1] + bb[i].y;
                 v[j] = (!has_res && p.relu) ? f32x2_to_f16x2_sat_relu(f0, f1) : f32x2_to_f16x2_sat(f0, f1);
+                if constexpr (kResHalo)
+                  if (res_smem) v[j] = add_res(v[j], rh[sub][hh][i]);
                 oh[i] = *reinterpret_cast<const __half2*>(&v[j]);
               }
-              if (!head || has_res) {
+              if (!head || res_gmem) {
                 quad_transpose(v, lane);
-                if (has_res) {
+                if (res_gmem) {
                   uint4 r4 = make_uint4(0u, 0u, 0u, 0u);
                   if (row_ok) r4 = __ldcg(rptr + 4 * m);
                   const uint32_t rv[4] = {r4.x, r4.y, r4.z, r4.w};
 #pragma unroll
-                  for (int j = 0; j < 4; ++j) {
-                    __half2 o = *reinterpret_cast<const __half2*>(&v[j]);
-                    o = __hmin2(__hmax2(__hadd2(o, *reinterpret_cast<const __half2*>(&rv[j])), hlo), hmax);
-                    v[j] = *reinterpret_cast<const uint32_t*>(&o);
-                  }
+                  for (int j = 0; j < 4; ++j) v[j] = add_res(v[j], rv[j]);
                 }
                 if (row_ok && !head && !LTB_DIAG(1)) optr[4 * m] = make_uint4(v[0], v[1], v[2], v[3]);
-                if (has_res && (p.gn_stats || head)) {   // the statistics and the head read the sums in accumulator order
+                if (res_gmem && (p.gn_stats || head)) {   // the statistics and the head read the sums in accumulator order
                   quad_transpose(v, lane);
 #pragma unroll
                   for (int j = 0; j < 4; ++j) oh[4 * m + j] = *reinterpret_cast<const __half2*>(&v[j]);
@@ -749,6 +789,10 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
   h.osy = p.osy;
   h.osx = p.osx;
   h.relu = p.relu;
+  // the residual is exactly the input slice the halo tiles hold (the wav2lip residual blocks): channels [n0, n0 + BN) of the
+  // tile's centre view
+  h.res_halo = halo_res_smem_ok(BN, NSUB, NACC, out->TAPS) && p.res != nullptr && p.res == p.in && p.Cin == p.Cout &&
+               p.rc_off == p.ic_off && p.RCtot == p.ICtot;
   h.halo_y0 = tr ? 0 : -1;
   h.halo_x0 = tr ? 0 : -1;
   if (up || tr) {

@@ -20,6 +20,9 @@ struct alignas(64) HaloParams {
   int OH, OW, osy, osx;
   int GH, GW;            // tile-grid extent (= input H, W): tiles may overhang it, rows/columns beyond are masked
   int relu;
+  // the residual is the conv's own input slice (3x3 stride-1, Cin == Cout): the epilogue takes it from the centre view of the
+  // halo tiles in shared memory instead of reading res from global memory
+  int res_halo;
   int halo_y0, halo_x0;  // halo origin relative to the tile origin (-1 for pad-1 conv, 0 for ConvT phases)
   // output offset of each accumulator slot (sub-pixel phase; slot order p0, p1, p3, p2, see conv_halo.cu FatTable)
   int acc_oy[4], acc_ox[4];

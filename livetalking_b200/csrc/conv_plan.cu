@@ -121,6 +121,7 @@ bool conv_plan_variant(const ConvPlan& pl, bool have_ws, size_t ws_floats, ltb_c
     out->nsub = pl.hp.NSUB;
     out->nacc = pl.hp.NACC;
     out->resident_chunks = conv_halo_resident_chunks(pl.hp, conv_halo_sms());
+    out->res_halo = pl.hp.hp.res_halo;
     return true;
   }
   int ksplit = 0;

@@ -94,6 +94,16 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const void* tmap, uint
       : "memory");
 }
 
+// ---------------------------------------------------------------- ldmatrix
+// four 8x8 b16 matrices; lanes 8k..8k+7 give the 16-byte row addresses of matrix k, and lane l receives row l/4, elements
+// 2(l%4) (+1) of each matrix: the wgmma accumulator fragment layout of one 8-row x 8-column block
+__device__ __forceinline__ void ldmatrix_x4(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(saddr)
+               : "memory");
+}
+
 // ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
 // K-major shared-memory matrix descriptor: rows of the swizzle span (128 / 64 / 32 B) packed densely, 8-row core groups SBO
 // bytes apart; LBO is the distance between K-adjacent core matrices (used by SWIZZLE_NONE only).

@@ -152,10 +152,20 @@ class Ctx:
         check(lib().ltb_op_conv2d(self._h, C.byref(self._conv_op(x, w, out, **kw))))
 
     def conv_plan(self, x: DevTensor, w: "ConvWeight", out: DevTensor, **kw) -> dict:
-        """The kernel instance conv(x, w, out, **kw) would run (ltb_op_conv2d_plan, a test hook): the ltb_conv_variant fields."""
+        """The kernel instance conv(x, w, out, **kw) would run (ltb_op_conv2d_plan, a test hook): the ltb_conv_variant fields
+        that name the instance (all but res_halo)."""
+        v = self._conv_variant(x, w, out, **kw)
+        return {n: getattr(v, n) for n, _ in v._fields_ if n != "res_halo"}
+
+    def conv_res_halo(self, x: DevTensor, w: "ConvWeight", out: DevTensor, **kw) -> bool:
+        """Whether conv(x, w, out, **kw) would add its residual from the TMA kernel's shared-memory halo tiles (res is the
+        input slice itself) rather than read it from global memory (ltb_conv_variant.res_halo, a test hook)."""
+        return bool(self._conv_variant(x, w, out, **kw).res_halo)
+
+    def _conv_variant(self, x: DevTensor, w: "ConvWeight", out: DevTensor, **kw) -> "_capi.ConvVariant":
         v = _capi.ConvVariant()
         check(lib().ltb_op_conv2d_plan(self._h, C.byref(self._conv_op(x, w, out, **kw)), C.byref(v)))
-        return {n: getattr(v, n) for n, _ in v._fields_}
+        return v
 
     def _conv_op(self, x: DevTensor, w: "ConvWeight", out: DevTensor, *, N: int, IH: int, IW: int, OH: int, OW: int, stride=(1, 1),
                  pad=(0, 0), res: Optional[DevTensor] = None, relu: bool = False, cin: Optional[int] = None, no_halo: bool = False,

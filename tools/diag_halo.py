@@ -37,11 +37,16 @@ def main():
     if os.environ.get("LTB_DIAG_ONLY"):          # e.g. "0:0" = first case, variant 0 (for an ncu capture)
         ci, v = os.environ["LTB_DIAG_ONLY"].split(":")
         cases, variants = [cases[int(ci)]], [int(v)]
-    for name, N, H, cin, cout, res in cases:
-        x = ctx.upload((rng.standard_normal((N * H * H, cin)) * 0.5).astype(np.float16))
+    # a residual case runs twice: residual = the conv input itself (taken from the halo tiles in shared memory) and
+    # residual = a copy of it (read from global memory)
+    cases = [(name + (" copy" if copy else ""), N, H, cin, cout, res, copy) for name, N, H, cin, cout, res in cases
+             for copy in ((False, True) if res else (False,))]
+    for name, N, H, cin, cout, res, copy in cases:
+        xh = (rng.standard_normal((N * H * H, cin)) * 0.5).astype(np.float16)
+        x = ctx.upload(xh)
         w = ops.ConvWeight(ctx, (rng.standard_normal((cout, cin, 3, 3)) * 0.05).astype(np.float32), np.zeros(cout, np.float32))
         out = ctx.alloc((N * H * H, cout), np.float16)
-        r = x if (res and cin == cout) else None
+        r = (ctx.upload(xh) if copy else x) if (res and cin == cout) else None
         flops = 2.0 * N * H * H * 9 * cin * cout
         line = [name]
         for v in variants:
