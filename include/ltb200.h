@@ -297,6 +297,13 @@ int ltb_op_hubert_pos_conv(ltb_ctx* c, const void* h, int T, int D, int groups, 
  * HubertASR.run_step calls it (hubert.py:42-45): out_f32 [B][R][D] and / or out_nhwc fp16 [B][D][R] */
 int ltb_op_hubert_slice(ltb_ctx* c, const void* hidden, int Tc, int T, int D, int B, int R, float start, float mult, int win_l, float* out_f32,
                         void* out_nhwc);
+/* The three HuBERT ops above over G windows stacked on the row dimension (cross-session batching: one encoder forward for G sessions).
+ * pcm f32 [G][n], stats [G][4] (each window normalised with its own mean / variance), conv0 out [G][(n-10)/5+1][C]; pos_conv h / out
+ * [G][T][D], zero padding per window; slice hidden [G][Tc][D] -> out_f32 [G][B][R][D] / out_nhwc [G][B][D][R].  G = 1 is the op above. */
+int ltb_op_hubert_conv0_grouped(ltb_ctx* c, const float* pcm, int G, int n, const float* w, const float* bias, int C, float* stats, void* out);
+int ltb_op_hubert_pos_conv_grouped(ltb_ctx* c, const void* h, int G, int T, int D, int groups, int K, const void* w, const float* bias, void* out);
+int ltb_op_hubert_slice_grouped(ltb_ctx* c, const void* hidden, int G, int Tc, int T, int D, int B, int R, float start, float mult, int win_l,
+                                float* out_f32, void* out_nhwc);
 /* VAE.decode_latents post-processing, avatars/musetalk/models/vae.py:104-107 -> uint8 BGR NHWC */
 int ltb_op_vae_post(ltb_ctx* c, const void* x, long long npix, int Ctot, void* out_u8);
 /* Encoder hand-off (SURVEY 8(f) rank 3): composited uint8 BGR frames [N,H,W,3] -> planar I420 [N, H*3/2, W] on the device,

@@ -140,6 +140,12 @@ _SIGS = {
     "ltb_op_hubert_pos_conv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ltb_op_hubert_slice": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int,
                                       C.c_void_p, C.c_void_p]),
+    "ltb_op_hubert_conv0_grouped": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                              C.c_void_p]),
+    "ltb_op_hubert_pos_conv_grouped": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p]),
+    "ltb_op_hubert_slice_grouped": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                              C.c_float, C.c_int, C.c_void_p, C.c_void_p]),
     "ltb_op_vae_post": (C.c_int, [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_void_p]),
     "ltb_op_bgr_to_i420": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "ltb_op_stamp_pixels": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]),

@@ -10,10 +10,16 @@
 
 namespace ltb {
 
+// Every kernel takes a sequence count G: G windows of n samples stacked on the row dimension ([G][n] PCM, [G][T][C] activations,
+// [G][B][R][D] windows).  Sequence g reads and writes only its own rows; G = 1 is the single-window layout.
+
 // ------------------------------------------------------------------------------------------------ utterance statistics
-// stats[0] = mean, stats[1] = 1 / sqrt(var + 1e-7) (population variance) — Wav2Vec2FeatureExtractor.zero_mean_unit_var_norm.
+// stats[4g + 0] = mean, stats[4g + 1] = 1 / sqrt(var + 1e-7) (population variance) of window g (one block per window) —
+// Wav2Vec2FeatureExtractor.zero_mean_unit_var_norm, which normalises each input sequence on its own.
 __global__ void __launch_bounds__(1024) wave_stats_kernel(const float* __restrict__ x, int n, float* __restrict__ stats) {
   __shared__ double s1[32], s2[32];
+  x += (size_t)blockIdx.x * n;
+  stats += 4 * blockIdx.x;
   double a = 0.0, b = 0.0;
   for (int i = threadIdx.x; i < n; i += 1024) {
     const double v = (double)x[i];
@@ -37,10 +43,15 @@ __global__ void __launch_bounds__(1024) wave_stats_kernel(const float* __restric
 }
 
 // out[t][c] = bias[c] + sum_k w[c][k] * (x[5t + k] - mean) * inv_std,  t < T0 = (n - 10) / 5 + 1 ; fp32 math, fp16 out [T0][512]
-__global__ void __launch_bounds__(256) hubert_conv0_kernel(const float* __restrict__ x, const float* __restrict__ stats, const float* __restrict__ w,
-                                                           const float* __restrict__ bias, int T0, int C, __half* __restrict__ out) {
+// per window (blockIdx.y)
+__global__ void __launch_bounds__(256) hubert_conv0_kernel(const float* __restrict__ x, int n, const float* __restrict__ stats,
+                                                           const float* __restrict__ w, const float* __restrict__ bias, int T0, int C,
+                                                           __half* __restrict__ out) {
   pdl_launch_dependents();   // a PDL-launched successor (the conv kernels) may start its prologue now; it waits before reading
-  const int t = blockIdx.x;
+  const int t = blockIdx.x, g = blockIdx.y;
+  x += (size_t)g * n;
+  stats += 4 * g;
+  out += (size_t)g * T0 * C;
   __shared__ float xs[10];
   if (threadIdx.x < 10) xs[threadIdx.x] = (x[5 * t + threadIdx.x] - stats[0]) * stats[1];
   __syncthreads();
@@ -52,11 +63,12 @@ __global__ void __launch_bounds__(256) hubert_conv0_kernel(const float* __restri
   }
 }
 
-cudaError_t launch_hubert_conv0(const float* pcm, int n, const float* w, const float* bias, int C, float* stats, __half* out, cudaStream_t st) {
-  if (n < 10) return cudaErrorInvalidValue;
-  wave_stats_kernel<<<1, 1024, 0, st>>>(pcm, n, stats);
+cudaError_t launch_hubert_conv0(const float* pcm, int G, int n, const float* w, const float* bias, int C, float* stats, __half* out,
+                                cudaStream_t st) {
+  if (n < 10 || G < 1 || G > 65535) return cudaErrorInvalidValue;
+  wave_stats_kernel<<<G, 1024, 0, st>>>(pcm, n, stats);
   const int T0 = (n - 10) / 5 + 1;
-  return launch_kernel_plain(hubert_conv0_kernel, dim3(T0), dim3(256), 0, st, pcm, stats, w, bias, T0, C, out);
+  return launch_kernel_plain(hubert_conv0_kernel, dim3(T0, G), dim3(256), 0, st, pcm, n, stats, w, bias, T0, C, out);
 }
 
 // ------------------------------------------------------------------------------------------------ positional convolution
@@ -64,6 +76,7 @@ cudaError_t launch_hubert_conv0(const float* pcm, int n, const float* w, const f
 // gelu(bias[co] + sum_{k < K, ci < D/G} h[t + k - K/2][g*D/G + ci] * w[co][k][ci])  for t < T (the SamePad layer drops the extra
 // last step an even kernel produces).  One block = 4 output channels of one group x 64 time steps; the group's input slab
 // lives in shared memory (rows padded by one word: conflict-free column walks), weights stream through L1 as broadcasts.
+// blockIdx.z = sequence: its T rows are zero-padded on their own, so no tap reads a neighbouring sequence.
 constexpr int kPcK = 128, kPcCg = 64, kPcRows = 64 + kPcK - 1, kPcPitch = kPcCg / 2 + 1;   // pitch in 32-bit words
 
 __device__ __forceinline__ float gelu_erf(float v) { return 0.5f * v * (1.f + erff(v * 0.70710678118654752f)); }
@@ -72,6 +85,8 @@ __global__ void __launch_bounds__(256) hubert_pos_conv_kernel(const __half* __re
                                                               const float* __restrict__ bias, __half* __restrict__ out) {
   pdl_launch_dependents();   // a PDL-launched successor (the conv kernels) may start its prologue now; it waits before reading
   __shared__ uint32_t slab[kPcRows * kPcPitch];
+  h += (size_t)blockIdx.z * T * D;
+  out += (size_t)blockIdx.z * T * D;
   const int g = blockIdx.y, co = g * kPcCg + blockIdx.x * 4 + (threadIdx.x >> 6), tl = threadIdx.x & 63;
   for (int t0 = 0; t0 < T; t0 += 64) {
     __syncthreads();
@@ -106,21 +121,25 @@ __global__ void __launch_bounds__(256) hubert_pos_conv_kernel(const __half* __re
   }
 }
 
-cudaError_t launch_hubert_pos_conv(const __half* h, int T, int D, int groups, int K, const __half* w, const float* bias, __half* out,
+cudaError_t launch_hubert_pos_conv(const __half* h, int G, int T, int D, int groups, int K, const __half* w, const float* bias, __half* out,
                                    cudaStream_t st) {
-  if (K != kPcK || D % groups || D / groups != kPcCg || h == out) return cudaErrorInvalidValue;
-  return launch_kernel_plain(hubert_pos_conv_kernel, dim3(dim3(kPcCg / 4, groups)), dim3(256), 0, st, h, T, D, w, bias, out);
+  if (K != kPcK || D % groups || D / groups != kPcCg || h == out || G < 1 || G > 65535) return cudaErrorInvalidValue;
+  return launch_kernel_plain(hubert_pos_conv_kernel, dim3(kPcCg / 4, groups, G), dim3(256), 0, st, h, T, D, w, bias, out);
 }
 
 // ------------------------------------------------------------------------------------------------ window gather
 // hidden fp16 [Tc][D] (Tc = conv frames); the reference trims / zero-pads it to T = (n - 80) / 320 rows (audio2feature.py:50-55), then
 // frame i takes rows clamp(left .. right-1, 0, T-1), left = int((i + start) * mult) - int(win_l * mult) (base_asr.py:107-129).
 // out_f32 [B][R][D] (what HubertASR queues, float32) and/or out_nhwc fp16 [B][D][R] (the U-Net's (B,32,32,16) NHWC input:
-// audiofeat.reshape(16,32,32) -> channel = row, pixel = feature index; ultralight_avatar.py:162).
+// audiofeat.reshape(16,32,32) -> channel = row, pixel = feature index; ultralight_avatar.py:162).  blockIdx.z = sequence g: it gathers
+// from its own hidden rows [g*Tc, (g+1)*Tc) into its own B windows.
 __global__ void __launch_bounds__(256) hubert_slice_kernel(const __half* __restrict__ hidden, int Tc, int T, int D, int B, int R, float start,
                                                            float mult, int win_l, float* __restrict__ out_f32, __half* __restrict__ out_nhwc) {
   pdl_launch_dependents();   // a PDL-launched successor (the conv kernels) may start its prologue now; it waits before reading
-  const int b = blockIdx.y, r = blockIdx.x;
+  const int b = blockIdx.y, r = blockIdx.x, g = blockIdx.z;
+  hidden += (size_t)g * Tc * D;
+  if (out_f32) out_f32 += (size_t)g * B * R * D;
+  if (out_nhwc) out_nhwc += (size_t)g * B * D * R;
   const int center = (int)(((float)b + start) * mult);
   const int left = (int)((float)center - (float)win_l * mult);
   const int row = min(max(left + r, 0), T - 1);
@@ -131,10 +150,11 @@ __global__ void __launch_bounds__(256) hubert_slice_kernel(const __half* __restr
   }
 }
 
-cudaError_t launch_hubert_slice(const __half* hidden, int Tc, int T, int D, int B, int R, float start, float mult, int win_l, float* out_f32,
-                                __half* out_nhwc, cudaStream_t st) {
-  if (T < 1 || Tc < 1) return cudaErrorInvalidValue;
-  return launch_kernel_plain(hubert_slice_kernel, dim3(dim3(R, B)), dim3(256), 0, st, hidden, Tc, T, D, B, R, start, mult, win_l, out_f32, out_nhwc);
+cudaError_t launch_hubert_slice(const __half* hidden, int G, int Tc, int T, int D, int B, int R, float start, float mult, int win_l,
+                                float* out_f32, __half* out_nhwc, cudaStream_t st) {
+  if (T < 1 || Tc < 1 || G < 1 || G > 65535) return cudaErrorInvalidValue;
+  return launch_kernel_plain(hubert_slice_kernel, dim3(R, B, G), dim3(256), 0, st, hidden, Tc, T, D, B, R, start, mult, win_l, out_f32,
+                             out_nhwc);
 }
 
 }  // namespace ltb

@@ -50,11 +50,13 @@ cudaError_t launch_upsample_bilinear2x(const __half* x, int N, int H, int W, int
 cudaError_t launch_ul_prep(const uint8_t* faces, int nf, const int* d_index, int B, __half* out, cudaStream_t st);
 cudaError_t launch_ul_paste(const uint8_t* frames, const uint8_t* faces, const int* coords, const float* pred, uint8_t* out, int nf, int H, int W,
                             int index, int explicit_idx, int slot0, int count, cudaStream_t st);
-cudaError_t launch_hubert_conv0(const float* pcm, int n, const float* w, const float* bias, int C, float* stats, __half* out, cudaStream_t st);
-cudaError_t launch_hubert_pos_conv(const __half* h, int T, int D, int groups, int K, const __half* w, const float* bias, __half* out,
+// HuBERT ops over G sequences stacked on the row dimension (G = 1: one window)
+cudaError_t launch_hubert_conv0(const float* pcm, int G, int n, const float* w, const float* bias, int C, float* stats, __half* out,
+                                cudaStream_t st);
+cudaError_t launch_hubert_pos_conv(const __half* h, int G, int T, int D, int groups, int K, const __half* w, const float* bias, __half* out,
                                    cudaStream_t st);
-cudaError_t launch_hubert_slice(const __half* hidden, int Tc, int T, int D, int B, int R, float start, float mult, int win_l, float* out_f32,
-                                __half* out_nhwc, cudaStream_t st);
+cudaError_t launch_hubert_slice(const __half* hidden, int G, int Tc, int T, int D, int B, int R, float start, float mult, int win_l,
+                                float* out_f32, __half* out_nhwc, cudaStream_t st);
 cudaError_t launch_vae_post(const __half* x, size_t npix, int Ctot, uint8_t* out, cudaStream_t st);
 // uint8 BGR [N,H,W,3] -> planar I420 [N, H*3/2, W] (OpenCV COLOR_BGR2YUV_I420 arithmetic); H even, W % 4 == 0
 cudaError_t launch_bgr_to_i420(const uint8_t* bgr, int N, int H, int W, uint8_t* out, cudaStream_t st);

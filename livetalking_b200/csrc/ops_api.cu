@@ -448,30 +448,43 @@ int ltb_op_ul_paste(ltb_ctx* c, const void* frames, const void* faces, const voi
   c->launches += 1;
   return 0;
 }
-int ltb_op_hubert_conv0(ltb_ctx* c, const float* pcm, int n, const float* w, const float* bias, int C, float* stats, void* out) {
+int ltb_op_hubert_conv0_grouped(ltb_ctx* c, const float* pcm, int G, int n, const float* w, const float* bias, int C, float* stats, void* out) {
   if (!c || !pcm || !w || !stats || !out) return LTB_FAIL("hubert_conv0: null argument");
   LTB_CTX_ENTER(c);
-  cudaError_t e = launch_hubert_conv0(pcm, n, w, bias, C, stats, static_cast<__half*>(out), c->st);
-  if (e != cudaSuccess) return LTB_FAIL(std::string("hubert_conv0: ") + cudaGetErrorString(e));
+  cudaError_t e = launch_hubert_conv0(pcm, G, n, w, bias, C, stats, static_cast<__half*>(out), c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("hubert_conv0 (n >= 10, 1 <= G <= 65535): ") + cudaGetErrorString(e));
   c->launches += 2;
   return 0;
 }
-int ltb_op_hubert_pos_conv(ltb_ctx* c, const void* h, int T, int D, int groups, int K, const void* w, const float* bias, void* out) {
+int ltb_op_hubert_conv0(ltb_ctx* c, const float* pcm, int n, const float* w, const float* bias, int C, float* stats, void* out) {
+  return ltb_op_hubert_conv0_grouped(c, pcm, 1, n, w, bias, C, stats, out);
+}
+int ltb_op_hubert_pos_conv_grouped(ltb_ctx* c, const void* h, int G, int T, int D, int groups, int K, const void* w, const float* bias, void* out) {
   if (!c || !h || !w || !bias || !out) return LTB_FAIL("hubert_pos_conv: null argument");
   LTB_CTX_ENTER(c);
-  cudaError_t e = launch_hubert_pos_conv(static_cast<const __half*>(h), T, D, groups, K, static_cast<const __half*>(w), bias, static_cast<__half*>(out), c->st);
-  if (e != cudaSuccess) return LTB_FAIL(std::string("hubert_pos_conv (K = 128, D / groups = 64, out != h): ") + cudaGetErrorString(e));
+  cudaError_t e = launch_hubert_pos_conv(static_cast<const __half*>(h), G, T, D, groups, K, static_cast<const __half*>(w), bias,
+                                         static_cast<__half*>(out), c->st);
+  if (e != cudaSuccess)
+    return LTB_FAIL(std::string("hubert_pos_conv (K = 128, D / groups = 64, out != h, 1 <= G <= 65535): ") + cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
+int ltb_op_hubert_pos_conv(ltb_ctx* c, const void* h, int T, int D, int groups, int K, const void* w, const float* bias, void* out) {
+  return ltb_op_hubert_pos_conv_grouped(c, h, 1, T, D, groups, K, w, bias, out);
+}
+int ltb_op_hubert_slice_grouped(ltb_ctx* c, const void* hidden, int G, int Tc, int T, int D, int B, int R, float start, float mult, int win_l,
+                                float* out_f32, void* out_nhwc) {
+  if (!c || !hidden || (!out_f32 && !out_nhwc)) return LTB_FAIL("hubert_slice: null argument");
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_hubert_slice(static_cast<const __half*>(hidden), G, Tc, T, D, B, R, start, mult, win_l, out_f32,
+                                      static_cast<__half*>(out_nhwc), c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("hubert_slice: ") + cudaGetErrorString(e));
   c->launches += 1;
   return 0;
 }
 int ltb_op_hubert_slice(ltb_ctx* c, const void* hidden, int Tc, int T, int D, int B, int R, float start, float mult, int win_l, float* out_f32,
                         void* out_nhwc) {
-  if (!c || !hidden || (!out_f32 && !out_nhwc)) return LTB_FAIL("hubert_slice: null argument");
-  LTB_CTX_ENTER(c);
-  cudaError_t e = launch_hubert_slice(static_cast<const __half*>(hidden), Tc, T, D, B, R, start, mult, win_l, out_f32, static_cast<__half*>(out_nhwc), c->st);
-  if (e != cudaSuccess) return LTB_FAIL(std::string("hubert_slice: ") + cudaGetErrorString(e));
-  c->launches += 1;
-  return 0;
+  return ltb_op_hubert_slice_grouped(c, hidden, 1, Tc, T, D, B, R, start, mult, win_l, out_f32, out_nhwc);
 }
 int ltb_op_vae_post(ltb_ctx* c, const void* x, long long npix, int Ctot, void* out_u8) {
   if (!c || !x || !out_u8) return LTB_FAIL("vae_post: null argument");

@@ -5,10 +5,12 @@
 Weights come from the HF ``HubertModel`` state_dict of the checkpoint the reference loads (hubert-large-ls960-ft: 7 conv layers with
 per-layer LayerNorm and bias, 1024-d stable-LayerNorm transformer, 16-group positional conv with weight norm).  Conv layers 1-6, the
 projections, attention and MLPs run on the tcgen05 conv / fused-attention kernels; conv layer 0 (+ the processor's utterance
-normalisation), the grouped positional conv and the window gather are csrc/hubert.cu.  One CUDA graph per extractor."""
+normalisation), the grouped positional conv and the window gather are csrc/hubert.cu.  One CUDA graph per extractor.
+
+``HubertBatchFeatures`` is the cross-session form: G sessions' windows stacked on the row dimension, one encoder forward for all."""
 from __future__ import annotations
 
-from typing import Dict, Optional
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
@@ -93,50 +95,62 @@ class HubertEncoder:
     def emit(self, b: Builder, pcm: DevTensor, n: int, stats: DevTensor) -> DevTensor:
         """pcm: float32 [n] raw 16 kHz samples -> last_hidden_state (conv_frames(n), D) fp16 (HubertModel.forward on the
         processor-normalised input; stable-LayerNorm encoder: hidden += pos_conv(hidden); pre-LN layers; final LayerNorm)."""
+        return self.emit_grouped(b, pcm, 1, n, stats)
+
+    def emit_grouped(self, b: Builder, pcm: DevTensor, G: int, n: int, stats: DevTensor) -> DevTensor:
+        """emit() for G windows at once: pcm float32 [G][n], stats [G][4] -> (G * conv_frames(n), D) fp16, window g in rows
+        [g*T, (g+1)*T).  Each window is normalised with its own statistics, the conv stack runs with N = G images, row-wise ops
+        run over G*T rows and attention with batch G, so no window sees another's samples or keys."""
         ctx, C, D = b.ctx, self.C, self.D
         T = (n - CONV_KERNEL[0]) // CONV_STRIDE[0] + 1
-        h = b.new(1, 1, T, C)
-        ctx.hubert_conv0(pcm, n, self.conv0_w, self.conv0_b, C, stats, h)
+        h = b.new(G, 1, T, C)
+        ctx.hubert_conv0(pcm, n, self.conv0_w, self.conv0_b, C, stats, h, G=G)
         for i in range(7):
             if i > 0:
                 k, s = CONV_KERNEL[i], CONV_STRIDE[i]
                 T2 = (T - k) // s + 1
-                h2 = b.new(1, 1, T2, C)
-                ctx.conv(h, self.convs[i - 1], h2, N=1, IH=1, IW=T, OH=1, OW=T2, stride=(1, s), pad=(0, 0))
+                h2 = b.new(G, 1, T2, C)
+                ctx.conv(h, self.convs[i - 1], h2, N=G, IH=1, IW=T, OH=1, OW=T2, stride=(1, s), pad=(0, 0))
                 h, T = h2, T2
-            y = b.new(1, 1, T, C)
-            ctx.layernorm(h, T, C, self.eps, self.conv_ln[i].gamma, self.conv_ln[i].beta, y)      # HubertLayerNormConvLayer
-            ctx.eltwise(y, None, T * C, 8, 1, y)                                                  # GELU
+            y = b.new(G, 1, T, C)
+            ctx.layernorm(h, G * T, C, self.eps, self.conv_ln[i].gamma, self.conv_ln[i].beta, y)  # HubertLayerNormConvLayer
+            ctx.eltwise(y, None, G * T * C, 8, 1, y)                                              # GELU
             h = y
-        x = DevTensor(h.ptr, (T, C))
+        x = DevTensor(h.ptr, (G * T, C))
         x = b.linear(b.layernorm(x, self.proj_ln, self.eps), self.proj)                           # HubertFeatureProjection
-        xp = b.new(T, D)
-        ctx.hubert_pos_conv(x, T, D, POS_GROUPS, POS_K, self.pos_w, self.pos_b, xp)               # + positional conv embedding
+        xp = b.new(G * T, D)
+        ctx.hubert_pos_conv(x, T, D, POS_GROUPS, POS_K, self.pos_w, self.pos_b, xp, G=G)          # + positional conv embedding
         x = xp
         for L in self.layers:                                                                     # HubertEncoderLayerStableLayerNorm
-            x = b.attention(L["attn"], b.layernorm(x, L["ln1"], self.eps), 1, T, res=x)
+            x = b.attention(L["attn"], b.layernorm(x, L["ln1"], self.eps), G, T, res=x)
             f = b.linear(b.layernorm(x, L["ln2"], self.eps), L["fc1"])
             ctx.eltwise(f, None, f.rows * f.C, 8, 1, f)
             x = b.linear(f, L["fc2"], res=x)
         return b.layernorm(x, self.ln_post, self.eps)
 
 
+def window_samples(batch: int, stride_left: int, stride_right: int) -> tuple:
+    """HubertASR's window of (stride_left + stride_right + 2 * batch) 20 ms chunks -> (samples n, conv frames Tc, expected rows T).
+    Always below the reference's 320000-sample clip length, so the single-clip branch of audio2feature.py:38-47 applies."""
+    n = (stride_left + stride_right + 2 * int(batch)) * 320
+    if not 400 <= n < 320000:
+        raise ValueError("audio window must be 400 .. 319999 samples")
+    Tc, T = conv_frames(n), (n - 80) // 320
+    if abs(Tc - T) > 1:
+        raise ValueError("conv frame count and expected_T differ by more than one (audio2feature.py:52)")
+    return n, Tc, T
+
+
 class HubertFeatures:
     """get_hubert_from_16k_speech + HubertASR's window gather for one session: PCM buffer -> (B, 16, D) features, one CUDA graph.
-    The window is (stride_left + stride_right + 2 * batch) 20 ms chunks (HubertASR keeps exactly that many, hubert.py:30-48): always
-    below the reference's 320000-sample clip length, so the single-clip branch of audio2feature.py:38-47 applies."""
+    The window is (stride_left + stride_right + 2 * batch) 20 ms chunks (HubertASR keeps exactly that many, hubert.py:30-48)."""
 
     def __init__(self, enc: HubertEncoder, batch: int, stride_left: int = 10, stride_right: int = 10, out_nhwc: Optional[DevTensor] = None,
                  ctx: Optional[Ctx] = None):
         self.enc, self.B = enc, int(batch)
         self._own_ctx = ctx is None
         ctx = self.ctx = Ctx() if ctx is None else ctx
-        self.n = (stride_left + stride_right + 2 * self.B) * 320
-        if not 400 <= self.n < 320000:
-            raise ValueError("audio window must be 400 .. 319999 samples")
-        self.Tc, self.T = conv_frames(self.n), (self.n - 80) // 320
-        if abs(self.Tc - self.T) > 1:
-            raise ValueError("conv frame count and expected_T differ by more than one (audio2feature.py:52)")
+        self.n, self.Tc, self.T = window_samples(self.B, stride_left, stride_right)
         self.pcm = ctx.alloc((self.n,), np.float32, zero=True)
         self.stats = ctx.alloc((4,), np.float32, zero=True)
         self.out = ctx.alloc((self.B, ROWS, enc.D), np.float32, zero=True)
@@ -173,6 +187,78 @@ class HubertFeatures:
     def hidden_states(self) -> np.ndarray:
         with self.ctx.lock:
             return self.ctx.download(self.hidden)
+
+    def close(self):
+        if getattr(self, "graph", None) is not None:
+            self.graph.close()
+            self.graph = None
+        if self._own_ctx and self.ctx is not None:
+            self.ctx.close()
+        self.ctx = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class HubertBatchFeatures:
+    """HubertFeatures for up to G sessions at once: G PCM windows of the same layout -> G x (B, 16, D) features, ONE CUDA graph of
+    one encoder forward over the G windows stacked on the row dimension (HubertEncoder.emit_grouped).  At B = 16 a window is ~51
+    tokens, under half of one 128-row GEMM tile, and every window re-reads the encoder's weights: G windows per forward share
+    both.  Each window keeps its own normalisation statistics, positional-conv padding and attention keys, so a session's features do
+    not depend on which other windows share its round.  A call with k < G windows is a partial round: groups [k, G) keep their
+    last window (zeros before the first call) and their output is not read.  `batch` / `infer_slots` make it a mux for
+    plugin.batcher.CrossSessionBatcher (a request is one session's PCM window)."""
+
+    def __init__(self, enc: HubertEncoder, batch: int, groups: int, stride_left: int = 10, stride_right: int = 10,
+                 ctx: Optional[Ctx] = None):
+        self.enc, self.B, self.G = enc, int(batch), int(groups)
+        if self.G < 1:
+            raise ValueError("groups must be >= 1")
+        self.batch = self.G                                  # CrossSessionBatcher: requests per engine call
+        self._own_ctx = ctx is None
+        ctx = self.ctx = Ctx() if ctx is None else ctx
+        self.n, self.Tc, self.T = window_samples(self.B, stride_left, stride_right)
+        self.pcm = ctx.alloc((self.G, self.n), np.float32, zero=True)
+        self.stats = ctx.alloc((self.G, 4), np.float32, zero=True)
+        self.out = ctx.alloc((self.G, self.B, ROWS, enc.D), np.float32, zero=True)
+        self.start = stride_left / 2.0
+        self.builder = Builder(ctx)
+
+        def emit():
+            self.hidden = enc.emit_grouped(self.builder, self.pcm, self.G, self.n, self.stats)
+            ctx.hubert_slice(self.hidden, self.Tc, self.T, enc.D, self.B, ROWS, self.start, 2.0, WIN[0], self.out, None, G=self.G)
+
+        emit()
+        ctx.sync()
+        temps, self.builder.temps = self.builder.temps, []
+        self.builder.new = _Replay(temps)
+        with ctx.capture() as cap:
+            emit()
+        self.graph = cap.graph
+
+    def run_async(self, pcms: Sequence[np.ndarray]) -> int:
+        """Stage windows 0 .. k-1 and launch the graph; -> k."""
+        k = len(pcms)
+        if not 1 <= k <= self.G:
+            raise ValueError(f"1..{self.G} windows per call, got {k}")
+        x = np.stack([np.ascontiguousarray(p, np.float32).reshape(-1) for p in pcms])
+        if x.shape[1] != self.n:
+            raise ValueError(f"expected windows of {self.n} samples, got {x.shape[1]}")
+        self.ctx.h2d(DevTensor(self.pcm.ptr, (k, self.n), np.float32), x, sync=False)
+        self.graph.launch()
+        return k
+
+    def run_groups(self, pcms: Sequence[np.ndarray]) -> List[np.ndarray]:
+        """-> per window its (B, 16, D) float32 features: what HubertFeatures.run returns for that window alone."""
+        with self.ctx.lock:
+            k = self.run_async(pcms)
+            out = self.ctx.download(DevTensor(self.out.ptr, (k, self.B, ROWS, self.enc.D), np.float32))
+        return [out[g] for g in range(k)]
+
+    infer_slots = run_groups
 
     def close(self):
         if getattr(self, "graph", None) is not None:

@@ -206,8 +206,8 @@ class Builder:
         if a.self_attn:
             nk = _ceil16(nq)
             valid = nq
-            if nk != nq:
-                assert B == 1, "key padding of self-attention needs per-batch row padding"
+            # batch b's padded keys [nq, nk) are rows of batch b + 1 (the zero rows below for the last batch) on the unfused path and
+            # TMA zero fill on the fused one: both are masked to probability 0, and VT (transpose_heads) is zero for keys >= nq
             qkv = self.new(B * nq + (nk - nq), 3 * Hdp)                   # padded key rows stay zero
             self.linear(xq, a.qkv, out=DevTensor(qkv.ptr, (B * nq, 3 * Hdp)))
             q_ptr, q_pitch = qkv.ptr, 3 * Hdp

@@ -291,19 +291,22 @@ class Ctx:
         check(lib().ltb_op_ul_paste(self._h, C.c_void_p(frames.ptr), C.c_void_p(faces.ptr), C.c_void_p(coords.ptr), C.c_void_p(pred.ptr),
                                     C.c_void_p(out.ptr), nf, H, W, index, explicit_idx, slot0, count))
 
-    def hubert_conv0(self, pcm: DevTensor, n: int, w: DevTensor, bias: Optional[DevTensor], Cc: int, stats: DevTensor, out: DevTensor):
-        check(lib().ltb_op_hubert_conv0(self._h, C.c_void_p(pcm.ptr), n, C.c_void_p(w.ptr), C.c_void_p(bias.ptr) if bias is not None else None,
-                                        Cc, C.c_void_p(stats.ptr), C.c_void_p(out.ptr)))
+    # HuBERT ops over G windows stacked on the row dimension; each window is normalised, padded and gathered on its own
+    def hubert_conv0(self, pcm: DevTensor, n: int, w: DevTensor, bias: Optional[DevTensor], Cc: int, stats: DevTensor, out: DevTensor,
+                     G: int = 1):
+        check(lib().ltb_op_hubert_conv0_grouped(self._h, C.c_void_p(pcm.ptr), G, n, C.c_void_p(w.ptr),
+                                                C.c_void_p(bias.ptr) if bias is not None else None, Cc, C.c_void_p(stats.ptr),
+                                                C.c_void_p(out.ptr)))
 
-    def hubert_pos_conv(self, h: DevTensor, T: int, D: int, groups: int, K: int, w: DevTensor, bias: DevTensor, out: DevTensor):
-        check(lib().ltb_op_hubert_pos_conv(self._h, C.c_void_p(h.ptr), T, D, groups, K, C.c_void_p(w.ptr), C.c_void_p(bias.ptr),
-                                           C.c_void_p(out.ptr)))
+    def hubert_pos_conv(self, h: DevTensor, T: int, D: int, groups: int, K: int, w: DevTensor, bias: DevTensor, out: DevTensor, G: int = 1):
+        check(lib().ltb_op_hubert_pos_conv_grouped(self._h, C.c_void_p(h.ptr), G, T, D, groups, K, C.c_void_p(w.ptr), C.c_void_p(bias.ptr),
+                                                   C.c_void_p(out.ptr)))
 
     def hubert_slice(self, hidden: DevTensor, Tc: int, T: int, D: int, B: int, R: int, start: float, mult: float, win_l: int,
-                     out_f32: Optional[DevTensor], out_nhwc: Optional[DevTensor]):
-        check(lib().ltb_op_hubert_slice(self._h, C.c_void_p(hidden.ptr), Tc, T, D, B, R, float(start), float(mult), win_l,
-                                        C.c_void_p(out_f32.ptr) if out_f32 is not None else None,
-                                        C.c_void_p(out_nhwc.ptr) if out_nhwc is not None else None))
+                     out_f32: Optional[DevTensor], out_nhwc: Optional[DevTensor], G: int = 1):
+        check(lib().ltb_op_hubert_slice_grouped(self._h, C.c_void_p(hidden.ptr), G, Tc, T, D, B, R, float(start), float(mult), win_l,
+                                                C.c_void_p(out_f32.ptr) if out_f32 is not None else None,
+                                                C.c_void_p(out_nhwc.ptr) if out_nhwc is not None else None))
 
     def bgr_to_i420(self, frames_u8: DevTensor, N: int, H: int, W: int, out_u8: DevTensor):
         """uint8 BGR [N,H,W,3] -> planar I420 [N, H*3/2, W] (encoder hand-off; cv2.COLOR_BGR2YUV_I420 arithmetic)."""

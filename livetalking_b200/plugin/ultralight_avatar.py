@@ -11,8 +11,10 @@ already hold the composited frames; ``paste_back_frame`` hands the matching one 
 reference's exact data flow (float32 (B,160,160,3) predictions x 255, pasted per frame from the host).
 
 Cross-session mode (``opt.ltb_cross_session`` / ``LTB_CROSS_SESSION=1``): ``inference_batch`` submits one group request to a shared
-``UltraLightBatchSession`` (``LTB_UL_GROUPS`` sessions per launch, default 4, with a bank of twice as many avatar networks); the
-session keeps its own HuBERT extractor and render threads and only a paste-back context of its own."""
+``UltraLightBatchSession`` (``LTB_UL_GROUPS`` sessions per launch, default 4, with a bank of twice as many avatar networks), and
+``HubertASR.run_step`` submits its PCM window as one group request to a shared ``HubertBatchFeatures`` (up to ``LTB_UL_GROUPS``
+windows per encoder forward).  Both schedulers dispatch a round when it is full or its oldest request is ``LTB_MUX_WAIT_MS`` old.
+The session keeps its render threads and only a paste-back context of its own."""
 from __future__ import annotations
 
 import glob
@@ -23,7 +25,7 @@ import threading
 import numpy as np
 
 from .. import engine
-from ..hubert import HubertEncoder, HubertFeatures
+from ..hubert import HubertBatchFeatures, HubertEncoder, HubertFeatures
 from ..ops import Ctx
 from ..ultralight import FACE, UltraLightAvatar, UltraLightBatchSession, UltraLightModel, UltraLightSession
 from .batcher import CrossSessionBatcher
@@ -118,6 +120,35 @@ def shared_batcher(audio: EngineAudio, template: UltraLightModel, frames_per_ses
         return table[key]
 
 
+def shared_feature_batcher(audio: EngineAudio, batch: int, stride_left: int, stride_right: int) -> CrossSessionBatcher:
+    """Cross-session mode: one HuBERT scheduler per (HuBERT model, window layout), created by the first session that asks.  Its mux
+    is a HubertBatchFeatures of LTB_UL_GROUPS windows: sessions whose steps fall in the same round share one encoder forward."""
+    with _BATCHER_LOCK:
+        table = getattr(audio, "_ltb_feature_batchers", None)
+        if table is None:
+            table = audio._ltb_feature_batchers = {}
+        key = (int(batch), int(stride_left), int(stride_right))
+        if key not in table:
+            groups = int(os.environ.get("LTB_UL_GROUPS", "4"))
+            mux = HubertBatchFeatures(audio.encoder, batch, groups, stride_left, stride_right)
+            table[key] = CrossSessionBatcher(mux, float(os.environ.get("LTB_MUX_WAIT_MS", "4")))
+        return table[key]
+
+
+class SharedFeatures:
+    """HubertASR's extractor in cross-session mode: run(pcm) is one group request of the shared HuBERT scheduler and blocks until its
+    round is served.  The scheduler and its graph belong to the model, so close() releases nothing."""
+
+    def __init__(self, batcher: CrossSessionBatcher):
+        self.batcher = batcher
+
+    def run(self, pcm: np.ndarray) -> np.ndarray:
+        return self.batcher.submit([pcm])[0]
+
+    def close(self):
+        pass
+
+
 @register("avatar", "ultralight")
 class LightReal(BaseAvatar):
     def __init__(self, opt, model, avatar):
@@ -134,7 +165,11 @@ class LightReal(BaseAvatar):
         # every session owns its stream + scratch (two: U-Net graph, HuBERT graph); weights / avatar assets are shared.
         # Cross-session mode: the session keeps only a paste-back context, its U-Net pass runs in the shared batch.
         self.engine_session = UltraLightSession(eng_avatar, self.batch_size, paste_only=cross)
-        self.audio_processor = HubertFeatures(audio_processor.encoder, self.batch_size, opt.l, opt.r)
+        # cross-session mode shares one grouped HuBERT forward per round; a stand-in encoder (no device weights) keeps its own extractor
+        if cross and isinstance(audio_processor.encoder, HubertEncoder):
+            self.audio_processor = SharedFeatures(shared_feature_batcher(audio_processor, self.batch_size, opt.l, opt.r))
+        else:
+            self.audio_processor = HubertFeatures(audio_processor.encoder, self.batch_size, opt.l, opt.r)
         self.asr = HubertASR(opt, self, self.audio_processor, audio_feat_length=[4, 4])
         self.asr.warm_up()
         # page-locked output ring for the fused mode (a D2H into pageable memory runs at a few GB/s, pinned at PCIe speed); a buffer is
