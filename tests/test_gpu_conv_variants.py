@@ -17,15 +17,13 @@ and, where the ungrouped op on that group plans the same instance, bit for bit w
 The expected variants are those of the 132-SM H100 SXM.  test_variants_cover_every_compiled_instance (CPU) checks that VARIANTS
 lists exactly the instances in the built objects, so a new instance without a row fails the suite."""
 import os
-import re
-import shutil
-import subprocess
 import types
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
+from kernel_instances import compiled_instances
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 H100_SMS = 132
@@ -148,23 +146,9 @@ def _key_id(key):
 
 
 # ------------------------------------------------------------------------------------------------ completeness (CPU)
-def _instances(obj, kernel):
-    cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(cuobjdump):
-        pytest.skip("cuobjdump not available")
-    if not os.path.exists(obj):
-        pytest.skip("object file not kept")
-    sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
-    out = set()
-    for m in re.finditer(r"Function : _ZN3ltb\d+" + kernel + r"I((?:L[ib]\d+E)+)E", sass):
-        out.add(tuple(int(v) for _t, v in re.findall(r"L([ib])(\d+)E", m.group(1))))
-    return out
-
-
 def test_variants_cover_every_compiled_instance():
-    build = os.path.join(ROOT, "livetalking_b200", "build")
-    halo = _instances(os.path.join(build, "conv_halo.o"), "conv_halo_wgmma_kernel")
-    gather = _instances(os.path.join(build, "conv_gather.o"), "conv_gather_wgmma_kernel")
+    halo = compiled_instances("conv_halo.o", "conv_halo_wgmma_kernel")
+    gather = compiled_instances("conv_gather.o", "conv_gather_wgmma_kernel")
     compiled = {H(bn, ns, na, t, rc, bool(g)) for bn, ns, na, t, rc, g in halo} | {G(bn, kb, bool(g)) for bn, kb, g in gather}
     assert len(halo) == 28 and len(gather) == 24, (len(halo), len(gather))
     missing = sorted(map(_key_id, compiled - set(VARIANTS)))
