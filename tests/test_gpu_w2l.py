@@ -1,7 +1,7 @@
 """GPU parity tests proper: the CUDA wav2lip256 path (through the C ABI) against the CPU oracle.
 
-Bars: model forward PSNR >= 40 dB after the reference's own u8 truncation (north_star), per-layer relative error
-for localisation, mel within 1e-6 of the float64 oracle, paste-back bit-exact."""
+Bars: model forward PSNR >= 40 dB after the reference's own u8 truncation (north_star), mel within 1e-5 of the float64
+oracle, paste-back bit-exact.  Every layer on its own against float64: tests/test_gpu_w2l_layers.py."""
 import os
 import sys
 import zlib
@@ -40,31 +40,17 @@ def model(w2l_state_dict):
     m.close()
 
 
-def test_per_layer_parity_and_psnr(model, w2l_state_dict):
+def test_forward_psnr_against_oracle(model, w2l_state_dict):
+    """The whole forward against the CPU fp32 oracle run end to end.  Each layer is checked on its own against float64 in
+    tests/test_gpu_w2l_layers.py."""
     from livetalking_b200 import engine
     from oracle import wav2lip_ref as R
     B = 2
     mel, img = R.synth_inputs(B, seed=5)
-    taps = {}
-    ref = R.wav2lip_forward(w2l_state_dict, mel, img, taps)
+    ref = R.wav2lip_forward(w2l_state_dict, mel, img)
     av, _, _ = _avatar(_faces_from_inputs(img))
     s = engine.W2LSession(model, av, B, keep_layers=True)
     pred = s.infer(0, mel.numpy().reshape(B, 80, 16))
-    names = [p for p, _ in R.layer_list()]
-    report = []
-    for li, name in enumerate(names):
-        got = s.layer_output(li).astype(np.float32)
-        want = taps[name].permute(0, 2, 3, 1).numpy()
-        if li == 34:   # ConvT k4 output is stored [B,4,4,512] already
-            pass
-        assert got.shape == want.shape, (li, name, got.shape, want.shape)
-        assert np.isfinite(got).all(), (li, name)
-        rel = np.abs(got - want).max() / max(1e-6, np.abs(want).max())
-        mrel = np.abs(got - want).mean() / max(1e-6, np.abs(want).mean())
-        report.append((li, name, rel, mrel))
-    bad = [r for r in report if r[2] > 3e-2 or r[3] > 8e-3]
-    assert not bad, "layers out of tolerance (idx, name, max-rel, mean-rel): " + "; ".join(
-        f"{li}:{n}:{a:.4f}:{b:.5f}" for li, n, a, b in bad[:6])
     want = ref.permute(0, 2, 3, 1).numpy() * 255.0
     psnr = R.psnr_u8(pred.astype(np.uint8), want.astype(np.uint8))
     assert psnr >= 40.0, psnr
@@ -123,7 +109,7 @@ def test_full_batch16_properties(model, w2l_state_dict):
     s16 = engine.W2LSession(model, av, 16)
     p1 = s16.infer(4, melB)
     p2 = s16.infer(4, melB)
-    assert np.abs(p1 - p2).max() <= 1.0                 # replay-stable (split-K layers reduce with float atomics: last-bit jitter)
+    assert np.array_equal(p1, p2)                       # replay-stable: split-K partials go to per-split slices, summed in order
     s1 = engine.W2LSession(model, av, 1)
     for slot in (0, 5, 15):
         fidx = mirror_index(3, 4 + slot)
