@@ -335,6 +335,20 @@ typedef struct ltb_mt_paste_op {
 } ltb_mt_paste_op;
 int ltb_op_mt_paste(ltb_ctx* c, const ltb_mt_paste_op* d);
 
+/* S3FD face detector of the wav2lip avatar generator (avatars/wav2lip/genavatar.py -> face_detection/detection/sfd); the convolutions
+ * run on ltb_op_conv2d, these are the ops around them (livetalking_b200/s3fd.py).
+ * prep: u8 BGR [N,H,W,3] -> fp16 [N,H,W,16] = (R-104, G-117, B-123, 0 ...), exact. */
+int ltb_op_s3fd_prep(ltb_ctx* c, const void* bgr_u8, int N, int H, int W, void* out);
+/* F.max_pool2d(x, 2, 2) on fp16 NHWC [N,H,W,C] -> [N,H/2,W/2,C] (floor); C % 8 == 0 */
+int ltb_op_maxpool2x2(ltb_ctx* c, const void* x, int N, int H, int W, int C, void* out);
+/* L2Norm per pixel: out = x / (sqrt(sum_c x^2) + eps) * w[c] (fp32 arithmetic); C % 8 == 0, C <= 512; out may equal x */
+int ltb_op_l2norm(ltb_ctx* c, const void* x, long long npix, int C, const float* w, float eps, void* out);
+/* Per image: fp32 softmax face score of every anchor of the six heads (heads6: device pointers to [N][h][w][pitch] fp16, hw12: host
+ * (h, w) pairs; level 0 has 4 conf channels with max-out background, then 4 loc; the others 2 conf then 4 loc), the arg-max (ties:
+ * lowest anchor number, levels then rows then columns) and its decoded, clipped, truncated box.  out_i32 [N][6] = {score > thresh,
+ * x1, y1, x2, y2, anchor}, out_score [N] (both device). */
+int ltb_op_s3fd_select(ltb_ctx* c, const void* const* heads6, const int* hw12, int N, int pitch, float thresh, int* out_i32, float* out_score);
+
 #ifdef __cplusplus
 }
 #endif

@@ -155,6 +155,11 @@ _SIGS = {
     "ltb_op_whisper_slice": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p,
                                        C.c_int]),
     "ltb_op_mt_paste": (C.c_int, [C.c_void_p, C.POINTER(MtPasteOp)]),
+    "ltb_op_s3fd_prep": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "ltb_op_maxpool2x2": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "ltb_op_l2norm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_float, C.c_void_p]),
+    "ltb_op_s3fd_select": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.c_int, C.c_int, C.c_float, C.c_void_p,
+                                     C.c_void_p]),
     "ltb_conv2d_f16": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ltb_conv2d_f16_timed": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                        C.POINTER(C.c_float)]),

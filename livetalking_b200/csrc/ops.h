@@ -85,4 +85,17 @@ struct MtPasteArgs {
 };
 cudaError_t launch_mt_paste(const MtPasteArgs& a, int count, cudaStream_t st);
 
+// S3FD face detector glue (s3fd.cu)
+constexpr int kS3fdInC = 16;     // channels of the prepared image: RGB minus means, zero-padded (conv1_1 runs with Cin = 16)
+constexpr int kS3fdLevels = 6;
+struct S3fdHeads {               // the six fused conf + loc head outputs, [N][h][w][pitch] fp16 each
+  const __half* p[kS3fdLevels];
+  int h[kS3fdLevels], w[kS3fdLevels];
+  int pitch;
+};
+cudaError_t launch_s3fd_prep(const uint8_t* bgr, int N, int H, int W, __half* out, cudaStream_t st);
+cudaError_t launch_maxpool2x2(const __half* x, int N, int H, int W, int C, __half* out, cudaStream_t st);
+cudaError_t launch_l2norm_scale(const __half* x, long long npix, int C, const float* w, float eps, __half* out, cudaStream_t st);
+cudaError_t launch_s3fd_select(const S3fdHeads& heads, int N, float thresh, int* out_i, float* out_s, cudaStream_t st);
+
 }  // namespace ltb

@@ -512,6 +512,47 @@ int ltb_op_stamp_pixels(ltb_ctx* c, void* frames_u8, int N, int H, int W, const 
   c->launches += 1;
   return 0;
 }
+// ---- S3FD face detector glue (s3fd.cu)
+int ltb_op_s3fd_prep(ltb_ctx* c, const void* bgr_u8, int N, int H, int W, void* out) {
+  if (!c || !bgr_u8 || !out) return LTB_FAIL("s3fd_prep: null argument");
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_s3fd_prep(static_cast<const uint8_t*>(bgr_u8), N, H, W, static_cast<__half*>(out), c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("s3fd_prep (N, H, W > 0, 16-byte aligned output): ") + cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
+int ltb_op_maxpool2x2(ltb_ctx* c, const void* x, int N, int H, int W, int C, void* out) {
+  if (!c || !x || !out) return LTB_FAIL("maxpool2x2: null argument");
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_maxpool2x2(static_cast<const __half*>(x), N, H, W, C, static_cast<__half*>(out), c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("maxpool2x2 (H, W >= 2, C % 8 == 0, 16-byte aligned): ") + cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
+int ltb_op_l2norm(ltb_ctx* c, const void* x, long long npix, int C, const float* w, float eps, void* out) {
+  if (!c || !x || !w || !out) return LTB_FAIL("l2norm: null argument");
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_l2norm_scale(static_cast<const __half*>(x), npix, C, w, eps, static_cast<__half*>(out), c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("l2norm (C % 8 == 0, C <= 512, 16-byte aligned): ") + cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
+int ltb_op_s3fd_select(ltb_ctx* c, const void* const* heads6, const int* hw12, int N, int pitch, float thresh, int* out_i32, float* out_score) {
+  if (!c || !heads6 || !hw12 || !out_i32 || !out_score) return LTB_FAIL("s3fd_select: null argument");
+  if (pitch < 8 || (pitch & 7)) return LTB_FAIL("s3fd_select: the head pitch must be a multiple of 8");
+  LTB_CTX_ENTER(c);
+  S3fdHeads h;
+  for (int l = 0; l < kS3fdLevels; ++l) {
+    h.p[l] = static_cast<const __half*>(heads6[l]);
+    h.h[l] = hw12[2 * l];
+    h.w[l] = hw12[2 * l + 1];
+  }
+  h.pitch = pitch;
+  cudaError_t e = launch_s3fd_select(h, N, thresh, out_i32, out_score, c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("s3fd_select: ") + cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
 int ltb_op_vae_pre(ltb_ctx* c, const void* img_u8, int N, int H, int W, int half_mask, void* out) {
   if (!c || !img_u8 || !out) return LTB_FAIL("vae_pre: null argument");
   LTB_CTX_ENTER(c);

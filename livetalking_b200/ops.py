@@ -334,6 +334,23 @@ class Ctx:
     def mt_paste(self, op: MtPasteOp):
         check(lib().ltb_op_mt_paste(self._h, C.byref(op)))
 
+    # ---- S3FD face detector (livetalking_b200/s3fd.py)
+    def s3fd_prep(self, frames_u8: DevTensor, N: int, H: int, W: int, out: DevTensor):
+        """u8 BGR [N,H,W,3] -> fp16 [N,H,W,16]: R-104, G-117, B-123, then zeros."""
+        check(lib().ltb_op_s3fd_prep(self._h, C.c_void_p(frames_u8.ptr), N, H, W, C.c_void_p(out.ptr)))
+
+    def maxpool2x2(self, x: DevTensor, N: int, H: int, W: int, out: DevTensor):
+        check(lib().ltb_op_maxpool2x2(self._h, C.c_void_p(x.ptr), N, H, W, x.C, C.c_void_p(out.ptr)))
+
+    def l2norm(self, x: DevTensor, npix: int, w: DevTensor, eps: float, out: DevTensor):
+        check(lib().ltb_op_l2norm(self._h, C.c_void_p(x.ptr), npix, x.C, C.c_void_p(w.ptr), eps, C.c_void_p(out.ptr)))
+
+    def s3fd_select(self, heads: Sequence[DevTensor], N: int, thresh: float, out_i32: DevTensor, out_score: DevTensor):
+        """heads: six [N,h,w,pitch] fp16 maps (fused conf + loc); out_i32 [N,6] = found, x1, y1, x2, y2, anchor; out_score [N]."""
+        ptrs = (C.c_void_p * 6)(*[h.ptr for h in heads])
+        hw = (C.c_int * 12)(*[d for h in heads for d in h.shape[1:3]])
+        check(lib().ltb_op_s3fd_select(self._h, ptrs, hw, N, heads[0].pitch, thresh, C.c_void_p(out_i32.ptr), C.c_void_p(out_score.ptr)))
+
     def close(self):
         if self._h:
             lib().ltb_ctx_destroy(self._h)
