@@ -349,6 +349,16 @@ int ltb_op_l2norm(ltb_ctx* c, const void* x, long long npix, int C, const float*
  * x1, y1, x2, y2, anchor}, out_score [N] (both device). */
 int ltb_op_s3fd_select(ltb_ctx* c, const void* const* heads6, const int* hw12, int N, int pitch, float thresh, int* out_i32, float* out_score);
 
+/* PFLD_GhostOne landmark network of the UltraLight avatar generator (avatars/ultralight/genavatar.py -> face_detect_utils/get_landmark.py);
+ * the convolutions run on ltb_op_conv2d and ltb_op_dwconv3x3, these are the ops around them (livetalking_b200/pfld.py).
+ * prep: u8 BGR [N,H,W,3] -> fp16 [N,H,W,16] = (B/255, G/255, R/255, 0 ...), the fp32 quotient rounded to fp16 once. */
+int ltb_op_pfld_prep(ltb_ctx* c, const void* bgr_u8, int N, int H, int W, void* out);
+/* Per image: the fp32 average over the pixels of each of five fp16 taps (taps5: device pointers to [N][hw5[k]][pitch5[k]]; their
+ * nch5[k] real channels, host list ch, concatenated in tap order), then out = wt^T feat + bias (wt: fp32 [nfeat][nout], device),
+ * + mean, times crop_wh[n][k & 1] (device int32 [N][2] = w, h): out_f32 [N][nout] and its truncation out_i32 [N][nout] (device). */
+int ltb_op_pfld_head(ltb_ctx* c, const void* const* taps5, const int* hw5, const int* pitch5, const int* nch5, const int* ch, int N,
+                     const float* wt, const float* bias, const float* mean, const int* crop_wh, int nout, float* out_f32, int* out_i32);
+
 #ifdef __cplusplus
 }
 #endif

@@ -160,6 +160,10 @@ _SIGS = {
     "ltb_op_l2norm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_float, C.c_void_p]),
     "ltb_op_s3fd_select": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.c_int, C.c_int, C.c_float, C.c_void_p,
                                      C.c_void_p]),
+    "ltb_op_pfld_prep": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "ltb_op_pfld_head": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                   C.POINTER(C.c_int), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                   C.c_void_p]),
     "ltb_conv2d_f16": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ltb_conv2d_f16_timed": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                        C.POINTER(C.c_float)]),

@@ -98,4 +98,18 @@ cudaError_t launch_maxpool2x2(const __half* x, int N, int H, int W, int C, __hal
 cudaError_t launch_l2norm_scale(const __half* x, long long npix, int C, const float* w, float eps, __half* out, cudaStream_t st);
 cudaError_t launch_s3fd_select(const S3fdHeads& heads, int N, float thresh, int* out_i, float* out_s, cudaStream_t st);
 
+// PFLD landmark network glue (pfld.cu)
+constexpr int kPfldInC = 16;       // channels of the prepared crop: BGR / 255, zero-padded (conv1 runs with Cin = 16)
+constexpr int kPfldTaps = 5;       // x1..x4 (global average pools) and x5 (conv8, 1 x 1)
+constexpr int kPfldMaxPitch = 256;
+constexpr int kPfldMaxFeat = 256;
+struct PfldTaps {                  // tap t: [N][hw[t]][pitch[t]] fp16; its nch[t] real channels are listed in ch, taps in order
+  const __half* p[kPfldTaps];
+  int hw[kPfldTaps], pitch[kPfldTaps], nch[kPfldTaps];
+  unsigned char ch[kPfldMaxFeat];
+};
+cudaError_t launch_pfld_prep(const uint8_t* bgr, int N, int H, int W, __half* out, cudaStream_t st);
+cudaError_t launch_pfld_head(const PfldTaps& taps, int N, const float* wt, const float* bias, const float* mean, const int* crop_wh, int nout,
+                             float* out_f, int* out_i, cudaStream_t st);
+
 }  // namespace ltb

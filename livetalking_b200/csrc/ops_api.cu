@@ -553,6 +553,41 @@ int ltb_op_s3fd_select(ltb_ctx* c, const void* const* heads6, const int* hw12, i
   c->launches += 1;
   return 0;
 }
+// ---- PFLD landmark network glue (pfld.cu)
+int ltb_op_pfld_prep(ltb_ctx* c, const void* bgr_u8, int N, int H, int W, void* out) {
+  if (!c || !bgr_u8 || !out) return LTB_FAIL("pfld_prep: null argument");
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_pfld_prep(static_cast<const uint8_t*>(bgr_u8), N, H, W, static_cast<__half*>(out), c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("pfld_prep (N, H, W > 0, 16-byte aligned output): ") + cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
+int ltb_op_pfld_head(ltb_ctx* c, const void* const* taps5, const int* hw5, const int* pitch5, const int* nch5, const int* ch, int N,
+                     const float* wt, const float* bias, const float* mean, const int* crop_wh, int nout, float* out_f32, int* out_i32) {
+  if (!c || !taps5 || !hw5 || !pitch5 || !nch5 || !ch || !wt || !bias || !mean || !crop_wh || !out_f32 || !out_i32)
+    return LTB_FAIL("pfld_head: null argument");
+  PfldTaps t{};
+  int nfeat = 0;
+  for (int k = 0; k < kPfldTaps; ++k) {
+    t.p[k] = static_cast<const __half*>(taps5[k]);
+    t.hw[k] = hw5[k];
+    t.pitch[k] = pitch5[k];
+    t.nch[k] = nch5[k];
+    if (nch5[k] < 0 || nch5[k] > kPfldMaxFeat - nfeat) return LTB_FAIL("pfld_head: more than 256 features");
+    nfeat += nch5[k];
+  }
+  for (int j = 0; j < nfeat; ++j) {
+    if (ch[j] < 0 || ch[j] >= kPfldMaxPitch) return LTB_FAIL("pfld_head: channel index outside the pitch");
+    t.ch[j] = (unsigned char)ch[j];
+  }
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_pfld_head(t, N, wt, bias, mean, crop_wh, nout, out_f32, out_i32, c->st);
+  if (e != cudaSuccess)
+    return LTB_FAIL(std::string("pfld_head (pitch % 8 == 0 and <= 256, channels inside the pitch, 16-byte aligned taps, even nout <= 512): ") +
+                    cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
 int ltb_op_vae_pre(ltb_ctx* c, const void* img_u8, int N, int H, int W, int half_mask, void* out) {
   if (!c || !img_u8 || !out) return LTB_FAIL("vae_pre: null argument");
   LTB_CTX_ENTER(c);

@@ -351,6 +351,24 @@ class Ctx:
         hw = (C.c_int * 12)(*[d for h in heads for d in h.shape[1:3]])
         check(lib().ltb_op_s3fd_select(self._h, ptrs, hw, N, heads[0].pitch, thresh, C.c_void_p(out_i32.ptr), C.c_void_p(out_score.ptr)))
 
+    # ---- PFLD landmark network (livetalking_b200/pfld.py)
+    def pfld_prep(self, crops_u8: DevTensor, N: int, H: int, W: int, out: DevTensor):
+        """u8 BGR [N,H,W,3] -> fp16 [N,H,W,16]: B/255, G/255, R/255, then zeros."""
+        check(lib().ltb_op_pfld_prep(self._h, C.c_void_p(crops_u8.ptr), N, H, W, C.c_void_p(out.ptr)))
+
+    def pfld_head(self, taps: Sequence[DevTensor], chans: Sequence[Sequence[int]], N: int, wt: DevTensor, bias: DevTensor,
+                  mean: DevTensor, crop_wh: DevTensor, out_f32: DevTensor, out_i32: DevTensor):
+        """taps: five [N, ..., pitch] fp16 maps, chans[k] the real channels of tap k; wt fp32 [nfeat][nout]; crop_wh int32 [N,2];
+        out_f32 / out_i32 [N, nout] = (wt^T avg + bias + mean) * (w, h, w, h, ...) and its truncation."""
+        ptrs = (C.c_void_p * 5)(*[t.ptr for t in taps])
+        hw = (C.c_int * 5)(*[int(np.prod(t.shape[1:-1])) for t in taps])
+        pitch = (C.c_int * 5)(*[t.pitch for t in taps])
+        nch = (C.c_int * 5)(*[len(c) for c in chans])
+        flat = [int(c) for cs in chans for c in cs]
+        ch = (C.c_int * max(1, len(flat)))(*flat)
+        check(lib().ltb_op_pfld_head(self._h, ptrs, hw, pitch, nch, ch, N, C.c_void_p(wt.ptr), C.c_void_p(bias.ptr), C.c_void_p(mean.ptr),
+                                     C.c_void_p(crop_wh.ptr), int(bias.shape[0]), C.c_void_p(out_f32.ptr), C.c_void_p(out_i32.ptr)))
+
     def close(self):
         if self._h:
             lib().ltb_ctx_destroy(self._h)
