@@ -78,46 +78,54 @@ struct HaloCfg {
   static_assert(SMEM_BYTES + 3584 <= 227 * 1024, "shared memory overflow (dynamic + static)");
 };
 
-// Sub-pixel layers ("fat-N" issue): the (phase, tap) weight slices are stored view-major so that ONE wgmma per halo view
-// feeds every phase accumulator that reads it.  Accumulator slots are ordered p0, p1, p3, p2 (phase = oy*2 + ox) so that
-// slots sharing a view are adjacent.  {weight stage, halo view (row offset), first slot, first weight slice, slots}
-struct FatMma {
+// Sub-pixel layers: the (phase, tap) weight slices are stored view-major, the slices that read one halo view adjacent in their
+// weight stage.  Accumulator slots are ordered p0, p1, p3, p2 (phase = oy*2 + ox).  Each slice is one N = BN wgmma into its
+// slot's BN accumulator columns: every MMA writes a register range of the same shape that is either identical to or disjoint
+// from any other's, so the MMAs of a whole K chunk chain without waits, like the taps of the 3x3 path.  (One wider wgmma per
+// view over its adjacent slots reads each view once, but wgmmas of different N into overlapping columns must not be in flight
+// together: that issue drained the tensor pipe after every view and ran the wav2lip ConvTs 2-4.5x slower, DESIGN.md.)
+// {weight stage, halo view (row offset), first slot, first weight slice, slots}
+struct SubpixelView {
   int stage, view, slot0, brow, nslots;
 };
-constexpr int fat_view(int vy, int vx) { return (vy + 1) * kHaloP + (vx + 1); }
+constexpr int subpixel_view(int vy, int vx) { return (vy + 1) * kHaloP + (vx + 1); }
 template <int TAPS>
-struct FatTable;
+struct SubpixelTable;
 // ConvT(k3, s2): stage 0: v00->p0,p1,p3 | stage 1: v01->p1,p3 ; v11->p3 | stage 2: v00->p2 ; v10->p3,p2  (ConvT halos start at the
 // tile origin: view = dy*10 + dx)
 template <>
-struct FatTable<9> {
-  static constexpr int NG = 5;
-  static constexpr FatMma g[NG] = {{0, 0, 0, 0, 3}, {1, 1, 1, 0, 2}, {1, kHaloP + 1, 2, 2, 1}, {2, 0, 3, 2, 1}, {2, kHaloP, 2, 0, 2}};
+struct SubpixelTable<9> {
+  static constexpr int NV = 5;
+  static constexpr SubpixelView v[NV] = {{0, 0, 0, 0, 3}, {1, 1, 1, 0, 2}, {1, kHaloP + 1, 2, 2, 1}, {2, 0, 3, 2, 1}, {2, kHaloP, 2, 0, 2}};
 };
 // Upsample(nearest 2x) + conv3x3: output phase (a, b) = 2x2 conv over the low-res halo, 16 (phase, view) slices in 4 stages
 template <>
-struct FatTable<16> {
-  static constexpr int NG = 10;
-  static constexpr FatMma g[NG] = {{0, fat_view(0, 0), 0, 0, 4},
-                                   {1, fat_view(-1, 0), 0, 0, 2},  {1, fat_view(0, 1), 1, 2, 2},
-                                   {2, fat_view(1, 0), 2, 0, 2},   {2, fat_view(0, -1), 0, 2, 1}, {2, fat_view(0, -1), 3, 3, 1},
-                                   {3, fat_view(-1, -1), 0, 0, 1}, {3, fat_view(-1, 1), 1, 1, 1}, {3, fat_view(1, 1), 2, 2, 1},
-                                   {3, fat_view(1, -1), 3, 3, 1}};
+struct SubpixelTable<16> {
+  static constexpr int NV = 10;
+  static constexpr SubpixelView v[NV] = {{0, subpixel_view(0, 0), 0, 0, 4},
+                                         {1, subpixel_view(-1, 0), 0, 0, 2},  {1, subpixel_view(0, 1), 1, 2, 2},
+                                         {2, subpixel_view(1, 0), 2, 0, 2},   {2, subpixel_view(0, -1), 0, 2, 1}, {2, subpixel_view(0, -1), 3, 3, 1},
+                                         {3, subpixel_view(-1, -1), 0, 0, 1}, {3, subpixel_view(-1, 1), 1, 1, 1}, {3, subpixel_view(1, 1), 2, 2, 1},
+                                         {3, subpixel_view(1, -1), 3, 3, 1}};
 };
 
-template <int BN, int TAPS, int R, size_t... G>
-__device__ __forceinline__ void fat_issue(float (&acc)[R], int j, int k, uint32_t a_lo0, uint32_t b_lo0, uint32_t a_hi, uint32_t b_hi,
-                                          std::index_sequence<G...>) {
+// one view: weight slices BROW.. into accumulator slots SLOT0.., one N = BN wgmma each
+template <int BN, int SLOT0, int BROW, int R, size_t... S>
+__device__ __forceinline__ void subpixel_slots(float (&acc)[R], uint64_t a, uint32_t b_lo, uint32_t b_hi, std::index_sequence<S...>) {
+  (wgmma_ss_at<BN, (SLOT0 + (int)S) * BN>(acc, a, wgmma_lohi(b_lo + (BROW + (uint32_t)S) * BN * 8u, b_hi), 1u), ...);
+}
+
+// the MMAs of weight stage j, K step k, views in table order.  j must be a compile-time constant after unrolling: the stage
+// select then folds away and no branch sits between the MMAs.
+template <int BN, int TAPS, int R, size_t... V>
+__device__ __forceinline__ void subpixel_issue(float (&acc)[R], int j, int k, uint32_t a_lo0, uint32_t b_lo0, uint32_t a_hi, uint32_t b_hi,
+                                               std::index_sequence<V...>) {
   (
       [&] {
-        constexpr FatMma g = FatTable<TAPS>::g[G];
-        if (j == g.stage) {
-          wgmma_ss_at<g.nslots * BN, g.slot0 * BN>(acc, wgmma_lohi(a_lo0 + g.view * 8u + k * 2u, a_hi),
-                                                   wgmma_lohi(b_lo0 + g.brow * BN * 8u + k * 2u, b_hi), 1u);
-          // groups of different N overlap in accumulator columns and must not be in flight together
-          wgmma_commit();
-          wgmma_wait<0>();
-        }
+        constexpr SubpixelView g = SubpixelTable<TAPS>::v[V];
+        if (j == g.stage)
+          subpixel_slots<BN, g.slot0, g.brow>(acc, wgmma_lohi(a_lo0 + g.view * 8u + k * 2u, a_hi), b_lo0 + k * 2u, b_hi,
+                                              std::make_index_sequence<g.nslots>{});
       }(),
       ...);
 }
@@ -313,10 +321,8 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
         }
         const uint32_t a_lo0 = wgmma_lo(a_smem + as * C::A_BYTES) + wg_off;
         const uint32_t bs0 = bi % C::B_STAGES;
-        // 3x3 / GEMM layers: unrolled (a data-dependent branch around wgmma makes ptxas serialise the wgmma pipeline).  Sub-pixel
-        // layers stay rolled: two fat groups of one stage may accumulate into overlapping column ranges of different N, which must
-        // not be in flight together; the runtime stage select makes ptxas wait between them.
-#pragma unroll(NACC == 1 ? C::TG : 1)
+        // unrolled: a data-dependent branch around wgmma makes ptxas serialise the wgmma pipeline
+#pragma unroll
         for (int j = 0; j < C::TG; ++j) {
           const uint32_t bs = RC ? (uint32_t)(c * C::TG + j) : (bi + j) % C::B_STAGES;
           if (!RC) mbar_wait(smem_u32(&b_full[bs]), ((bi + j) / C::B_STAGES) & 1u);
@@ -338,7 +344,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
                   Wgmma<BN>::ss(acc[sub], wgmma_lohi(a_lo0 + aoff + sub * kRowsPerSub * 8 + k * 2, kAHi), bd, 1u);
               }
             } else {
-              fat_issue<BN, TAPS>(acc[0], j, k, a_lo0, b_lo0, kAHi, kBHi, std::make_index_sequence<FatTable<TAPS>::NG>{});
+              subpixel_issue<BN, TAPS>(acc[0], j, k, a_lo0, b_lo0, kAHi, kBHi, std::make_index_sequence<SubpixelTable<TAPS>::NV>{});
             }
           }
           if constexpr (!C::LAG) {   // the weight ring holds less than two chunks: hand each weight stage back as soon as it is read
@@ -796,7 +802,7 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
   h.halo_y0 = tr ? 0 : -1;
   h.halo_x0 = tr ? 0 : -1;
   if (up || tr) {
-    // accumulator slots p0, p1, p3, p2 (phase index = oy*2 + ox), see FatTable
+    // accumulator slots p0, p1, p3, p2 (phase index = oy*2 + ox), see SubpixelTable
     const int slot_phase[4] = {0, 1, 3, 2};
     for (int sl = 0; sl < 4; ++sl) {
       h.acc_oy[sl] = p.ph[slot_phase[sl]].ooy;

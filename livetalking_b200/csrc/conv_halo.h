@@ -24,7 +24,7 @@ struct alignas(64) HaloParams {
   // halo tiles in shared memory instead of reading res from global memory
   int res_halo;
   int halo_y0, halo_x0;  // halo origin relative to the tile origin (-1 for pad-1 conv, 0 for ConvT phases)
-  // output offset of each accumulator slot (sub-pixel phase; slot order p0, p1, p3, p2, see conv_halo.cu FatTable)
+  // output offset of each accumulator slot (sub-pixel phase; slot order p0, p1, p3, p2, see conv_halo.cu SubpixelTable)
   int acc_oy[4], acc_ox[4];
   int tiles_x, tiles_y, tiles_n, total_tiles;
   // optional fused GroupNorm statistics of the OUTPUT tensor (sum, sum of squares per (image, group)), accumulated by the
@@ -65,7 +65,7 @@ int conv_halo_resident_chunks(const HaloPlan& pl, int sms);
 bool conv_halo_gn_fusable(const HaloPlan& pl, int cout_total, int groups, int hw);
 cudaError_t launch_w_tap_major(const __half* w, __half* wt, int cout, int cin, cudaStream_t st, int ntaps = 9);
 // ConvT(k3,s2) weights: phase-major rows [Cout][9][Cin] (pack order of w2l_pack.py / pack_convT_w) -> the view-major slice
-// order the fat-N issue loop expects (see conv_halo.cu FatTable)
+// order the sub-pixel issue loop expects (see conv_halo.cu SubpixelTable)
 cudaError_t launch_w_tap_major_convT(const __half* w, __half* wt, int cout, int cin, cudaStream_t st);
 
 }  // namespace ltb
