@@ -65,13 +65,18 @@ struct HaloCfg {
   static constexpr int A_STAGES_STREAM = S2 ? 2 : ((BN <= 32) ? 4 : (BN <= 64 ? 3 : (NSUB == 1 ? 3 : 2)));
   static constexpr int A_STAGES_RES = ((BUDGET - RC * TG * B_BYTES) / A_BYTES) > 4 ? 4 : ((BUDGET - RC * TG * B_BYTES) / A_BYTES);
   static constexpr int A_STAGES = RC ? A_STAGES_RES : A_STAGES_STREAM;
-  static constexpr int B_STAGES_MAX = (BUDGET - A_STAGES * A_BYTES) / B_BYTES;
+  // <128,2,1> reads its residual from global memory (see halo_res_smem_ok); its ring leaves room for one 128-pixel sub-tile of
+  // it, so the consumers prefetch the residual while the tile's MMAs run: sub-tile 0 by cp.async into RES_BYTES of shared memory
+  // at the start of the tile, sub-tile 1 into registers before the last wgmma wait
+  static constexpr bool RES_PREFETCH = (BN == 128 && NSUB == 2 && NACC == 1 && TAPS == 9 && RC == 0);
+  static constexpr int RES_BYTES = RES_PREFETCH ? 128 * BN * 2 : 0;
+  static constexpr int B_STAGES_MAX = (BUDGET - A_STAGES * A_BYTES - RES_BYTES) / B_BYTES;
   static constexpr int B_STAGES = RC ? RC * TG : (B_STAGES_MAX > 8 ? 8 : B_STAGES_MAX);
   // release the stages of chunk c only once chunk c+1 is issued (one wgmma group in flight) when the weight ring can hold
   // two chunks; otherwise each weight stage is waited for and handed back right after its MMAs
   static constexpr bool LAG = RC || B_STAGES >= 2 * TG;
   static constexpr int ACOLS = NACC * BN;                                   // accumulator columns per sub-tile
-  static constexpr int SMEM_BYTES = A_STAGES * A_BYTES + B_STAGES * B_BYTES + 1024;
+  static constexpr int SMEM_BYTES = A_STAGES * A_BYTES + B_STAGES * B_BYTES + RES_BYTES + 1024;
   static_assert(NSUB * ACOLS <= 256, "register accumulator overflow");
   static_assert(B_STAGES >= 2, "not enough shared memory for the weight ring");
   static_assert(A_STAGES >= 2, "not enough shared memory for the halo ring");
@@ -284,9 +289,47 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
     constexpr bool kResHalo = halo_res_smem_ok(BN, NSUB, NACC, TAPS);
     const int res_row = (8 * wg + 2 * wq + ((lane >> 3) & 1) + 1) * C::P + (lane & 7) + 1;   // halo row of MMA row (r % 8 = lane % 8)
     const int res_kb = lane >> 4;
+    // halo modes: output (and residual) pixel of MMA row r of sub-tile `sub`, accumulator slot sl; ok = false past the map's edge
+    auto halo_pix = [&](int img, int ty, int tx, int sub, int sl, int r, bool& ok) -> size_t {
+      const int gy = ty * (16 * NSUB) + sub * 16 + wg * 8 + (r >> 3), gx = tx * 8 + (r & 7);
+      ok = gy < p.GH && gx < p.GW;   // tiles may overhang small / odd-sized maps
+      return ((size_t)img * p.OH + gy * p.osy + p.acc_oy[sl]) * p.OW + gx * p.osx + p.acc_ox[sl];
+    };
+    // RES_PREFETCH: sub-tile 0's residual, 16 bytes per (row half hh, 32-channel block m) of each consumer thread, laid out
+    // [hh][m][thread] so that a warp's accesses are contiguous.  Each thread reads back only the slots it filled itself.
+    const uint32_t res_buf = b_smem + C::B_STAGES * C::B_BYTES;
     if (RC) mbar_wait(smem_u32(&b_full[0]), 0);
     uint32_t ai = 0, bi = 0;
     for (int t = blockIdx.x; t < p.total_tiles; t += gridDim.x) {
+      const int nt = t / tiles_m;
+      int mt = t - nt * tiles_m;
+      int img = 0, ty = 0, tx = 0;
+      if (kHaloMode) {
+        img = mt / (p.tiles_x * p.tiles_y);
+        mt -= img * (p.tiles_x * p.tiles_y);
+        ty = mt / p.tiles_x;
+        tx = mt - ty * p.tiles_x;
+      }
+      const int n0 = nt * BN;
+      const bool res_pf = C::RES_PREFETCH && p.res != nullptr && !LTB_DIAG(1);
+      // the residual of MMA row r of sub-tile sub: 8 channels per 32-channel block, the lane's block of the row
+      auto res_src = [&](int sub, int r, bool& ok) {
+        const size_t px = halo_pix(img, ty, tx, sub, 0, r, ok);
+        return reinterpret_cast<const uint4*>(p.res + (ok ? px : 0) * p.RCtot + p.rc_off + n0 + 8 * (lane & 3));
+      };
+      if constexpr (C::RES_PREFETCH) {
+        if (res_pf) {   // the slots were last read in the previous tile's epilogue, by this thread, before its stores
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            bool ok;
+            const uint4* src = res_src(0, wq * 16 + (lane >> 2) + 8 * hh, ok);
+#pragma unroll
+            for (int m = 0; m < BN / 32; ++m) cp_async16(res_buf + ((hh * (BN / 32) + m) * 256 + tid) * 16, src + 4 * m, ok ? 16u : 0u);
+          }
+          cp_async_commit();
+        }
+      }
+      uint4 rpf[2][BN / 32];   // RES_PREFETCH: sub-tile 1's residual
       float acc[NSUB][C::ACOLS / 2];
 #pragma unroll
       for (int s = 0; s < NSUB; ++s)
@@ -375,7 +418,19 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
         ++ai;
         if (!RC) bi += C::TG;
       }
+      if constexpr (C::RES_PREFETCH) {
+        if (res_pf) {   // under the last chunk's MMAs
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            bool ok;
+            const uint4* src = res_src(1, wq * 16 + (lane >> 2) + 8 * hh, ok);
+#pragma unroll
+            for (int m = 0; m < BN / 32; ++m) rpf[hh][m] = ok ? __ldcg(src + 4 * m) : make_uint4(0u, 0u, 0u, 0u);
+          }
+        }
+      }
       wgmma_wait<0>();
+      if (C::RES_PREFETCH && res_pf) cp_async_wait<0>();
 #pragma unroll
       for (int s = 0; s < NSUB; ++s) wgmma_fence_regs(acc[s]);
       if (C::LAG && pend) {
@@ -389,16 +444,6 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
       if (LTB_DIAG(2)) continue;
 
       // ---------------------------------------------------------- epilogue from the accumulator fragments
-      const int nt = t / tiles_m;
-      int mt = t - nt * tiles_m;
-      int img = 0, ty = 0, tx = 0;
-      if (kHaloMode) {
-        img = mt / (p.tiles_x * p.tiles_y);
-        mt -= img * (p.tiles_x * p.tiles_y);
-        ty = mt / p.tiles_x;
-        tx = mt - ty * p.tiles_x;
-      }
-      const int n0 = nt * BN;
       const float* bias = p.bias;
       int g_tile = 0;   // grouped: this tile's group; its rows [g_tile * group_rows, (g_tile + 1) * group_rows) are the only ones written
       if constexpr (GRP) {
@@ -433,9 +478,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
             size_t opix;
             bool row_ok;
             if (kHaloMode) {
-              const int gy = ty * (16 * NSUB) + sub * 16 + wg * 8 + (r >> 3), gx = tx * 8 + (r & 7);
-              opix = ((size_t)img * p.OH + gy * p.osy + p.acc_oy[sl]) * p.OW + gx * p.osx + p.acc_ox[sl];
-              row_ok = gy < p.GH && gx < p.GW;   // tiles may overhang small / odd-sized maps
+              opix = halo_pix(img, ty, tx, sub, sl, r, row_ok);
             } else if constexpr (GRP) {
               // rows past the group's end belong to the next group, computed here with the wrong weights: never written
               const int lrow = (mt - g_tile * p.group_tiles) * (128 * NSUB) + sub * 128 + wg * 64 + r;
@@ -466,8 +509,9 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
               if (!head || res_gmem) {
                 quad_transpose(v, lane);
                 if (res_gmem) {
-                  uint4 r4 = make_uint4(0u, 0u, 0u, 0u);
-                  if (row_ok) r4 = __ldcg(rptr + 4 * m);
+                  uint4 r4 = make_uint4(0u, 0u, 0u, 0u);   // rows past the map's edge: zero, never stored
+                  if constexpr (C::RES_PREFETCH) r4 = sub == 0 ? lds128(res_buf + ((hh * (BN / 32) + m) * 256 + tid) * 16) : rpf[hh][m];
+                  else if (row_ok) r4 = __ldcg(rptr + 4 * m);
                   const uint32_t rv[4] = {r4.x, r4.y, r4.z, r4.w};
 #pragma unroll
                   for (int j = 0; j < 4; ++j) v[j] = add_res(v[j], rv[j]);

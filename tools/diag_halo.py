@@ -2,7 +2,9 @@
 
 Builds lib/libltb200_diag.so with -DLTB_HALO_DIAG (conv_halo.cu then honours the LTB_HALO_DIAG environment variable at
 plan time: bit0 no epilogue global I/O, bit1 no epilogue work, bit2 no MMAs, bit3 no A (halo) loads, bit4 no B (weight)
-loads) and times the wav2lip256 decoder's narrow layers with each role knocked out in turn.
+loads) and times the wav2lip256 decoder's 3x3 convs at batch 16 with each role knocked out in turn.  Each line starts with the
+kernel instance Ctx.conv_plan picks for that shape (the fused 1x1 head of L53 exists only inside the engine's forward plan:
+`tools/diag_layers.py --forward` times it there).
 
     python tools/diag_halo.py --build          # here (cross-compile)
     python tools/diag_halo.py                  # on the GPU box
@@ -29,9 +31,10 @@ def main():
     rng = np.random.default_rng(0)
     cases = [  # name, N, H, Cin, Cout, residual
         ("L52 64->64 res @256", 16, 256, 64, 64, True),
-        ("L53 64->32     @256", 16, 256, 64, 32, False),
+        ("L53 80->32     @256", 16, 256, 80, 32, False),
         ("L49 128->128 res @128", 16, 128, 128, 128, True),
         ("L46 256->256 res @64", 16, 64, 256, 256, True),
+        ("L43 384->384 res @32", 16, 32, 384, 384, True),
     ]
     variants = [0, 1, 2, 4, 8, 16, 24, 4 | 2, 8 | 16 | 2, 4 | 8 | 16, 4 | 8 | 16 | 2]
     if os.environ.get("LTB_DIAG_ONLY"):          # e.g. "0:0" = first case, variant 0 (for an ncu capture)
@@ -48,6 +51,8 @@ def main():
         out = ctx.alloc((N * H * H, cout), np.float16)
         r = (ctx.upload(xh) if copy else x) if (res and cin == cout) else None
         flops = 2.0 * N * H * H * 9 * cin * cout
+        plan = ctx.conv_plan(x, w, out, N=N, IH=H, IW=H, OH=H, OW=H, pad=(1, 1), res=r, relu=True)
+        inst = "kernel%d<%d,%d,%d,%d,RC=%d>" % (plan["kernel"], plan["bn"], plan["nsub"], plan["nacc"], plan["taps"], plan["resident_chunks"])
         line = [name]
         for v in variants:
             os.environ["LTB_HALO_DIAG"] = str(v)
@@ -61,7 +66,7 @@ def main():
             ctx.sync()
             us = (time.perf_counter() - t0) / reps * 1e6
             line.append(f"dbg{v}:{us:.1f}us")
-        print(" ".join(line), f"| full = {flops / 1e6 / float(line[1].split(':')[1][:-2]):.0f} TF/s", flush=True)
+        print(inst, " ".join(line), f"| full = {flops / 1e6 / float(line[1].split(':')[1][:-2]):.0f} TF/s", flush=True)
 
 
 if __name__ == "__main__":

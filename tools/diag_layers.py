@@ -2,9 +2,12 @@
 
     python -m livetalking_b200.build --diag          # here (cross-compile lib/libltb200_diag.so with -DLTB_HALO_DIAG)
     python tools/diag_layers.py                      # on the GPU box
+    python tools/diag_layers.py --forward            # the same knock-outs on every op of the real batch-16 forward plan
 
 For every shape: full kernel, then with one role knocked out (LTB_HALO_DIAG bits: 1 no epilogue global I/O, 2 no epilogue,
-4 no MMAs, 8 no A (halo) loads, 16 no B (weight) loads) — what the remaining time is tells which resource bounds the layer."""
+4 no MMAs, 8 no A (halo) loads, 16 no B (weight) loads) — what the remaining time is tells which resource bounds the layer.
+--forward: per-op event timings (median of 5 eager profiling passes) of the wav2lip256 batch-16 forward, fused 1x1 head and
+all, under LTB_HALO_DIAG 0 / 1 / 2, and the sum over the halo-kernel ops of (dbg0 - dbg1) and (dbg0 - dbg2)."""
 import os
 import sys
 
@@ -18,6 +21,8 @@ def main():
         _capi.LIB_PATH = os.path.join(os.path.dirname(_capi.LIB_PATH), "libltb200_diag.so")
     from livetalking_b200 import engine
     engine.set_device(0)
+    if "--forward" in sys.argv:
+        return forward(engine)
     rng = np.random.default_rng(0)
     cases = [  # name, N, H, Cin, Cout, transposed, residual
         ("L50 ConvT 160->64 @128", 16, 128, 160, 64, True, False),
@@ -28,6 +33,7 @@ def main():
         ("L45 conv 256->256 @64 res", 16, 64, 256, 256, False, True),
         ("L48 conv 128->128 @128 res", 16, 128, 128, 128, False, True),
         ("L51 conv 64->64 @256 res", 16, 256, 64, 64, False, True),
+        ("L53 conv 80->32 @256", 16, 256, 80, 32, False, False),
         ("L39 conv 512->512 @16 res", 16, 16, 512, 512, False, True),
         ("L25 conv 256->256 @16 res", 16, 16, 256, 256, False, True),
         ("L28 conv 512->512 @8 res", 16, 8, 512, 512, False, True),
@@ -51,6 +57,32 @@ def main():
                 base = ms
             line.append(f"dbg{v}:{ms * 1000:.1f}us")
         print(" ".join(line), f"| full = {flops / 1e9 / base:.0f} TF/s", flush=True)
+
+
+def forward(engine):
+    from livetalking_b200 import synth
+    from livetalking_b200.w2l_pack import pack_state_dict
+    model = engine.W2LModel(pack_state_dict(synth.random_state_dict(0)))
+    av = engine.W2LAvatar(*synth.synthetic_avatar(n=16, H=720, W=1280, bbox=(200, 520, 480, 800)))
+    med = {}
+    for v in (0, 1, 2):
+        os.environ["LTB_HALO_DIAG"] = str(v)    # read when the session plans its convs
+        sess = engine.W2LSession(model, av, 16)
+        sess.mel_step(synth.sine_audio(2.0)[:(10 + 10 + 2 * 16) * 320], want_output=False)   # one step's PCM window
+        sess.profile_ops(0)
+        passes = [sess.profile_ops(0) for _ in range(5)]
+        kinds, flops = passes[0][2], passes[0][1]
+        med[v] = np.median(np.stack([ms for ms, _, _ in passes]), axis=0)
+        sess.close()
+    halo = kinds == 4   # kind 4: halo kernel (3x3 / ConvT / GEMM mode)
+    print("op kind GFLOP  dbg0_us dbg1_us dbg2_us")
+    for i in range(len(kinds)):
+        if halo[i]:
+            print(f"{i:3d} {kinds[i]} {flops[i] / 1e9:7.1f} {med[0][i] * 1e3:7.1f} {med[1][i] * 1e3:7.1f} {med[2][i] * 1e3:7.1f}")
+    tot = med[0].sum() * 1e3
+    rec, ceil = ((med[0] - med[1])[halo].sum() * 1e3, (med[0] - med[2])[halo].sum() * 1e3)
+    print(f"all ops {tot:.1f} us | halo ops {med[0][halo].sum() * 1e3:.1f} us | sum(dbg0-dbg1) {rec:.1f} us ({100 * rec / tot:.1f} %)"
+          f" | sum(dbg0-dbg2) {ceil:.1f} us ({100 * ceil / tot:.1f} %)", flush=True)
 
 
 if __name__ == "__main__":
