@@ -33,7 +33,8 @@ def main():
     args = ap.parse_args()
     import torch
     from livetalking_b200 import configs, engine, synth
-    from livetalking_b200.musetalk import Builder, MuseTalkAvatar, MuseTalkModel, MuseTalkSession
+    from livetalking_b200.graph import GraphSession
+    from livetalking_b200.musetalk import MuseTalkAvatar, MuseTalkModel, MuseTalkSession
     from livetalking_b200.ops import Ctx
     from livetalking_b200.whisper import WhisperEncoder, WhisperFeatures
 
@@ -53,15 +54,9 @@ def main():
     # encoder graph (config 3): B crops -> latents
     crops_u8 = ctx.upload(np.random.default_rng(0).integers(0, 256, (B, 256, 256, 3), dtype=np.uint8))
     enc_out = ctx.alloc((B, 32, 32, 16), np.float16, zero=True)
-    eb = Builder(ctx)
-    net.emit_vae_encode(eb, crops_u8, enc_out)
-    ctx.sync()
-    from livetalking_b200.musetalk import _Replay
-    temps, eb.temps = eb.temps, []
-    eb.new = _Replay(temps)
-    with ctx.capture() as cap:
-        net.emit_vae_encode(eb, crops_u8, enc_out)
-    enc_graph = cap.graph
+    enc = GraphSession(ctx)
+    enc.capture(lambda b: net.emit_vae_encode(b, crops_u8, enc_out))
+    enc_graph = enc.graph
 
     pcm = synth.sine_audio(5.0)[:wf.n]
     wf.run_async(pcm)

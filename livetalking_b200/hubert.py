@@ -14,7 +14,7 @@ from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
-from .musetalk import Builder, _Norm, _Replay, _np
+from .graph import Builder, GraphSession, _Norm, _np
 from .ops import ConvWeight, Ctx, DevTensor
 
 CONV_KERNEL = (10, 3, 3, 3, 3, 2, 2)
@@ -141,34 +141,31 @@ def window_samples(batch: int, stride_left: int, stride_right: int) -> tuple:
     return n, Tc, T
 
 
-class HubertFeatures:
+class HubertFeatures(GraphSession):
     """get_hubert_from_16k_speech + HubertASR's window gather for one session: PCM buffer -> (B, 16, D) features, one CUDA graph.
     The window is (stride_left + stride_right + 2 * batch) 20 ms chunks (HubertASR keeps exactly that many, hubert.py:30-48)."""
 
     def __init__(self, enc: HubertEncoder, batch: int, stride_left: int = 10, stride_right: int = 10, out_nhwc: Optional[DevTensor] = None,
                  ctx: Optional[Ctx] = None):
+        super().__init__(ctx)
         self.enc, self.B = enc, int(batch)
-        self._own_ctx = ctx is None
-        ctx = self.ctx = Ctx() if ctx is None else ctx
-        self.n, self.Tc, self.T = window_samples(self.B, stride_left, stride_right)
-        self.pcm = ctx.alloc((self.n,), np.float32, zero=True)
-        self.stats = ctx.alloc((4,), np.float32, zero=True)
-        self.out = ctx.alloc((self.B, ROWS, enc.D), np.float32, zero=True)
-        self.out_nhwc = out_nhwc
-        self.start = stride_left / 2.0
-        self.builder = Builder(ctx)
+        try:
+            ctx = self.ctx
+            self.n, self.Tc, self.T = window_samples(self.B, stride_left, stride_right)
+            self.pcm = self.alloc((self.n,), np.float32, zero=True)
+            self.stats = self.alloc((4,), np.float32, zero=True)
+            self.out = self.alloc((self.B, ROWS, enc.D), np.float32, zero=True)
+            self.out_nhwc = out_nhwc
+            self.start = stride_left / 2.0
 
-        def emit():
-            self.hidden = enc.emit(self.builder, self.pcm, self.n, self.stats)
-            ctx.hubert_slice(self.hidden, self.Tc, self.T, enc.D, self.B, ROWS, self.start, 2.0, WIN[0], self.out, self.out_nhwc)
+            def emit(b: Builder):
+                self.hidden = enc.emit(b, self.pcm, self.n, self.stats)
+                ctx.hubert_slice(self.hidden, self.Tc, self.T, enc.D, self.B, ROWS, self.start, 2.0, WIN[0], self.out, self.out_nhwc)
 
-        emit()
-        ctx.sync()
-        temps, self.builder.temps = self.builder.temps, []
-        self.builder.new = _Replay(temps)
-        with ctx.capture() as cap:
-            emit()
-        self.graph = cap.graph
+            self.capture(emit)
+        except BaseException:
+            self.close()
+            raise
 
     def run_async(self, pcm: Optional[np.ndarray] = None):
         if pcm is not None:
@@ -188,22 +185,8 @@ class HubertFeatures:
         with self.ctx.lock:
             return self.ctx.download(self.hidden)
 
-    def close(self):
-        if getattr(self, "graph", None) is not None:
-            self.graph.close()
-            self.graph = None
-        if self._own_ctx and self.ctx is not None:
-            self.ctx.close()
-        self.ctx = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class HubertBatchFeatures:
+class HubertBatchFeatures(GraphSession):
     """HubertFeatures for up to G sessions at once: G PCM windows of the same layout -> G x (B, 16, D) features, ONE CUDA graph of
     one encoder forward over the G windows stacked on the row dimension (HubertEncoder.emit_grouped).  At B = 16 a window is ~51
     tokens, under half of one 128-row GEMM tile, and every window re-reads the encoder's weights: G windows per forward share
@@ -218,26 +201,23 @@ class HubertBatchFeatures:
         if self.G < 1:
             raise ValueError("groups must be >= 1")
         self.batch = self.G                                  # CrossSessionBatcher: requests per engine call
-        self._own_ctx = ctx is None
-        ctx = self.ctx = Ctx() if ctx is None else ctx
-        self.n, self.Tc, self.T = window_samples(self.B, stride_left, stride_right)
-        self.pcm = ctx.alloc((self.G, self.n), np.float32, zero=True)
-        self.stats = ctx.alloc((self.G, 4), np.float32, zero=True)
-        self.out = ctx.alloc((self.G, self.B, ROWS, enc.D), np.float32, zero=True)
-        self.start = stride_left / 2.0
-        self.builder = Builder(ctx)
+        super().__init__(ctx)
+        try:
+            ctx = self.ctx
+            self.n, self.Tc, self.T = window_samples(self.B, stride_left, stride_right)
+            self.pcm = self.alloc((self.G, self.n), np.float32, zero=True)
+            self.stats = self.alloc((self.G, 4), np.float32, zero=True)
+            self.out = self.alloc((self.G, self.B, ROWS, enc.D), np.float32, zero=True)
+            self.start = stride_left / 2.0
 
-        def emit():
-            self.hidden = enc.emit_grouped(self.builder, self.pcm, self.G, self.n, self.stats)
-            ctx.hubert_slice(self.hidden, self.Tc, self.T, enc.D, self.B, ROWS, self.start, 2.0, WIN[0], self.out, None, G=self.G)
+            def emit(b: Builder):
+                self.hidden = enc.emit_grouped(b, self.pcm, self.G, self.n, self.stats)
+                ctx.hubert_slice(self.hidden, self.Tc, self.T, enc.D, self.B, ROWS, self.start, 2.0, WIN[0], self.out, None, G=self.G)
 
-        emit()
-        ctx.sync()
-        temps, self.builder.temps = self.builder.temps, []
-        self.builder.new = _Replay(temps)
-        with ctx.capture() as cap:
-            emit()
-        self.graph = cap.graph
+            self.capture(emit)
+        except BaseException:
+            self.close()
+            raise
 
     def run_async(self, pcms: Sequence[np.ndarray]) -> int:
         """Stage windows 0 .. k-1 and launch the graph; -> k."""
@@ -259,20 +239,6 @@ class HubertBatchFeatures:
         return [out[g] for g in range(k)]
 
     infer_slots = run_groups
-
-    def close(self):
-        if getattr(self, "graph", None) is not None:
-            self.graph.close()
-            self.graph = None
-        if self._own_ctx and self.ctx is not None:
-            self.ctx.close()
-        self.ctx = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def gflop_per_window(n_samples: int, layers: int = 24, d_model: int = 1024, ffn: int = 4096, conv_dim: int = 512) -> float:

@@ -17,37 +17,20 @@ Load-time rewrites (exact up to fp16 rounding):
 """
 from __future__ import annotations
 
-import os
-
 import math
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
 from . import _capi
+from .graph import Builder, GraphSession, _ceil16, _Norm, _np
 from .ops import ConvWeight, Ctx, DevTensor
 
 KEY_PAD = 64  # cross-attention keys (50 audio tokens) padded to a multiple of 16
 
 
-def _np(t) -> np.ndarray:
-    if hasattr(t, "detach"):
-        t = t.detach().cpu().float().numpy()
-    return np.asarray(t, dtype=np.float32)
-
-
-def _ceil16(x: int) -> int:
-    return (x + 15) // 16 * 16
-
-
 def _silu(x):
     return x / (1.0 + np.exp(-x))
-
-
-class _Norm:
-    def __init__(self, ctx: Ctx, sd, p):
-        self.gamma = ctx.upload(_np(sd[p + ".weight"]))
-        self.beta = ctx.upload(_np(sd[p + ".bias"]))
 
 
 def _pad_heads_rows(w: np.ndarray, heads: int, d: int, dp: int) -> np.ndarray:
@@ -122,153 +105,6 @@ class _Transformer:
         self.attn2 = _Attn(ctx, sd, b + ".attn2", C, heads, ctx_dim)
         self.ff1 = ConvWeight(ctx, _np(sd[b + ".ff.net.0.proj.weight"]), _np(sd[b + ".ff.net.0.proj.bias"]), tap_major=False)
         self.ff2 = ConvWeight(ctx, _np(sd[b + ".ff.net.2.weight"]), _np(sd[b + ".ff.net.2.bias"]), tap_major=False)
-
-
-class Builder:
-    """Emits engine ops for the diffusers building blocks.  Tensors are NHWC fp16 ``DevTensor``s of shape (N,H,W,C)."""
-
-    GN_GROUPS = 32   # every GroupNorm of the diffusers UNet / VAE uses 32 groups
-    # Fusing the GroupNorm statistics into the producing conv's epilogue (ltb_conv_op.gn_stats) is implemented and tested per kernel
-    # path against float64 sums (tests/test_gpu_conv_op.py::test_conv_op_groupnorm_statistics), but off by default: the extra
-    # shuffles/atomics load the conv epilogue, and whether that beats the separate statistics pass has not been measured on H100.
-    FUSE_GN_STATS = os.environ.get("LTB_FUSE_GN", "0") == "1"
-
-    def __init__(self, ctx: Ctx):
-        self.ctx = ctx
-        self.temps: List[DevTensor] = []
-
-    def _stats_for(self, out: DevTensor, n_img: int):
-        """Ask the producing conv to also emit the GroupNorm statistics of `out` (fused into its epilogue when possible)."""
-        if not self.FUSE_GN_STATS or out.C % self.GN_GROUPS or out.pitch != out.C or out.c_off:
-            return None
-        st = self.new(n_img * self.GN_GROUPS * 4)                  # n_img * groups * 2 floats
-        out.stats = (st, self.GN_GROUPS)
-        return st
-
-    def new(self, *shape) -> DevTensor:
-        t = self.ctx.alloc(shape, np.float16, zero=True)
-        self.temps.append(t)
-        return t
-
-    # -- primitives
-    def conv3(self, x: DevTensor, w: ConvWeight, res: Optional[DevTensor] = None, stride: int = 1, pad=(1, 1), out: Optional[DevTensor] = None,
-              stats: bool = False):
-        N, H, W, _ = x.shape
-        OH = (H + (2 if pad == (1, 1) else 1) - 3) // stride + 1
-        OW = (W + (2 if pad == (1, 1) else 1) - 3) // stride + 1
-        if out is None:
-            out = self.new(N, OH, OW, w.cout)
-        st = self._stats_for(out, N) if stats else None
-        self.ctx.conv(x, w, out, N=N, IH=H, IW=W, OH=OH, OW=OW, stride=(stride, stride), pad=pad, res=res,
-                      gn_stats=st, gn_groups=self.GN_GROUPS if st is not None else 0, gn_hw=OH * OW)
-        return out
-
-    def linear(self, x: DevTensor, w: ConvWeight, res: Optional[DevTensor] = None, out: Optional[DevTensor] = None, stats_imgs: int = 0):
-        """x (..., Cin) -> (..., Cout) ; also 1x1 convs.  stats_imgs > 0: also produce GroupNorm statistics (rows/stats_imgs pixels per image)."""
-        rows = x.rows
-        if out is None:
-            out = self.new(*x.shape[:-1], w.cout)
-        st = self._stats_for(out, stats_imgs) if stats_imgs else None
-        self.ctx.conv(x, w, out, N=1, IH=1, IW=rows, OH=1, OW=rows, res=res,
-                      gn_stats=st, gn_groups=self.GN_GROUPS if st is not None else 0, gn_hw=(rows // stats_imgs) if stats_imgs else 0)
-        return out
-
-    def groupnorm(self, x: DevTensor, n: _Norm, groups: int, eps: float, silu: bool):
-        N, H, W, C = x.shape
-        out = self.new(N, H, W, C)
-        if x.stats is not None and x.stats[1] == groups:
-            self.ctx.groupnorm_apply(x, N, H * W, groups, eps, x.stats[0], n.gamma, n.beta, silu, out)
-        else:
-            self.ctx.groupnorm(x, N, H * W, groups, eps, n.gamma, n.beta, silu, out)
-        return out
-
-    def layernorm(self, x: DevTensor, n: _Norm, eps: float = 1e-5):
-        out = self.new(*x.shape)
-        self.ctx.layernorm(x, x.rows, x.C, eps, n.gamma, n.beta, out)
-        return out
-
-    # -- blocks
-    def resnet(self, x: DevTensor, r: _Resnet, groups: int, eps: float):
-        h = self.conv3(self.groupnorm(x, r.norm1, groups, eps, True), r.conv1, stats=True)
-        h = self.groupnorm(h, r.norm2, groups, eps, True)
-        skip = self.linear(x, r.shortcut) if r.shortcut is not None else x
-        return self.conv3(h, r.conv2, res=skip, stats=True)
-
-    # softmax(QK^T)V as one tcgen05 kernel (scores never reach HBM); LTB_FUSE_ATTENTION=0 restores GEMM + softmax + GEMM
-    FUSE_ATTENTION = os.environ.get("LTB_FUSE_ATTENTION", "1") == "1"
-
-    def attention(self, a, xq: DevTensor, B: int, nq: int, res: DevTensor, kv_src: Optional[DevTensor] = None, n_keys: Optional[int] = None,
-                  n_valid: Optional[int] = None, stats_imgs: int = 0):
-        """xq: (B*nq, C) normalised tokens.  Self-attention when kv_src is None, else keys/values from kv_src (B*n_keys, kv_dim).
-        Key counts are padded to a multiple of 16 (tensor-core N / K granularity); padded keys get probability 0."""
-        ctx, H, dp, d = self.ctx, a.heads, a.dp, a.d
-        Hdp = H * dp
-        if a.self_attn:
-            nk = _ceil16(nq)
-            valid = nq
-            # batch b's padded keys [nq, nk) are rows of batch b + 1 (the zero rows below for the last batch) on the unfused path and
-            # TMA zero fill on the fused one: both are masked to probability 0, and VT (transpose_heads) is zero for keys >= nq
-            qkv = self.new(B * nq + (nk - nq), 3 * Hdp)                   # padded key rows stay zero
-            self.linear(xq, a.qkv, out=DevTensor(qkv.ptr, (B * nq, 3 * Hdp)))
-            q_ptr, q_pitch = qkv.ptr, 3 * Hdp
-            k_ptr, v_ptr, kv_pitch = qkv.offset(Hdp), qkv.offset(2 * Hdp), 3 * Hdp
-            kv_rows = nq
-        else:
-            q = self.linear(xq, a.q)                                      # (B*nq, Hdp)
-            kv = self.linear(kv_src, a.kv)                                # (B*n_keys, 2*Hdp)
-            q_ptr, q_pitch = q.ptr, Hdp
-            k_ptr, v_ptr, kv_pitch = kv.ptr, kv.offset(Hdp), 2 * Hdp
-            nk, valid, kv_rows = n_keys, n_valid, n_keys
-        if self.FUSE_ATTENTION and dp % 16 == 0 and dp <= 160:
-            VT = self.new(B * H, dp, nk)
-            ctx.transpose_heads(v_ptr, B, kv_rows, kv_pitch, H, dp, nk, VT)
-            O = self.new(B * nq, Hdp)
-            ctx.attention(q_ptr, q_pitch, k_ptr, kv_pitch, kv_rows, VT, nk, B, H, nq, valid, dp, float(d) ** -0.5, O)
-            return self.linear(O, a.out, res=res, stats_imgs=stats_imgs)
-        S = self.new(B * H, nq, nk)
-        qv = DevTensor(q_ptr, (nq, dp), pitch=q_pitch)
-        sv = DevTensor(S.ptr, (nq, nk), pitch=nk)
-        ctx.conv(qv, None, sv, N=1, IH=1, IW=nq, OH=1, OW=nq, cin=dp, cout=nk, w_ptr=k_ptr, ktot=kv_pitch,
-                 zbatch=B * H, zdiv=H, in_z=(nq * q_pitch, dp), w_z=(kv_rows * kv_pitch, dp), out_z=(H * nq * nk, nq * nk))
-        ctx.softmax(S, B * H * nq, nk, valid, float(d) ** -0.5)
-        VT = self.new(B * H, dp, nk)
-        ctx.transpose_heads(v_ptr, B, kv_rows, kv_pitch, H, dp, nk, VT)
-        O = self.new(B * nq, Hdp)
-        ov = DevTensor(O.ptr, (nq, dp), pitch=Hdp)
-        ctx.conv(sv, None, ov, N=1, IH=1, IW=nq, OH=1, OW=nq, cin=nk, cout=dp, w_ptr=VT.ptr, ktot=nk,
-                 zbatch=B * H, zdiv=H, in_z=(H * nq * nk, nq * nk), w_z=(H * dp * nk, dp * nk), out_z=(nq * Hdp, dp))
-        return self.linear(O, a.out, res=res, stats_imgs=stats_imgs)
-
-    def transformer(self, x: DevTensor, t: _Transformer, audio: DevTensor, groups: int):
-        N, H, W, C = x.shape
-        tok = self.linear(self.groupnorm(x, t.norm, groups, 1e-6, False), t.proj_in)       # (N,H,W,C) == tokens (N*HW, C)
-        tok = self.attention(t.attn1, self.layernorm(tok, t.ln1), N, H * W, res=tok)
-        tok = self.attention(t.attn2, self.layernorm(tok, t.ln2), N, H * W, res=tok, kv_src=audio, n_keys=KEY_PAD, n_valid=50)
-        g = self.linear(self.layernorm(tok, t.ln3), t.ff1)                                 # (.., 8C)
-        gg = self.new(N, H, W, 4 * C)
-        self.ctx.geglu(g, N * H * W, 4 * C, gg)
-        tok = self.linear(gg, t.ff2, res=tok)
-        return self.linear(tok, t.proj_out, res=x)
-
-    # Upsample2D (nearest 2x + conv3x3) as ONE kernel: four 2x2 sub-pixel convs over the low-res map (ops.ConvWeight.upconv).
-    FUSE_UPSAMPLE = os.environ.get("LTB_FUSE_UPSAMPLE", "1") == "1"
-
-    def upsample(self, x: DevTensor, w: ConvWeight):
-        N, H, W, C = x.shape
-        if self.FUSE_UPSAMPLE and w.upconv_supported() and x.pitch % 8 == 0 and x.c_off % 8 == 0:
-            out = self.new(N, 2 * H, 2 * W, w.cout)
-            self.ctx.conv(x, w, out, N=N, IH=H, IW=W, OH=2 * H, OW=2 * W, pad=(1, 1), upsample2x=True)
-            return out
-        up = self.new(N, 2 * H, 2 * W, C)
-        self.ctx.upsample2x(x, N, H, W, up)
-        return self.conv3(up, w, stats=True)
-
-    def concat(self, a: DevTensor, b: DevTensor):
-        N, H, W, _ = a.shape
-        out = self.new(N, H, W, a.C + b.C)
-        self.ctx.copy_channels(a, DevTensor(out.ptr, (N, H, W, a.C), pitch=out.C, c_off=0))
-        self.ctx.copy_channels(b, DevTensor(out.ptr, (N, H, W, b.C), pitch=out.C, c_off=a.C))
-        return out
 
 
 class MuseTalkModel:
@@ -377,6 +213,25 @@ class MuseTalkModel:
                 _Resnet(ctx, sd, p + ".resnets.1", None))
 
     # ------------------------------------------------------------------------------------------ graph emitters
+    @staticmethod
+    def _resnet(b: Builder, x: DevTensor, r: _Resnet, groups: int, eps: float) -> DevTensor:
+        h = b.conv3(b.groupnorm(x, r.norm1, groups, eps, True), r.conv1, stats=True)
+        h = b.groupnorm(h, r.norm2, groups, eps, True)
+        skip = b.linear(x, r.shortcut) if r.shortcut is not None else x
+        return b.conv3(h, r.conv2, res=skip, stats=True)
+
+    @staticmethod
+    def _transformer(b: Builder, x: DevTensor, t: _Transformer, audio: DevTensor, groups: int) -> DevTensor:
+        N, H, W, C = x.shape
+        tok = b.linear(b.groupnorm(x, t.norm, groups, 1e-6, False), t.proj_in)          # (N,H,W,C) == tokens (N*HW, C)
+        tok = b.attention(t.attn1, b.layernorm(tok, t.ln1), N, H * W, res=tok)
+        tok = b.attention(t.attn2, b.layernorm(tok, t.ln2), N, H * W, res=tok, kv_src=audio, n_keys=KEY_PAD, n_valid=50)
+        g = b.linear(b.layernorm(tok, t.ln3), t.ff1)                                    # (.., 8C)
+        gg = b.new(N, H, W, 4 * C)
+        b.ctx.geglu(g, N * H * W, 4 * C, gg)
+        tok = b.linear(gg, t.ff2, res=tok)
+        return b.linear(tok, t.proj_out, res=x)
+
     def emit_unet(self, b: Builder, latents16: DevTensor, audio_pe: DevTensor, taps: Optional[dict] = None) -> DevTensor:
         """latents16 (B,h,w,16) [8 real channels], audio_pe (B*64, 384) -> predicted latents (B,h,w,16) [4 real channels]."""
         cfg = self.ucfg
@@ -385,25 +240,25 @@ class MuseTalkModel:
         skips = [h]
         for i, blk in enumerate(self.u_down):
             for j, r in enumerate(blk["res"]):
-                h = b.resnet(h, r, G, eps)
+                h = self._resnet(b, h, r, G, eps)
                 if blk["attn"]:
-                    h = b.transformer(h, blk["attn"][j], audio_pe, G)
+                    h = self._transformer(b, h, blk["attn"][j], audio_pe, G)
                 skips.append(h)
             if blk["down"] is not None:
                 h = b.conv3(h, blk["down"], stride=2)
                 skips.append(h)
             if taps is not None:
                 taps[f"down{i}"] = h
-        h = b.resnet(h, self.u_mid[0], G, eps)
-        h = b.transformer(h, self.u_mid[1], audio_pe, G)
-        h = b.resnet(h, self.u_mid[2], G, eps)
+        h = self._resnet(b, h, self.u_mid[0], G, eps)
+        h = self._transformer(b, h, self.u_mid[1], audio_pe, G)
+        h = self._resnet(b, h, self.u_mid[2], G, eps)
         if taps is not None:
             taps["mid"] = h
         for i, blk in enumerate(self.u_up):
             for j, r in enumerate(blk["res"]):
-                h = b.resnet(b.concat(h, skips.pop()), r, G, eps)
+                h = self._resnet(b, b.concat(h, skips.pop()), r, G, eps)
                 if blk["attn"]:
-                    h = b.transformer(h, blk["attn"][j], audio_pe, G)
+                    h = self._transformer(b, h, blk["attn"][j], audio_pe, G)
             if blk["up"] is not None:
                 h = b.upsample(h, blk["up"])
             if taps is not None:
@@ -412,13 +267,13 @@ class MuseTalkModel:
 
     def _emit_vae_mid(self, b: Builder, h: DevTensor, mid, G, eps):
         r0, gn, attn, r1 = mid
-        h = b.resnet(h, r0, G, eps)
+        h = self._resnet(b, h, r0, G, eps)
         N, H, W, C = h.shape
         h = b.attention(attn, b.groupnorm(h, gn, G, eps, False), N, H * W, res=h, stats_imgs=N)
         st = h.stats
         h = DevTensor(h.ptr, (N, H, W, C))
         h.stats = st
-        return b.resnet(h, r1, G, eps)
+        return self._resnet(b, h, r1, G, eps)
 
     def emit_vae_decode(self, b: Builder, pred16: DevTensor, out_u8: DevTensor, taps: Optional[dict] = None) -> DevTensor:
         """pred16 (B,h,w,16) latents [4 real channels] -> uint8 BGR image written to out_u8 (B,8h,8w,3)."""
@@ -430,7 +285,7 @@ class MuseTalkModel:
             taps["dec_mid"] = h
         for i, blk in enumerate(self.v_dec_up):
             for r in blk["res"]:
-                h = b.resnet(h, r, G, eps)
+                h = self._resnet(b, h, r, G, eps)
             if blk["up"] is not None:
                 h = b.upsample(h, blk["up"])
             if taps is not None:
@@ -452,7 +307,7 @@ class MuseTalkModel:
         h = b.conv3(x, self.v_enc_in, stats=True)
         for blk in self.v_enc_down:
             for r in blk["res"]:
-                h = b.resnet(h, r, G, eps)
+                h = self._resnet(b, h, r, G, eps)
             if blk["down"] is not None:
                 h = b.conv3(h, blk["down"], stride=2, pad=(0, 0), stats=True)     # F.pad(x,(0,1,0,1)) + conv s2 p0
         h = self._emit_vae_mid(b, h, self.v_enc_mid, G, eps)
@@ -501,7 +356,7 @@ class MuseTalkAvatar:
         self.latents = ctx.upload(lat16)
 
 
-class MuseTalkSession:
+class MuseTalkSession(GraphSession):
     """One avatar stream at a fixed batch size: the captured UNet + VAE-decode graph and the paste-back buffers."""
 
     def __init__(self, model: MuseTalkModel, avatar: MuseTalkAvatar, batch: int, keep_taps: bool = False, ctx: Optional[Ctx] = None,
@@ -511,40 +366,32 @@ class MuseTalkSession:
         synchronising a stream another session is using would corrupt both.
         paste_only: no network graph and no activation arena — only paste_pred() works (cross-session mode: the UNet / VAE pass of
         this session's frames runs in a shared MuseTalkBatchSession)."""
+        super().__init__(ctx, with_ctx=not paste_only)
         self.model, self.avatar, self.B = model, avatar, int(batch)
-        self._own_ctx = ctx is None
         self._paste_ctx = None
-        self.graph = None
         if paste_only:
-            self.ctx, self._own_ctx = None, False
             return
-        ctx = self.ctx = Ctx() if ctx is None else ctx
-        B, hw = self.B, avatar.lat_hw
-        self.builder = Builder(ctx)
-        self.d_index = ctx.alloc((4,), np.int32, zero=True)
-        self.audio_in = ctx.alloc((B, KEY_PAD, model.ucfg.cross_attention_dim), np.float16, zero=True)
-        self.audio_pe = ctx.alloc((B * KEY_PAD, model.ucfg.cross_attention_dim), np.float16, zero=True)
-        self.latents16 = ctx.alloc((B, hw, hw, 16), np.float16, zero=True)
-        self.image_u8 = ctx.alloc((B, hw * 8, hw * 8, 3), np.uint8, zero=True)
-        self.frames_out = ctx.alloc((B, avatar.H, avatar.W, 3), np.uint8, zero=True)
-        self.taps = {} if keep_taps else None
-        self._paste_ctx = None
-        self._audio_host = np.zeros((B, KEY_PAD, model.ucfg.cross_attention_dim), np.float16)
+        try:
+            ctx, B, hw = self.ctx, self.B, avatar.lat_hw
+            self.d_index = self.alloc((4,), np.int32, zero=True)
+            self.audio_in = self.alloc((B, KEY_PAD, model.ucfg.cross_attention_dim), np.float16, zero=True)
+            self.audio_pe = self.alloc((B * KEY_PAD, model.ucfg.cross_attention_dim), np.float16, zero=True)
+            self.latents16 = self.alloc((B, hw, hw, 16), np.float16, zero=True)
+            self.image_u8 = self.alloc((B, hw * 8, hw * 8, 3), np.uint8, zero=True)
+            self.frames_out = self.alloc((B, avatar.H, avatar.W, 3), np.uint8, zero=True)
+            self.taps = {} if keep_taps else None
+            self._audio_host = np.zeros((B, KEY_PAD, model.ucfg.cross_attention_dim), np.float16)
 
-        def emit():
-            ctx.gather_rows(avatar.latents, avatar.latents.shape[0], self.d_index, B, hw * hw * 16, self.latents16)
-            ctx.eltwise(self.audio_in, model.pe, self.audio_in.rows * self.audio_in.C, KEY_PAD * self.audio_in.C, 0, self.audio_pe)
-            self.pred16 = model.emit_unet(self.builder, self.latents16, self.audio_pe, self.taps)
-            self.image16 = model.emit_vae_decode(self.builder, self.pred16, self.image_u8, self.taps)
+            def emit(b: Builder):
+                ctx.gather_rows(avatar.latents, avatar.latents.shape[0], self.d_index, B, hw * hw * 16, self.latents16)
+                ctx.eltwise(self.audio_in, model.pe, self.audio_in.rows * self.audio_in.C, KEY_PAD * self.audio_in.C, 0, self.audio_pe)
+                self.pred16 = model.emit_unet(b, self.latents16, self.audio_pe, self.taps)
+                self.image16 = model.emit_vae_decode(b, self.pred16, self.image_u8, self.taps)
 
-        emit()                       # eager pass: allocates every intermediate and warms the kernels up
-        ctx.sync()
-        temps, self.builder.temps = self.builder.temps, []
-        self.builder.new = _Replay(temps)   # the captured pass reuses exactly the same buffers, in the same order
-        with ctx.capture() as cap:
-            emit()
-        self.graph = cap.graph
-        self.graph_launches = None
+            self.capture(emit)
+        except BaseException:
+            self.close()
+            raise
 
     # ---- MuseReal.inference_batch (musetalk_avatar.py:130-152)
     def infer_async(self, index: int, audio_feats: Optional[np.ndarray] = None):
@@ -568,18 +415,8 @@ class MuseTalkSession:
             return None
 
     # ---- MuseReal.paste_back_frame (musetalk_avatar.py:154-164)
-    def _make_paste_op(self, pred: DevTensor, out: DevTensor, slot0: int, index: int, explicit_idx: int, count: int):
-        a = self.avatar
-        op = _capi.MtPasteOp()
-        op.frames, op.coords, op.crop, op.masks, op.mask_off = a.frames.ptr, a.coords.ptr, a.crop.ptr, a.masks.ptr, a.mask_off.ptr
-        op.pred, op.out = pred.ptr, out.ptr
-        op.nf, op.H, op.W = a.n, a.H, a.W
-        op.index, op.explicit_idx, op.slot0, op.count = index, explicit_idx, slot0, count
-        op.pred_hw = a.lat_hw * 8
-        return op
-
     def _paste_op(self, pred: DevTensor, slot0: int, index: int, explicit_idx: int, count: int):
-        self.ctx.mt_paste(self._make_paste_op(pred, self.frames_out, slot0, index, explicit_idx, count))
+        self.ctx.mt_paste(_paste_op(self.avatar, pred, self.frames_out, slot0, index, explicit_idx, count))
 
     def paste(self, slot: int, idx: int) -> np.ndarray:
         if not (0 <= slot < self.B and 0 <= idx < self.avatar.n):
@@ -599,13 +436,13 @@ class MuseTalkSession:
         if not 0 <= idx < self.avatar.n:
             raise ValueError("paste_pred: idx out of range")
         if self._paste_ctx is None:
-            self._paste_ctx = Ctx()
+            self._paste_ctx = self.new_ctx()
             self._pred_scratch = self._paste_ctx.alloc((1, S, S, 3), np.uint8)
             self._paste_out = self._paste_ctx.alloc((self.avatar.H, self.avatar.W, 3), np.uint8)
         pc = self._paste_ctx
         with pc.lock:
             pc.h2d(self._pred_scratch, pred_u8, sync=False)
-            pc.mt_paste(self._make_paste_op(self._pred_scratch, self._paste_out, 0, 0, idx, 1))
+            pc.mt_paste(_paste_op(self.avatar, self._pred_scratch, self._paste_out, 0, 0, idx, 1))
             return pc.download(self._paste_out)
 
     def paste_batch_async(self, index: int):
@@ -616,31 +453,13 @@ class MuseTalkSession:
             self.paste_batch_async(index)
             return self.ctx.download(self.frames_out, out)
 
-    def close(self):
-        """Release the session's graph, streams and device buffers (one WebRTC connection = one session: no HBM leak)."""
-        if getattr(self, "graph", None) is not None:
-            self.graph.close()
-            self.graph = None
-        if self._paste_ctx is not None:
-            self._paste_ctx.close()
-            self._paste_ctx = None
-        if self._own_ctx and self.ctx is not None:
-            self.ctx.close()
-        self.ctx = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
     def step_async(self, index: int):
         """Everything resident (audio features already on the device): UNet + VAE decode + blend paste-back."""
         self.infer_async(index, None)
         self.paste_batch_async(index)
 
 
-class MuseTalkBatchSession:
+class MuseTalkBatchSession(GraphSession):
     """Cross-session batching for MuseTalk (SURVEY 8(f) rank 1, the MuseTalk twin of ltb_w2l_infer_slots): up to G sessions x Bs
     frames run as ONE captured PE + UNet + VAE-decode graph of batch G*Bs.  A *group request* is (avatar, first frame index,
     Whisper features (Bs, 50, 384) or None): group g's latents are gathered from ITS avatar's table (mirror-indexed, outside the
@@ -650,36 +469,32 @@ class MuseTalkBatchSession:
     launch cost far less than four launches.  `batch` / `infer_slots` make it a mux for plugin.batcher.CrossSessionBatcher."""
 
     def __init__(self, model: MuseTalkModel, lat_hw: int, groups: int, frames_per_session: int, ctx: Optional[Ctx] = None):
+        super().__init__(ctx)
         self.model, self.lat_hw, self.Bs, self.G = model, int(lat_hw), int(frames_per_session), int(groups)
         self.batch = self.G                                  # CrossSessionBatcher: requests per engine call
         self.B = B = self.G * self.Bs
-        self._own_ctx = ctx is None
-        ctx = self.ctx = Ctx() if ctx is None else ctx
-        Bs, hw, cad = self.Bs, self.lat_hw, model.ucfg.cross_attention_dim
-        self.builder = Builder(ctx)
-        self._d_index = ctx.alloc((4 * self.G,), np.int32, zero=True)
-        self.d_index = [DevTensor(self._d_index.ptr + 16 * g, (4,), np.int32) for g in range(self.G)]
-        self.audio_in = ctx.alloc((B, KEY_PAD, cad), np.float16, zero=True)
-        self.audio_in_of = [DevTensor(self.audio_in.ptr + g * Bs * KEY_PAD * cad * 2, (Bs, KEY_PAD, cad)) for g in range(self.G)]
-        self.audio_pe = ctx.alloc((B * KEY_PAD, cad), np.float16, zero=True)
-        self.latents16 = ctx.alloc((B, hw, hw, 16), np.float16, zero=True)
-        self.latents16_of = [DevTensor(self.latents16.ptr + g * Bs * hw * hw * 16 * 2, (Bs, hw, hw, 16)) for g in range(self.G)]
-        self.image_u8 = ctx.alloc((B, hw * 8, hw * 8, 3), np.uint8, zero=True)
-        self._frames_out: Dict[tuple, DevTensor] = {}
-        self._audio_host = np.zeros((B, KEY_PAD, cad), np.float16)
+        try:
+            ctx, Bs, hw, cad = self.ctx, self.Bs, self.lat_hw, model.ucfg.cross_attention_dim
+            self._d_index = self.alloc((4 * self.G,), np.int32, zero=True)
+            self.d_index = [DevTensor(self._d_index.ptr + 16 * g, (4,), np.int32) for g in range(self.G)]
+            self.audio_in = self.alloc((B, KEY_PAD, cad), np.float16, zero=True)
+            self.audio_in_of = [DevTensor(self.audio_in.ptr + g * Bs * KEY_PAD * cad * 2, (Bs, KEY_PAD, cad)) for g in range(self.G)]
+            self.audio_pe = self.alloc((B * KEY_PAD, cad), np.float16, zero=True)
+            self.latents16 = self.alloc((B, hw, hw, 16), np.float16, zero=True)
+            self.latents16_of = [DevTensor(self.latents16.ptr + g * Bs * hw * hw * 16 * 2, (Bs, hw, hw, 16)) for g in range(self.G)]
+            self.image_u8 = self.alloc((B, hw * 8, hw * 8, 3), np.uint8, zero=True)
+            self._frames_out: Dict[tuple, DevTensor] = {}
+            self._audio_host = np.zeros((B, KEY_PAD, cad), np.float16)
 
-        def emit():
-            ctx.eltwise(self.audio_in, model.pe, self.audio_in.rows * self.audio_in.C, KEY_PAD * self.audio_in.C, 0, self.audio_pe)
-            self.pred16 = model.emit_unet(self.builder, self.latents16, self.audio_pe, None)
-            self.image16 = model.emit_vae_decode(self.builder, self.pred16, self.image_u8, None)
+            def emit(b: Builder):
+                ctx.eltwise(self.audio_in, model.pe, self.audio_in.rows * self.audio_in.C, KEY_PAD * self.audio_in.C, 0, self.audio_pe)
+                self.pred16 = model.emit_unet(b, self.latents16, self.audio_pe, None)
+                self.image16 = model.emit_vae_decode(b, self.pred16, self.image_u8, None)
 
-        emit()
-        ctx.sync()
-        temps, self.builder.temps = self.builder.temps, []
-        self.builder.new = _Replay(temps)
-        with ctx.capture() as cap:
-            emit()
-        self.graph = cap.graph
+            self.capture(emit)
+        except BaseException:
+            self.close()
+            raise
 
     def _check(self, requests):
         if not 1 <= len(requests) <= self.G:
@@ -721,7 +536,7 @@ class MuseTalkBatchSession:
     def _out(self, g: int, av: MuseTalkAvatar) -> DevTensor:
         key = (g, av.H, av.W)
         if key not in self._frames_out:
-            self._frames_out[key] = self.ctx.alloc((self.Bs, av.H, av.W, 3), np.uint8, zero=True)
+            self._frames_out[key] = self.alloc((self.Bs, av.H, av.W, 3), np.uint8, zero=True)
         return self._frames_out[key]
 
     def paste_async(self, requests: Sequence[tuple]) -> List[DevTensor]:
@@ -729,14 +544,8 @@ class MuseTalkBatchSession:
         self._check(requests)
         outs = []
         for g, (a, index, _f) in enumerate(requests):
-            op = _capi.MtPasteOp()
-            op.frames, op.coords, op.crop, op.masks, op.mask_off = a.frames.ptr, a.coords.ptr, a.crop.ptr, a.masks.ptr, a.mask_off.ptr
             out = self._out(g, a)
-            op.pred, op.out = self.image_u8.ptr, out.ptr
-            op.nf, op.H, op.W = a.n, a.H, a.W
-            op.index, op.explicit_idx, op.slot0, op.count = int(index), -1, g * self.Bs, self.Bs
-            op.pred_hw = a.lat_hw * 8
-            self.ctx.mt_paste(op)
+            self.ctx.mt_paste(_paste_op(a, self.image_u8, out, g * self.Bs, int(index), -1, self.Bs))
             outs.append(out)
         return outs
 
@@ -752,32 +561,16 @@ class MuseTalkBatchSession:
             self.ctx.sync()
             return outs
 
-    def close(self):
-        if getattr(self, "graph", None) is not None:
-            self.graph.close()
-            self.graph = None
-        if self._own_ctx and self.ctx is not None:
-            self.ctx.close()
-        self.ctx = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class _Replay:
-    """Hands back the buffers of the eager pass, in order, while the same op sequence is being captured."""
-
-    def __init__(self, temps):
-        self.temps, self.i = temps, 0
-
-    def __call__(self, *shape):
-        t = self.temps[self.i]
-        self.i += 1
-        assert t.shape == tuple(shape), (t.shape, shape)
-        return t
+def _paste_op(a: MuseTalkAvatar, pred: DevTensor, out: DevTensor, slot0: int, index: int, explicit_idx: int, count: int) -> _capi.MtPasteOp:
+    """The blend paste-back of `count` predictions from pred slot `slot0` into avatar `a`'s frames (index / explicit_idx as ltb_mt_paste_op)."""
+    op = _capi.MtPasteOp()
+    op.frames, op.coords, op.crop, op.masks, op.mask_off = a.frames.ptr, a.coords.ptr, a.crop.ptr, a.masks.ptr, a.mask_off.ptr
+    op.pred, op.out = pred.ptr, out.ptr
+    op.nf, op.H, op.W = a.n, a.H, a.W
+    op.index, op.explicit_idx, op.slot0, op.count = index, explicit_idx, slot0, count
+    op.pred_hw = a.lat_hw * 8
+    return op
 
 
 def encode_avatar_latents(model: MuseTalkModel, images_u8: np.ndarray) -> np.ndarray:
@@ -786,13 +579,13 @@ def encode_avatar_latents(model: MuseTalkModel, images_u8: np.ndarray) -> np.nda
     ctx = model.ctx
     imgs = np.ascontiguousarray(images_u8, np.uint8)
     n, H, W, _ = imgs.shape
-    d_img = ctx.upload(imgs)
-    out = ctx.alloc((n, H // 8, W // 8, 16), np.float16, zero=True)
-    b = Builder(ctx)
-    model.emit_vae_encode(b, d_img, out)
-    lat = ctx.download(out)
-    for t in b.temps:
-        ctx.free(t)
-    ctx.free(d_img)
-    ctx.free(out)
+    run = GraphSession(ctx)                      # owns the buffers of this one eager pass
+    try:
+        d_img = run.alloc(imgs.shape, np.uint8)
+        ctx.h2d(d_img, imgs)
+        out = run.alloc((n, H // 8, W // 8, 16), np.float16, zero=True)
+        model.emit_vae_encode(Builder(ctx, run.alloc), d_img, out)
+        lat = ctx.download(out)
+    finally:
+        run.close()
     return np.ascontiguousarray(lat[..., :8].transpose(0, 3, 1, 2))

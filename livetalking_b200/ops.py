@@ -207,7 +207,7 @@ class Ctx:
             table, d.group_images, d.slots, d.w_slot_stride, d.bias_slot_stride = group
             d.group_slot = table.ptr
         if upsample2x:          # fused nearest-2x upsample + 3x3 conv: the 16-slice weights of ConvWeight.upconv()
-            up = w.upconv(self)
+            up = w.upconv(w.ctx)    # beside the weights: a session's ctx may close while the model still uses them
             d.w, d.w_tap, d.Ktot, d.upsample2x = up[0].ptr, up[1].ptr, 16 * w.cin, 1
         d.transposed = int(transposed)
         return d
@@ -334,6 +334,19 @@ class Ctx:
     def mt_paste(self, op: MtPasteOp):
         check(lib().ltb_op_mt_paste(self._h, C.byref(op)))
 
+    # ---- Whisper front end and feature slicing (livetalking_b200/whisper.py)
+    def whisper_logmel(self, pcm: DevTensor, n: int, fb: DevTensor, logspec: DevTensor, gmax: DevTensor, feats16: DevTensor,
+                       feats32: Optional[DevTensor] = None):
+        check(lib().ltb_op_whisper_logmel(self._h, C.c_void_p(pcm.ptr), n, C.c_void_p(fb.ptr), C.c_void_p(logspec.ptr), C.c_void_p(gmax.ptr),
+                                          C.c_void_p(feats16.ptr), C.c_void_p(feats32.ptr) if feats32 is not None else None))
+
+    def whisper_slice(self, hidden: Sequence[DevTensor], T: int, D: int, B: int, start: float, mult: float, out: DevTensor, out_rows: int):
+        """hidden: the five (T, D) fp16 encoder states; frame i of B takes steps int((i + start) * mult) + 0..9 -> out[i][out_rows][D]."""
+        if len(hidden) != 5:
+            raise ValueError(f"whisper_slice reads 5 hidden states, got {len(hidden)}")
+        ptrs = (C.c_void_p * 5)(*[h.ptr for h in hidden])
+        check(lib().ltb_op_whisper_slice(self._h, ptrs, T, D, B, float(start), float(mult), C.c_void_p(out.ptr), out_rows))
+
     # ---- S3FD face detector (livetalking_b200/s3fd.py)
     def s3fd_prep(self, frames_u8: DevTensor, N: int, H: int, W: int, out: DevTensor):
         """u8 BGR [N,H,W,3] -> fp16 [N,H,W,16]: R-104, G-117, B-123, then zeros."""
@@ -413,6 +426,7 @@ class ConvWeight:
             b[:cout] = np.asarray(bias, np.float32)
         self.bias = ctx.upload(b)
         self.w_tap = None
+        self.ctx = ctx                                             # the ctx holding these weights
         self._w_f32 = w if (kh == 3 and kw == 3) else None       # kept for upconv() (dropped after the first use)
         self._upconv = None
         if tap_major and kh == 3 and kw == 3 and cin_p >= 16:

@@ -34,6 +34,7 @@ from typing import List, Optional, Tuple
 
 import numpy as np
 
+from .graph import GraphSession, _ceil16
 from .ops import ConvWeight, Ctx, DevTensor
 
 INPUT, LANDMARKS, IN_C = 192, 110, 16
@@ -45,10 +46,6 @@ BOTTLENECKS = [("conv3_1", 32, 48, 40, 2), ("conv3_2", 40, 60, 40, 1), ("conv3_3
                ("conv5_1", 48, 168, 72, 2), ("conv5_2", 72, 252, 72, 1), ("conv5_3", 72, 252, 72, 1), ("conv5_4", 72, 252, 72, 1),
                ("conv6", 72, 108, 8, 1)]
 TAPS = ("conv2", "conv3_3", "conv4_3", "conv5_4")           # x1..x4; x5 is conv8
-
-
-def _ceil16(c: int) -> int:
-    return (c + 15) // 16 * 16
 
 
 def gflop_per_frame() -> float:
@@ -226,31 +223,25 @@ class PFLDNet:
         return net
 
 
-class PFLDLandmarker:
+class PFLDLandmarker(GraphSession):
     """One captured graph for batches of N crops of 192 x 192.  Every layer writes its own buffer (the layer tests read them)."""
 
     def __init__(self, net: PFLDNet, N: int, ctx: Optional[Ctx] = None):
+        super().__init__(ctx)
         self.net, self.N = net, int(N)
-        self.ctx = ctx or Ctx()
-        self._owned = []
         try:
             self._build()
-        except Exception:
+        except BaseException:
             self.close()
             raise
 
-    def _alloc(self, shape, dtype=np.float16) -> DevTensor:
-        t = self.ctx.alloc(shape, dtype, zero=True)
-        self._owned.append(t)
-        return t
-
     def _build(self):
         N, net = self.N, self.net
-        self.crops = self._alloc((N, INPUT, INPUT, 3), np.uint8)
-        self.crop_wh = self._alloc((N, 2), np.int32)
-        self.buf = {name: self._alloc((N, h, w, c)) for name, (h, w, c) in net.bufs.items()}
-        self.out_f = self._alloc((N, 2 * LANDMARKS), np.float32)
-        self.out_i = self._alloc((N, 2 * LANDMARKS), np.int32)
+        self.crops = self.alloc((N, INPUT, INPUT, 3), np.uint8, zero=True)
+        self.crop_wh = self.alloc((N, 2), np.int32, zero=True)
+        self.buf = {name: self.alloc((N, h, w, c), zero=True) for name, (h, w, c) in net.bufs.items()}
+        self.out_f = self.alloc((N, 2 * LANDMARKS), np.float32, zero=True)
+        self.out_i = self.alloc((N, 2 * LANDMARKS), np.int32, zero=True)
         self.ops = [("prep", None, self.crops, self.buf["in"])]
         for L in net.layers:
             self.ops.append((L.kind, L, self.view(L.src), self.view(L.dst)))
@@ -313,15 +304,3 @@ class PFLDLandmarker:
             of = self.ctx.download(self.out_f)
             oi = self.ctx.download(self.out_i)
         return of[:n].reshape(n, LANDMARKS, 2), oi[:n].reshape(n, LANDMARKS, 2)
-
-    def close(self):
-        g = getattr(self, "graph", None)
-        if g is not None:
-            g.close()
-            self.graph = None
-        for t in self._owned:
-            try:
-                self.ctx.free(t)
-            except Exception:
-                pass
-        self._owned = []

@@ -27,6 +27,7 @@ from typing import List, Optional, Tuple
 
 import numpy as np
 
+from .graph import GraphSession, _np
 from .ops import ConvWeight, Ctx, DevTensor
 
 IN_C = 16            # channels of the prepared image (both conv kernels need Cin >= 16)
@@ -73,10 +74,6 @@ def gflop_per_frame(H: int, W: int) -> float:
     return 2.0 * mac / 1e9
 
 
-def _np(t) -> np.ndarray:
-    return t.detach().cpu().float().numpy() if hasattr(t, "detach") else np.asarray(t, np.float32)
-
-
 class S3FDNet:
     """Device-resident S3FD weights: trunk convs, L2Norm scales and the six fused heads."""
 
@@ -114,31 +111,25 @@ def _expected_keys():
     return keys
 
 
-class S3FDDetector:
+class S3FDDetector(GraphSession):
     """One captured graph for batches of N frames of H x W.  keep_layers: every op writes its own buffer (the layer tests read
     them back); otherwise the trunk ping-pongs between two buffers and only the six level features have their own."""
 
     def __init__(self, net: S3FDNet, N: int, H: int, W: int, keep_layers: bool = False, ctx: Optional[Ctx] = None):
         if H < 32 or W < 32:
             raise ValueError(f"S3FD needs frames of at least 32 x 32, got {H} x {W}")
+        super().__init__(ctx)
         self.net, self.N, self.H, self.W = net, int(N), int(H), int(W)
-        self.ctx = ctx or Ctx()
-        self._owned = []
         try:
             self._build(keep_layers)
-        except Exception:
+        except BaseException:
             self.close()
             raise
 
-    def _alloc(self, shape, dtype=np.float16) -> DevTensor:
-        t = self.ctx.alloc(shape, dtype)
-        self._owned.append(t)
-        return t
-
     def _build(self, keep: bool):
         N, H, W = self.N, self.H, self.W
-        self.frames = self._alloc((N, H, W, 3), np.uint8)
-        x0 = self._alloc((N, H, W, IN_C))
+        self.frames = self.alloc((N, H, W, 3), np.uint8)
+        x0 = self.alloc((N, H, W, IN_C))
         self.ops: List[tuple] = [("prep", "prep", self.frames, x0, {})]
         feats = {src for src, _, _, _ in LEVELS}
         # pass 1: shapes, so that the ping-pong buffers can be sized
@@ -155,11 +146,11 @@ class S3FDDetector:
         pp = []
         if not keep:
             big = max(int(np.prod(shape)) for kind, name, shape, _ in plan if name not in feats)
-            pp = [self._alloc((big,)), self._alloc((big,))]
+            pp = [self.alloc((big,)), self.alloc((big,))]
         cur, nxt, fmap = x0, 0, {}
         for kind, name, shape, kw in plan:
             if keep or name in feats:
-                out = self._alloc(shape)
+                out = self.alloc(shape)
             else:
                 if cur.ptr == pp[nxt].ptr:
                     nxt ^= 1
@@ -174,15 +165,15 @@ class S3FDDetector:
             f = fmap[src]
             n_, fh, fw, fc = f.shape
             if normed:
-                g = self._alloc(f.shape) if keep else f          # in place: the pool has already read f
+                g = self.alloc(f.shape) if keep else f          # in place: the pool has already read f
                 self.ops.append(("l2norm", src + "_norm", f, g, dict(npix=n_ * fh * fw, w=self.net.norms[src])))
                 f = g
-            hd = self._alloc((N, fh, fw, HEAD_C))
+            hd = self.alloc((N, fh, fw, HEAD_C))
             self.ops.append(("head", _head_name(src, normed) + "_mbox", f, hd,
                              dict(N=N, IH=fh, IW=fw, OH=fh, OW=fw, stride=(1, 1), pad=(1, 1), relu=False, level=lv)))
             self.heads.append(hd)
-        self.out_i = self._alloc((N, 6), np.int32)
-        self.out_s = self._alloc((N,), np.float32)
+        self.out_i = self.alloc((N, 6), np.int32)
+        self.out_s = self.alloc((N,), np.float32)
         self.ops.append(("select", "select", None, self.out_i, {}))
         self.ctx.sync()
         with self.ctx.capture() as g:
@@ -235,15 +226,3 @@ class S3FDDetector:
     def detect(self, frames_u8: np.ndarray) -> List[Optional[Tuple[int, int, int, int]]]:
         oi, _ = self.run_raw(frames_u8)
         return [tuple(int(v) for v in r[1:5]) if r[0] else None for r in oi]
-
-    def close(self):
-        g = getattr(self, "graph", None)
-        if g is not None:
-            g.close()
-            self.graph = None
-        for t in self._owned:
-            try:
-                self.ctx.free(t)
-            except Exception:
-                pass
-        self._owned = []

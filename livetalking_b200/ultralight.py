@@ -17,7 +17,7 @@ from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
-from .musetalk import Builder, _Replay, _ceil16, _np
+from .graph import Builder, GraphSession, _ceil16, _np
 from .ops import ConvWeight, Ctx, DevTensor, ul_prep_table
 
 CH = [32, 64, 128, 256, 512]          # unet.py:188
@@ -178,16 +178,17 @@ class UltraLightAvatar:
 class UltraLightBank:
     """The weights of up to ``slots`` UltraLight networks, stacked slot by slot: one device buffer (slots, *shape) per weight tensor
     of ``UltraLightModel.weight_tensors()``.  ``slot_of(model)`` loads a network on a miss (stream-ordered device-to-device copies from
-    its resident weights) into a free slot or the least recently used one.  Used by one dispatcher thread only: no lock."""
+    its resident weights) into a free slot or the least recently used one.  Used by one dispatcher thread only: no lock.
+    alloc(shape, dtype, zero=...): where the stacked buffers come from (ctx.alloc unless given; the batch session passes its own)."""
 
-    def __init__(self, ctx: Ctx, template: UltraLightModel, slots: int):
+    def __init__(self, ctx: Ctx, template: UltraLightModel, slots: int, alloc=None):
         self.ctx, self.slots = ctx, int(slots)
         if self.slots < 1:
             raise ValueError("UltraLightBank needs at least one slot")
         ts = template.weight_tensors()
         self._layout = [(t.shape, t.dtype) for t in ts]
         self._index = {id(t): i for i, t in enumerate(ts)}
-        self._bufs = [ctx.alloc((self.slots,) + t.shape, t.dtype, zero=True) for t in ts]
+        self._bufs = [(alloc or ctx.alloc)((self.slots,) + t.shape, t.dtype, zero=True) for t in ts]
         self.nbytes = sum(b.nbytes for b in self._bufs)
         self._model: List[Optional[UltraLightModel]] = [None] * self.slots
         self._used = [0] * self.slots                   # tick of the last slot_of() that returned the slot; 0 = never
@@ -237,41 +238,34 @@ class _Grouping:
         return (self.table, self.images, int(np.prod(w.shape)), int(np.prod(b.shape)))
 
 
-class UltraLightSession:
+class UltraLightSession(GraphSession):
     """One avatar stream at a fixed batch size: captured prep + U-Net + head graph, paste-back buffers."""
 
     def __init__(self, avatar: UltraLightAvatar, batch: int, keep_taps: bool = False, ctx: Optional[Ctx] = None, paste_only: bool = False):
         """paste_only: no network graph and no activation arena — only paste_pred() works (cross-session mode: this session's
         U-Net pass runs in a shared UltraLightBatchSession)."""
+        super().__init__(ctx, with_ctx=not paste_only)
         self.avatar, self.B = avatar, int(batch)
-        self._own_ctx = ctx is None
         self._paste_ctx = None
-        self.graph = None
         if paste_only:
-            self.ctx, self._own_ctx = None, False
             return
-        ctx = self.ctx = Ctx() if ctx is None else ctx
-        B = self.B
-        self.builder = Builder(ctx)
-        self.d_index = ctx.alloc((4,), np.int32, zero=True)
-        self.audio16 = ctx.alloc((B, 32, 32, 16), np.float16, zero=True)           # NHWC view of audiofeat.reshape(16, 32, 32)
-        self.img16 = ctx.alloc((B, FACE, FACE, 16), np.float16, zero=True)
-        self.pred = ctx.alloc((B, FACE, FACE, 3), np.float32, zero=True)
-        self.frames_out = ctx.alloc((B, avatar.H, avatar.W, 3), np.uint8, zero=True)
-        self.taps = {} if keep_taps else None
-        self._paste_ctx = None
+        try:
+            ctx, B = self.ctx, self.B
+            self.d_index = self.alloc((4,), np.int32, zero=True)
+            self.audio16 = self.alloc((B, 32, 32, 16), np.float16, zero=True)           # NHWC view of audiofeat.reshape(16, 32, 32)
+            self.img16 = self.alloc((B, FACE, FACE, 16), np.float16, zero=True)
+            self.pred = self.alloc((B, FACE, FACE, 3), np.float32, zero=True)
+            self.frames_out = self.alloc((B, avatar.H, avatar.W, 3), np.uint8, zero=True)
+            self.taps = {} if keep_taps else None
 
-        def emit():
-            ctx.ul_prep(avatar.faces, avatar.n, self.d_index, B, self.img16)
-            avatar.model.emit(self.builder, self.img16, self.audio16, self.pred, self.taps)
+            def emit(b: Builder):
+                ctx.ul_prep(avatar.faces, avatar.n, self.d_index, B, self.img16)
+                avatar.model.emit(b, self.img16, self.audio16, self.pred, self.taps)
 
-        emit()
-        ctx.sync()
-        temps, self.builder.temps = self.builder.temps, []
-        self.builder.new = _Replay(temps)
-        with ctx.capture() as cap:
-            emit()
-        self.graph = cap.graph
+            self.capture(emit)
+        except BaseException:
+            self.close()
+            raise
 
     # ---- LightReal.inference_batch (ultralight_avatar.py:141-169)
     def infer_async(self, index: int, audio_feats: Optional[np.ndarray] = None):
@@ -320,7 +314,7 @@ class UltraLightSession:
         if not 0 <= idx < a.n:
             raise ValueError("paste_pred: idx out of range")
         if self._paste_ctx is None:
-            self._paste_ctx = Ctx()
+            self._paste_ctx = self.new_ctx()
             self._pred_scratch = self._paste_ctx.alloc((1, FACE, FACE, 3), np.float32)
             self._paste_out = self._paste_ctx.alloc((a.H, a.W, 3), np.uint8)
         pc = self._paste_ctx
@@ -333,25 +327,8 @@ class UltraLightSession:
         self.infer_async(index, None)
         self.paste_batch_async(index)
 
-    def close(self):
-        if getattr(self, "graph", None) is not None:
-            self.graph.close()
-            self.graph = None
-        if self._paste_ctx is not None:
-            self._paste_ctx.close()
-            self._paste_ctx = None
-        if self._own_ctx and self.ctx is not None:
-            self.ctx.close()
-        self.ctx = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class UltraLightBatchSession:
+class UltraLightBatchSession(GraphSession):
     """Cross-session batching for UltraLight: up to G sessions x Bs frames run as ONE captured prep + U-Net + head graph of batch
     G*Bs.  A *group request* is (UltraLightAvatar, first frame index, HuBERT features (Bs, 16, 1024) or None = resident).  Each
     avatar brings its own network: the graph's ops are grouped, group g reads the weights of bank slot group_slot[g] and its crops
@@ -361,38 +338,37 @@ class UltraLightBatchSession:
 
     def __init__(self, template: UltraLightModel, groups: int, frames_per_session: int, slots: Optional[int] = None,
                  return_pred: bool = False, ctx: Optional[Ctx] = None):
+        super().__init__(ctx)
         self.G, self.Bs, self.return_pred = int(groups), int(frames_per_session), bool(return_pred)
         self.batch = self.G                                  # CrossSessionBatcher: requests per engine call
         self.B = B = self.G * self.Bs
-        self._own_ctx = ctx is None
-        ctx = self.ctx = Ctx() if ctx is None else ctx
-        self.bank = UltraLightBank(ctx, template, slots if slots is not None else 2 * self.G)
-        if self.bank.slots < self.G:
-            raise ValueError(f"the bank needs at least {self.G} slots")
-        self.builder = Builder(ctx)
-        self.d_slot = ctx.alloc((self.G,), np.int32, zero=True)
-        self._slot_host = np.zeros(self.G, np.int32)
-        self._blank = ctx.alloc((1, CROP, CROP, 3), np.uint8, zero=True)      # crop source of the groups a call leaves empty
-        self._prep = [(self._blank, 1, 0)] * self.G
-        self.d_prep = ctx.upload(ul_prep_table(self._prep))
-        self.audio16 = ctx.alloc((B, 32, 32, 16), np.float16, zero=True)
-        self.img16 = ctx.alloc((B, FACE, FACE, 16), np.float16, zero=True)
-        self.pred = ctx.alloc((B, FACE, FACE, 3), np.float32, zero=True)
-        self._audio_host = np.zeros((B, 1024, 16), np.float16)
-        self._frames_out: Dict[tuple, DevTensor] = {}
-        grp = _Grouping(self.bank, self.d_slot, self.Bs)
+        try:
+            ctx = self.ctx
+            self.bank = UltraLightBank(ctx, template, slots if slots is not None else 2 * self.G, alloc=self.alloc)
+            if self.bank.slots < self.G:
+                raise ValueError(f"the bank needs at least {self.G} slots")
+            self.d_slot = self.alloc((self.G,), np.int32, zero=True)
+            self._slot_host = np.zeros(self.G, np.int32)
+            self._blank = self.alloc((1, CROP, CROP, 3), np.uint8, zero=True)      # crop source of the groups a call leaves empty
+            self._prep = [(self._blank, 1, 0)] * self.G
+            table = ul_prep_table(self._prep)
+            self.d_prep = self.alloc(table.shape, table.dtype)
+            ctx.h2d(self.d_prep, table)
+            self.audio16 = self.alloc((B, 32, 32, 16), np.float16, zero=True)
+            self.img16 = self.alloc((B, FACE, FACE, 16), np.float16, zero=True)
+            self.pred = self.alloc((B, FACE, FACE, 3), np.float32, zero=True)
+            self._audio_host = np.zeros((B, 1024, 16), np.float16)
+            self._frames_out: Dict[tuple, DevTensor] = {}
+            grp = _Grouping(self.bank, self.d_slot, self.Bs)
 
-        def emit():
-            ctx.ul_prep_grouped(self.d_prep, self.Bs, B, self.img16)
-            template.emit(self.builder, self.img16, self.audio16, self.pred, None, grp)
+            def emit(b: Builder):
+                ctx.ul_prep_grouped(self.d_prep, self.Bs, B, self.img16)
+                template.emit(b, self.img16, self.audio16, self.pred, None, grp)
 
-        emit()
-        ctx.sync()
-        temps, self.builder.temps = self.builder.temps, []
-        self.builder.new = _Replay(temps)
-        with ctx.capture() as cap:
-            emit()
-        self.graph = cap.graph
+            self.capture(emit)
+        except BaseException:
+            self.close()
+            raise
 
     def _check(self, requests):
         if not 1 <= len(requests) <= self.G:
@@ -427,7 +403,7 @@ class UltraLightBatchSession:
     def _out(self, g: int, av: UltraLightAvatar) -> DevTensor:
         key = (g, av.H, av.W)
         if key not in self._frames_out:
-            self._frames_out[key] = self.ctx.alloc((self.Bs, av.H, av.W, 3), np.uint8, zero=True)
+            self._frames_out[key] = self.alloc((self.Bs, av.H, av.W, 3), np.uint8, zero=True)
         return self._frames_out[key]
 
     def paste_async(self, requests: Sequence[tuple]) -> List[DevTensor]:
@@ -458,20 +434,6 @@ class UltraLightBatchSession:
             return outs
 
     infer_slots = infer_groups
-
-    def close(self):
-        if getattr(self, "graph", None) is not None:
-            self.graph.close()
-            self.graph = None
-        if self._own_ctx and self.ctx is not None:
-            self.ctx.close()
-        self.ctx = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def unet_gflop_per_frame() -> float:

@@ -7,13 +7,11 @@ layers over 1500 steps) is assembled from the same engine ops as the UNet and ca
 the log-mel kernels and the per-frame (50, 384) slicing."""
 from __future__ import annotations
 
-import ctypes as C
 from typing import Dict, Optional
 
 import numpy as np
 
-from ._capi import check, lib
-from .musetalk import Builder, _Norm, _np
+from .graph import Builder, GraphSession, _Norm, _np
 from .ops import ConvWeight, Ctx, DevTensor
 
 N_FRAMES, N_MELS, N_BINS, N_SAMPLES = 3000, 80, 201, 480000
@@ -98,7 +96,7 @@ class WhisperEncoder:
         return hidden
 
 
-class WhisperFeatures:
+class WhisperFeatures(GraphSession):
     """audio2feat + WhisperASR slicing for one session: PCM buffer -> (B, 50, D) features, one CUDA graph."""
 
     def __init__(self, enc: WhisperEncoder, batch: int, stride_left: int = 10, stride_right: int = 10, out: Optional[DevTensor] = None,
@@ -106,38 +104,30 @@ class WhisperFeatures:
         """ctx: this extractor's own stream + scratch (created here unless given): WhisperASR.run_step runs on the render
         thread concurrently with inference_batch on the inference thread (avatars/base_avatar.py:483-489 vs :366)."""
         self.enc, self.B = enc, int(batch)
-        self._own_ctx = ctx is None
-        ctx = self.ctx = Ctx() if ctx is None else ctx
         self.n = (stride_left + stride_right + 2 * self.B) * 320
         if self.n > N_SAMPLES:
             raise ValueError("audio window longer than 30 s")
-        self.pcm = ctx.alloc((self.n,), np.float32, zero=True)
-        self.logspec = ctx.alloc((N_MELS * N_FRAMES,), np.float32, zero=True)
-        self.gmax = ctx.alloc((4,), np.int32, zero=True)
-        self.feats16 = ctx.alloc((N_FRAMES, N_MELS), np.float16, zero=True)
-        self.feats32 = ctx.alloc((N_MELS, N_FRAMES), np.float32, zero=True) if keep_hidden else None
-        self.out_rows = out_rows
-        self.out = out if out is not None else ctx.alloc((self.B, out_rows, enc.D), np.float16, zero=True)
-        self.start = stride_left / 2.0
-        self.builder = Builder(ctx)
+        super().__init__(ctx)
+        try:
+            ctx = self.ctx
+            self.pcm = self.alloc((self.n,), np.float32, zero=True)
+            self.logspec = self.alloc((N_MELS * N_FRAMES,), np.float32, zero=True)
+            self.gmax = self.alloc((4,), np.int32, zero=True)
+            self.feats16 = self.alloc((N_FRAMES, N_MELS), np.float16, zero=True)
+            self.feats32 = self.alloc((N_MELS, N_FRAMES), np.float32, zero=True) if keep_hidden else None
+            self.out_rows = out_rows
+            self.out = out if out is not None else self.alloc((self.B, out_rows, enc.D), np.float16, zero=True)
+            self.start = stride_left / 2.0
 
-        def emit():
-            check(lib().ltb_op_whisper_logmel(ctx._h, C.c_void_p(self.pcm.ptr), self.n, C.c_void_p(enc.fb.ptr), C.c_void_p(self.logspec.ptr),
-                                              C.c_void_p(self.gmax.ptr), C.c_void_p(self.feats16.ptr),
-                                              C.c_void_p(self.feats32.ptr) if self.feats32 is not None else None))
-            self.hidden = enc.emit(self.builder, self.feats16)
-            ptrs = (C.c_void_p * 5)(*[h.ptr for h in self.hidden])
-            check(lib().ltb_op_whisper_slice(ctx._h, ptrs, N_FRAMES // 2, enc.D, self.B, float(self.start), 2.0, C.c_void_p(self.out.ptr),
-                                             self.out_rows))
+            def emit(b: Builder):
+                ctx.whisper_logmel(self.pcm, self.n, enc.fb, self.logspec, self.gmax, self.feats16, self.feats32)
+                self.hidden = enc.emit(b, self.feats16)
+                ctx.whisper_slice(self.hidden, N_FRAMES // 2, enc.D, self.B, self.start, 2.0, self.out, self.out_rows)
 
-        emit()
-        ctx.sync()
-        from .musetalk import _Replay
-        temps, self.builder.temps = self.builder.temps, []
-        self.builder.new = _Replay(temps)
-        with ctx.capture() as cap:
-            emit()
-        self.graph = cap.graph
+            self.capture(emit)
+        except BaseException:
+            self.close()
+            raise
 
     def run_async(self, pcm: Optional[np.ndarray] = None):
         if pcm is not None:
@@ -153,17 +143,3 @@ class WhisperFeatures:
             self.run_async(pcm)
             full = self.ctx.download(self.out)
         return full[:, :50]
-
-    def close(self):
-        if getattr(self, "graph", None) is not None:
-            self.graph.close()
-            self.graph = None
-        if self._own_ctx and self.ctx is not None:
-            self.ctx.close()
-        self.ctx = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass

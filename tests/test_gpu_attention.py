@@ -344,7 +344,7 @@ def test_builder_attention_hubert_grouped(ctx, monkeypatch, fused):
     O W_o^T + b_o + res from the engine's own fp16 O within 1024 2^-23 (|O| |W_o|^T + |b_o| + |res|) (fp32 accumulation) plus
     2^-11 |ref| + 2^-25 (fp16 rounding)."""
     from livetalking_b200.hubert import _HAttn
-    from livetalking_b200.musetalk import Builder
+    from livetalking_b200.graph import Builder
     monkeypatch.setattr(Builder, "FUSE_ATTENTION", fused)
     G, T, H, d = 3, 27, 16, 64
     D = H * d

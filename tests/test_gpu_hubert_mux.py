@@ -122,7 +122,7 @@ def test_partial_rounds_match_the_full_round(hubert):
 def test_grouped_attention_without_the_fused_kernel(hubert, monkeypatch):
     """Builder.attention with batch G and a key count that is not a multiple of 16 on the GEMM + softmax + GEMM path."""
     from livetalking_b200.hubert import HubertBatchFeatures, HubertFeatures
-    from livetalking_b200.musetalk import Builder
+    from livetalking_b200.graph import Builder
     _model, enc = hubert
     monkeypatch.setattr(Builder, "FUSE_ATTENTION", False)
     G, B = 3, 4

@@ -154,7 +154,7 @@ class _UlNet:
 
     def __init__(self, model, sd):
         from livetalking_b200.ultralight import _fold
-        from livetalking_b200.musetalk import _np
+        from livetalking_b200.graph import _np
         self.model, self.w, self.names = model, {}, {}
         for blk, p in _prefixes(model):
             hid = int(_np(sd[p + ".conv.0.weight"]).shape[0])
@@ -444,7 +444,7 @@ class _Sub:
 def test_unet_every_op_against_float64(ul, run):
     """UltraLightSession's op sequence (set_i32 + h2d + ul_prep + UltraLightModel.emit) traced eagerly; every op of the checked
     images against float64, and UltraLightSession.infer must give the traced pass's pred bit for bit."""
-    from livetalking_b200.musetalk import Builder
+    from livetalking_b200.graph import Builder
     from livetalking_b200.ops import Ctx
     from livetalking_b200.ultralight import UltraLightSession
     nets, avs = ul
@@ -485,7 +485,7 @@ def test_grouped_unet_every_op_against_float64(ul):
     one slot used by two groups.  The grouped op sequence (ul_prep_grouped + emit with the session's _Grouping) is traced
     eagerly over the session's bank and tables; every op of GROUP_IMAGES (each group's) against float64 with that image's network,
     and the session's pred (return_pred) must equal the traced pass's bit for bit."""
-    from livetalking_b200.musetalk import Builder
+    from livetalking_b200.graph import Builder
     from livetalking_b200.ops import Ctx
     from livetalking_b200.ultralight import UltraLightBatchSession, _Grouping
     nets, avs = ul
@@ -712,7 +712,7 @@ def test_hubert_every_op_against_float64(hubert, run):
     """HubertEncoder.emit (G = 1) / emit_grouped (G = 3) over B = 16 windows traced eagerly, every op on every row against float64;
     the production graph (HubertFeatures / HubertBatchFeatures) must give the traced hidden states bit for bit."""
     from livetalking_b200.hubert import HubertBatchFeatures, HubertFeatures, window_samples
-    from livetalking_b200.musetalk import Builder
+    from livetalking_b200.graph import Builder
     from livetalking_b200.ops import Ctx
     enc, sd = hubert
     G = HUBERT_RUNS[run]
