@@ -184,6 +184,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
   const uint32_t a_smem = smem0;
   const uint32_t b_smem = smem0 + C::A_STAGES * C::A_BYTES;
   const int chunks = (p.Cin + 63) / 64;
+  const int kl_last = (p.Cin - 64 * (chunks - 1) + 15) / 16;   // K steps of 16 channels in the last chunk
 
   if (tid == 0) {
     for (int s = 0; s < C::A_STAGES; ++s) {
@@ -341,8 +342,9 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
       const int cb_res = (BN == 32) ? (n0_res & 63) >> 3 : 0;              // first 8-channel block of the tile in its chunk
       uint32_t pend_as = 0, pend_bs = 0;   // stages of the previous chunk (LAG mode), released once its wgmma group retired
       bool pend = false;
-#pragma unroll 1
-      for (int c = 0; c < chunks; ++c) {
+      // K chunk c, KL K steps of 16 channels per weight stage
+      auto run_chunk = [&](int c, auto kl_t) {
+        constexpr int KL = decltype(kl_t)::value;
         const uint32_t as = ai % C::A_STAGES;
         mbar_wait(smem_u32(&a_full[as]), (ai / C::A_STAGES) & 1u);
         if constexpr (kResHalo) {
@@ -371,9 +373,8 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
           if (!RC) mbar_wait(smem_u32(&b_full[bs]), ((bi + j) / C::B_STAGES) & 1u);
           const uint32_t b_lo0 = wgmma_lo(b_smem + bs * C::B_BYTES);
           if (!LTB_DIAG(4)) wgmma_fence();
-          // all four K steps, also in a ragged last chunk: TMA zero-fills the channels >= Cin of both operands
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
+          for (int k = 0; k < KL; ++k) {
             if (LTB_DIAG(4)) break;
             if constexpr (NACC == 1) {
 #pragma unroll
@@ -417,7 +418,18 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
         }
         ++ai;
         if (!RC) bi += C::TG;
-      }
+      };
+      // A last chunk that holds at most 32 channels issues only its first two K steps: TMA zero-fills the rest of both operands,
+      // whose products would add exact zeros.  It runs after the loop over the full chunks as a separate unrolled chunk body, so
+      // that no branch sits between MMAs.  One such body, not one per step count: every extra body made the kernel's code larger
+      // and the full-chunk layers slower (per-op events on an H100 80GB HBM3, 700 W limit: 2-5 us on the 128-channel and ConvT
+      // layers of the wav2lip256 decoder with bodies for one, two and three steps), while two steps cover the 16- and 32-channel
+      // remainders of wav2lip256 (L15/L16, L50, L53 and the audio encoder, all BN <= 64).  The BN = 128 instances, already the
+      // largest (the two-step body took <128, 2, 1> from 6.7 k to 7.1 k SASS lines), keep four steps in every chunk.
+      const bool ragged = BN <= 64 && kl_last <= 2;
+#pragma unroll 1
+      for (int c = 0; c < chunks - ragged; ++c) run_chunk(c, std::integral_constant<int, 4>{});
+      if (ragged) run_chunk(chunks - 1, std::integral_constant<int, 2>{});
       if constexpr (C::RES_PREFETCH) {
         if (res_pf) {   // under the last chunk's MMAs
 #pragma unroll
@@ -464,6 +476,8 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
         const __half2 o = __hmin2(__hmax2(__hadd2(*reinterpret_cast<const __half2*>(&v), *reinterpret_cast<const __half2*>(&r)), hlo), hmax);
         return *reinterpret_cast<const uint32_t*>(&o);
       };
+      // fused head: the lane's channel-pair words of its rows (sub, hh), row 2 sub + hh (unused rows of NSUB = 1 stay zero)
+      uint32_t hrow[4][4] = {};
 #pragma unroll
       for (int sub = 0; sub < NSUB; ++sub) {
         // GroupNorm partial sums of this warp's 16 rows, per 8-column block
@@ -532,38 +546,9 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
                 gq[i] += f.x * f.x + f.y * f.y;
               }
             }
-            if constexpr (kHeadOk) {
-              if (head) {
-                // the four lanes of a row hold channels 8i + 2(lane%4) (+1): gather all 32 at the row's first lane and sum them in
-                // channel order (the order of w2l_head_kernel, so the fused head is bit-identical to the separate one)
-                uint32_t hv[4][4];
+            if constexpr (kHeadOk)
 #pragma unroll
-                for (int src = 0; src < 4; ++src)
-#pragma unroll
-                  for (int i = 0; i < 4; ++i)
-                    hv[src][i] = __shfl_sync(0xffffffffu, *reinterpret_cast<uint32_t*>(&oh[i]), (lane & ~3) + src);
-                if ((lane & 3) == 0 && row_ok) {
-                  float ha0 = head_sw[96], ha1 = head_sw[97], ha2 = head_sw[98];
-#pragma unroll
-                  for (int i = 0; i < 4; ++i)
-#pragma unroll
-                    for (int src = 0; src < 4; ++src) {
-                      const float2 f = __half22float2(*reinterpret_cast<__half2*>(&hv[src][i]));
-                      const int cc = 8 * i + 2 * src;
-                      ha0 = fmaf(f.x, head_sw[cc], ha0);
-                      ha0 = fmaf(f.y, head_sw[cc + 1], ha0);
-                      ha1 = fmaf(f.x, head_sw[32 + cc], ha1);
-                      ha1 = fmaf(f.y, head_sw[32 + cc + 1], ha1);
-                      ha2 = fmaf(f.x, head_sw[64 + cc], ha2);
-                      ha2 = fmaf(f.y, head_sw[64 + cc + 1], ha2);
-                    }
-                  float* o = p.head_out + opix * 3;
-                  o[0] = (1.f / (1.f + expf(-ha0))) * 255.f;
-                  o[1] = (1.f / (1.f + expf(-ha1))) * 255.f;
-                  o[2] = (1.f / (1.f + expf(-ha2))) * 255.f;
-                }
-              }
-            }
+              for (int i = 0; i < 4; ++i) hrow[2 * sub + hh][i] = *reinterpret_cast<const uint32_t*>(&oh[i]);
           }
         }
         // GEMM mode: a warp whose 16 rows all lie at or past M (the second sub-tile of a ragged last tile) has nothing to add, and
@@ -593,6 +578,44 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
               atomicAdd(sbase + 2 * g, a);
               atomicAdd(sbase + 2 * g + 1, b);
             }
+          }
+        }
+      }
+      if constexpr (kHeadOk) {
+        if (head) {
+          // The four lanes of a quad share its 2 * NSUB rows and each holds channels 8i + 2(lane%4) (+1) of them.  A 4 x 4 word
+          // transpose per 8-channel block i gives lane q all 32 channels of row q, and the lane computes the row's three outputs,
+          // each summed in channel order (the order of w2l_head_kernel, so the fused head is bit-identical to the separate one).
+          uint32_t hv[4][4];   // [src][i]: channels 8i + 2 src (+1) of row q
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            uint32_t x[4] = {hrow[0][i], hrow[1][i], hrow[2][i], hrow[3][i]};
+            quad_transpose(x, lane);
+#pragma unroll
+            for (int src = 0; src < 4; ++src) hv[src][i] = x[src];
+          }
+          const int q = lane & 3;
+          bool row_ok = false;
+          const size_t opix = halo_pix(img, ty, tx, q >> 1, 0, wq * 16 + (lane >> 2) + 8 * (q & 1), row_ok);
+          if (q < 2 * NSUB && row_ok) {
+            float ha0 = head_sw[96], ha1 = head_sw[97], ha2 = head_sw[98];
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+              for (int src = 0; src < 4; ++src) {
+                const float2 f = __half22float2(*reinterpret_cast<__half2*>(&hv[src][i]));
+                const int cc = 8 * i + 2 * src;
+                ha0 = fmaf(f.x, head_sw[cc], ha0);
+                ha0 = fmaf(f.y, head_sw[cc + 1], ha0);
+                ha1 = fmaf(f.x, head_sw[32 + cc], ha1);
+                ha1 = fmaf(f.y, head_sw[32 + cc + 1], ha1);
+                ha2 = fmaf(f.x, head_sw[64 + cc], ha2);
+                ha2 = fmaf(f.y, head_sw[64 + cc + 1], ha2);
+              }
+            float* o = p.head_out + opix * 3;
+            o[0] = (1.f / (1.f + expf(-ha0))) * 255.f;
+            o[1] = (1.f / (1.f + expf(-ha1))) * 255.f;
+            o[2] = (1.f / (1.f + expf(-ha2))) * 255.f;
           }
         }
       }
