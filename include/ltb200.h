@@ -359,6 +359,25 @@ int ltb_op_pfld_prep(ltb_ctx* c, const void* bgr_u8, int N, int H, int W, void* 
 int ltb_op_pfld_head(ltb_ctx* c, const void* const* taps5, const int* hw5, const int* pitch5, const int* nch5, const int* ch, int N,
                      const float* wt, const float* bias, const float* mean, const int* crop_wh, int nout, float* out_f32, int* out_i32);
 
+/* BiSeNet face parser of the MuseTalk avatar generator (avatars/musetalk/utils/face_parsing); the convolutions run on ltb_op_conv2d,
+ * these are the ops around them (livetalking_b200/bisenet.py).
+ * prep: u8 RGB [N,512,512,3] -> fp16 [N,259,259,16]: (v / 255 - mean) / std in fp32, space-to-depth 2x2 (channel (2 by + bx) * 3 + c
+ * holds input pixel (2 (y - 2) + by, 2 (x - 2) + bx)), zero outside the image and in channels 12-15. */
+int ltb_op_bisenet_prep(ltb_ctx* c, const void* rgb_u8, int N, void* out);
+/* MaxPool2d(3, stride 2, pad 1) on fp16 NHWC [N,H,W,C] (C % 8 == 0) -> [N,(H-1)/2+1,(W-1)/2+1,C]. */
+int ltb_op_maxpool3x3s2(ltb_ctx* c, const void* x, int N, int H, int W, int C, void* out);
+/* Per image n: a = fp32 mean over the HW pixels of x[n][.][c_off + c] (pitch halves per pixel, c < C), h = act1(w1t^T a + b1) (w1t fp32
+ * [C][n1]); with w2t: out[n] = act2(w2t^T h + b2) (w2t [n1][n2]), else out[n] = h.  act: 0 none, 1 ReLU, 2 sigmoid.  b1 / b2 may be
+ * null (no bias).  C, n1, n2 <= 512. */
+int ltb_op_chan_gate(ltb_ctx* c, const void* x, int N, int HW, int C, int pitch, int c_off, const float* w1t, const float* b1, int n1, int act1,
+                     const float* w2t, const float* b2, int n2, int act2, float* out);
+/* out[n][p][ooff + c] = fp16(x[n][p][xoff + c] * g[n][c] + y), y = yvec[n][c] (mode 0), y[n][p][yoff + c] (mode 1) or x (mode 2). */
+int ltb_op_chan_scale_add(ltb_ctx* c, const void* x, int N, int HW, int C, int xpitch, int xoff, const float* g, int mode, const float* yvec,
+                          const void* y, int ypitch, int yoff, void* out, int opitch, int ooff);
+/* Bilinear align_corners=True resize of fp16 logits [N,IH,IW,pitch] to OH x OW and the arg-max over channels [0, ncls) (ties: the
+ * lowest class) -> u8 labels [N,OH,OW]. */
+int ltb_op_bisenet_upsample_argmax(ltb_ctx* c, const void* logits, int N, int IH, int IW, int pitch, int ncls, int OH, int OW, void* labels);
+
 #ifdef __cplusplus
 }
 #endif

@@ -164,6 +164,14 @@ _SIGS = {
     "ltb_op_pfld_head": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
                                    C.POINTER(C.c_int), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                    C.c_void_p]),
+    "ltb_op_bisenet_prep": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
+    "ltb_op_maxpool3x3s2": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "ltb_op_chan_gate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                   C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "ltb_op_chan_scale_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                        C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]),
+    "ltb_op_bisenet_upsample_argmax": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                 C.c_void_p]),
     "ltb_conv2d_f16": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ltb_conv2d_f16_timed": (C.c_int, [C.POINTER(ConvDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                        C.POINTER(C.c_float)]),

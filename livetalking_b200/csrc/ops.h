@@ -112,4 +112,38 @@ cudaError_t launch_pfld_prep(const uint8_t* bgr, int N, int H, int W, __half* ou
 cudaError_t launch_pfld_head(const PfldTaps& taps, int N, const float* wt, const float* bias, const float* mean, const int* crop_wh, int nout,
                              float* out_f, int* out_i, cudaStream_t st);
 
+// BiSeNet face-parsing glue (bisenet.cu)
+constexpr int kBisenetIn = 512;    // FaceParsing resizes every crop to 512 x 512
+constexpr int kBisenetS2d = 259;   // space-to-depth 2 x 2 map of the stem: 2 pixels of zero border before, 1 after
+constexpr int kBisenetInC = 16;    // 12 real channels ((by, bx, c) order), zero-padded
+constexpr int kChanGateMax = 512;  // chan_gate: largest C, n1, n2
+enum { kActNone = 0, kActRelu = 1, kActSigmoid = 2 };
+enum { kScaleAddVec = 0, kScaleAddTensor = 1, kScaleAddSelf = 2 };
+struct ChanGateArgs {              // x: [N][HW][pitch] fp16, channels [c_off, c_off + C); w1t fp32 [C][n1], w2t [n1][n2] (null: one layer)
+  const __half* x;
+  int N, HW, C, pitch, c_off;
+  const float *w1t, *b1;
+  int n1, act1;
+  const float *w2t, *b2;
+  int n2, act2;
+  float* out;                      // [N][n2] (or [N][n1])
+};
+struct ChanScaleAddArgs {          // out = x * g[n][c] + (yvec[n][c] | y | x); x / y / out: [N][HW][pitch] fp16 channel slices
+  const __half* x;
+  int N, HW, C, xpitch, xoff;
+  const float* g;
+  int mode;
+  const float* yvec;
+  const __half* y;
+  int ypitch, yoff;
+  __half* out;
+  int opitch, ooff;
+};
+cudaError_t launch_bisenet_prep(const uint8_t* rgb, int N, __half* out, cudaStream_t st);
+cudaError_t launch_maxpool3x3s2(const __half* x, int N, int H, int W, int C, __half* out, cudaStream_t st);
+cudaError_t launch_chan_gate(const ChanGateArgs& a, cudaStream_t st);
+cudaError_t launch_chan_scale_add(const ChanScaleAddArgs& a, cudaStream_t st);
+cudaError_t launch_bisenet_upsample_argmax(const __half* logits, int N, int IH, int IW, int pitch, int ncls, int OH, int OW, uint8_t* out,
+                                           cudaStream_t st);
+
 }  // namespace ltb

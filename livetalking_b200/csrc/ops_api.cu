@@ -588,6 +588,59 @@ int ltb_op_pfld_head(ltb_ctx* c, const void* const* taps5, const int* hw5, const
   c->launches += 1;
   return 0;
 }
+// ---- BiSeNet face-parsing glue (bisenet.cu)
+int ltb_op_bisenet_prep(ltb_ctx* c, const void* rgb_u8, int N, void* out) {
+  if (!c || !rgb_u8 || !out) return LTB_FAIL("bisenet_prep: null argument");
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_bisenet_prep(static_cast<const uint8_t*>(rgb_u8), N, static_cast<__half*>(out), c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("bisenet_prep (N > 0, 16-byte aligned output): ") + cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
+int ltb_op_maxpool3x3s2(ltb_ctx* c, const void* x, int N, int H, int W, int C, void* out) {
+  if (!c || !x || !out) return LTB_FAIL("maxpool3x3s2: null argument");
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_maxpool3x3s2(static_cast<const __half*>(x), N, H, W, C, static_cast<__half*>(out), c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("maxpool3x3s2 (C % 8 == 0, 16-byte aligned): ") + cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
+int ltb_op_chan_gate(ltb_ctx* c, const void* x, int N, int HW, int C, int pitch, int c_off, const float* w1t, const float* b1, int n1, int act1,
+                     const float* w2t, const float* b2, int n2, int act2, float* out) {
+  if (!c || !x || !w1t || !out) return LTB_FAIL("chan_gate: null argument");
+  ChanGateArgs a{static_cast<const __half*>(x), N, HW, C, pitch, c_off, w1t, b1, n1, act1, w2t, b2, n2, act2, out};
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_chan_gate(a, c->st);
+  if (e != cudaSuccess)
+    return LTB_FAIL(std::string("chan_gate (C, pitch, c_off % 8 == 0, C, n1, n2 <= 512, act in 0..2, 16-byte aligned x): ") +
+                    cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
+int ltb_op_chan_scale_add(ltb_ctx* c, const void* x, int N, int HW, int C, int xpitch, int xoff, const float* g, int mode, const float* yvec,
+                          const void* y, int ypitch, int yoff, void* out, int opitch, int ooff) {
+  if (!c || !x || !g || !out) return LTB_FAIL("chan_scale_add: null argument");
+  ChanScaleAddArgs a{static_cast<const __half*>(x), N, HW, C, xpitch, xoff, g, mode, yvec, static_cast<const __half*>(y), ypitch, yoff,
+                     static_cast<__half*>(out), opitch, ooff};
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_chan_scale_add(a, c->st);
+  if (e != cudaSuccess)
+    return LTB_FAIL(std::string("chan_scale_add (C, pitches, offsets % 8 == 0, mode 0..2 with its operand, 16-byte aligned): ") +
+                    cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
+int ltb_op_bisenet_upsample_argmax(ltb_ctx* c, const void* logits, int N, int IH, int IW, int pitch, int ncls, int OH, int OW, void* labels) {
+  if (!c || !logits || !labels) return LTB_FAIL("bisenet_upsample_argmax: null argument");
+  LTB_CTX_ENTER(c);
+  cudaError_t e = launch_bisenet_upsample_argmax(static_cast<const __half*>(logits), N, IH, IW, pitch, ncls, OH, OW, static_cast<uint8_t*>(labels),
+                                                 c->st);
+  if (e != cudaSuccess)
+    return LTB_FAIL(std::string("bisenet_upsample_argmax (pitch % 8 == 0 covering ncls rounded up to 8, 16-byte aligned logits): ") +
+                    cudaGetErrorString(e));
+  c->launches += 1;
+  return 0;
+}
 int ltb_op_vae_pre(ltb_ctx* c, const void* img_u8, int N, int H, int W, int half_mask, void* out) {
   if (!c || !img_u8 || !out) return LTB_FAIL("vae_pre: null argument");
   LTB_CTX_ENTER(c);

@@ -382,6 +382,47 @@ class Ctx:
         check(lib().ltb_op_pfld_head(self._h, ptrs, hw, pitch, nch, ch, N, C.c_void_p(wt.ptr), C.c_void_p(bias.ptr), C.c_void_p(mean.ptr),
                                      C.c_void_p(crop_wh.ptr), int(bias.shape[0]), C.c_void_p(out_f32.ptr), C.c_void_p(out_i32.ptr)))
 
+    # ---- BiSeNet face parser (livetalking_b200/bisenet.py)
+    ACT_NONE, ACT_RELU, ACT_SIGMOID = 0, 1, 2
+
+    def bisenet_prep(self, rgb_u8: DevTensor, N: int, out: DevTensor):
+        """u8 RGB [N,512,512,3] -> fp16 [N,259,259,16]: normalised, space-to-depth 2x2, zero border."""
+        check(lib().ltb_op_bisenet_prep(self._h, C.c_void_p(rgb_u8.ptr), N, C.c_void_p(out.ptr)))
+
+    def maxpool3x3s2(self, x: DevTensor, N: int, H: int, W: int, out: DevTensor):
+        """Dense NHWC maps only: the op has no pitch or channel offset."""
+        _dense("maxpool3x3s2", x, out)
+        check(lib().ltb_op_maxpool3x3s2(self._h, C.c_void_p(x.ptr), N, H, W, x.C, C.c_void_p(out.ptr)))
+
+    def chan_gate(self, x: DevTensor, N: int, w1t: DevTensor, b1: Optional[DevTensor], act1: int, out: DevTensor,
+                  w2t: Optional[DevTensor] = None, b2: Optional[DevTensor] = None, act2: int = 0):
+        """out fp32 [N, n] = act2(w2t^T act1(w1t^T mean_hw(x) + b1) + b2) (one layer when w2t is None); w1t fp32 [C, n1]."""
+        hw = int(np.prod(x.shape[1:-1]))
+        n2 = int(w2t.shape[1]) if w2t is not None else 0
+        check(lib().ltb_op_chan_gate(self._h, C.c_void_p(x.ptr), N, hw, x.C, x.pitch, x.c_off, C.c_void_p(w1t.ptr),
+                                     C.c_void_p(b1.ptr) if b1 is not None else None, int(w1t.shape[1]), act1,
+                                     C.c_void_p(w2t.ptr) if w2t is not None else None, C.c_void_p(b2.ptr) if b2 is not None else None, n2,
+                                     act2, C.c_void_p(out.ptr)))
+
+    def chan_scale_add(self, x: DevTensor, N: int, g: DevTensor, out: DevTensor, yvec: Optional[DevTensor] = None,
+                       y: Optional[DevTensor] = None):
+        """out = x * g[n, c] + y, y the fp32 [N, C] vector yvec, the fp16 tensor y, or x itself when neither is given."""
+        hw = int(np.prod(x.shape[1:-1]))
+        mode = 0 if yvec is not None else (1 if y is not None else 2)
+        check(lib().ltb_op_chan_scale_add(self._h, C.c_void_p(x.ptr), N, hw, x.C, x.pitch, x.c_off, C.c_void_p(g.ptr), mode,
+                                          C.c_void_p(yvec.ptr) if yvec is not None else None, C.c_void_p(y.ptr) if y is not None else None,
+                                          y.pitch if y is not None else 0, y.c_off if y is not None else 0, C.c_void_p(out.ptr), out.pitch,
+                                          out.c_off))
+
+    def bisenet_upsample_argmax(self, logits: DevTensor, N: int, ncls: int, out_u8: DevTensor):
+        """fp16 logits [N,h,w,pitch] -> u8 [N,H,W] (out_u8's shape): bilinear align_corners=True, arg-max over ncls classes."""
+        if logits.c_off:
+            raise ValueError("bisenet_upsample_argmax: the logits must start at channel 0 of their pitch")
+        _dense("bisenet_upsample_argmax", out_u8)
+        _, IH, IW, _ = logits.shape
+        check(lib().ltb_op_bisenet_upsample_argmax(self._h, C.c_void_p(logits.ptr), N, IH, IW, logits.pitch, ncls, out_u8.shape[1],
+                                                   out_u8.shape[2], C.c_void_p(out_u8.ptr)))
+
     def close(self):
         if self._h:
             lib().ltb_ctx_destroy(self._h)
@@ -392,6 +433,12 @@ class Ctx:
             self.close()
         except Exception:
             pass
+
+
+def _dense(op: str, *ts: DevTensor):
+    for t in ts:
+        if t.pitch != t.C or t.c_off:
+            raise ValueError(f"{op}: expects dense tensors, got a channel slice (C {t.C}, pitch {t.pitch}, offset {t.c_off})")
 
 
 def ul_prep_table(groups) -> np.ndarray:

@@ -20,7 +20,8 @@ def install_aliases():
                          ("livetalking_b200.plugin.ultralight_avatar", "avatars.ultralight_avatar"),
                          ("livetalking_b200.plugin.hubert_asr", "avatars.audio_features.hubert"),
                          ("livetalking_b200.plugin.wav2lip_genavatar", "avatars.wav2lip.genavatar"),
-                         ("livetalking_b200.plugin.ultralight_genavatar", "avatars.ultralight.genavatar")):
+                         ("livetalking_b200.plugin.ultralight_genavatar", "avatars.ultralight.genavatar"),
+                         ("livetalking_b200.plugin.musetalk_genavatar", "avatars.musetalk.genavatar")):
         sys.modules[theirs] = importlib.import_module(ours)
 
 
