@@ -649,8 +649,8 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-static bool encode(CUtensorMap* tm, int rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                   const cuuint32_t* box, int spatial_stride = 1) {
+bool encode_tmap_f16(CUtensorMap* tm, int rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
+                     const cuuint32_t* box, int spatial_stride) {
   EncodeTiledFn fn = get_encode();
   if (!fn) return false;
   cuuint32_t es[5] = {1, (cuuint32_t)spatial_stride, (cuuint32_t)spatial_stride, 1, 1};   // traversal stride of the W and H dimensions
@@ -810,12 +810,12 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
     cuuint64_t dims[2] = {(cuuint64_t)p.Cin, (cuuint64_t)p.M};
     cuuint64_t strides[1] = {(cuuint64_t)p.ICtot * 2};
     cuuint32_t box[2] = {64, (cuuint32_t)(128 * NSUB)};
-    if (!encode(&h.tm_in, 2, p.in + p.ic_off, dims, strides, box)) return 2;
+    if (!encode_tmap_f16(&h.tm_in, 2, p.in + p.ic_off, dims, strides, box)) return 2;
     // grouped: 3-D (K, Cout, slot) over the whole bank, one slot per box
     cuuint64_t wdims[3] = {(cuuint64_t)p.Cin, (cuuint64_t)p.Cout, (cuuint64_t)p.slots};
     cuuint64_t wstrides[2] = {(cuuint64_t)p.Ktot * 2, (cuuint64_t)p.w_slot_stride * 2};
     cuuint32_t wbox[3] = {64, (cuuint32_t)BN, 1};
-    if (!encode(&h.tm_w, p.group_slot ? 3 : 2, p.w + p.ph[0].koff, wdims, wstrides, wbox)) return 2;
+    if (!encode_tmap_f16(&h.tm_w, p.group_slot ? 3 : 2, p.w + p.ph[0].koff, wdims, wstrides, wbox)) return 2;
   } else
   // input: 4-D (C, W, H, N) view of the NHWC channel slice
   {
@@ -826,7 +826,7 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
       box[1] = 2 * 9 - 1;
       box[2] = 2 * (16 * NSUB + 1) - 1;
     }
-    if (!encode(&h.tm_in, 4, p.in + p.ic_off, dims, strides, box, s2 ? 2 : 1)) return 2;
+    if (!encode_tmap_f16(&h.tm_in, 4, p.in + p.ic_off, dims, strides, box, s2 ? 2 : 1)) return 2;
   }
   // weights: 3-D (k = Cin, n = Cout, tap = 9) view of the tap-major copy [9][Cout][Cin]
   if (up) {
@@ -834,12 +834,12 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
     cuuint64_t dims[3] = {(cuuint64_t)p.Cin, (cuuint64_t)p.Cout, 16};
     cuuint64_t strides[2] = {(cuuint64_t)p.Cin * 2, (cuuint64_t)p.Cout * p.Cin * 2};
     cuuint32_t box[3] = {64, (cuuint32_t)BN, 4};
-    if (!encode(&h.tm_w, 3, w_tap_major, dims, strides, box)) return 2;
+    if (!encode_tmap_f16(&h.tm_w, 3, w_tap_major, dims, strides, box)) return 2;
   } else if (!gemm) {
     cuuint64_t dims[3] = {(cuuint64_t)p.Cin, (cuuint64_t)p.Cout, 9};
     cuuint64_t strides[2] = {(cuuint64_t)p.Cin * 2, (cuuint64_t)p.Cout * p.Cin * 2};
     cuuint32_t box[3] = {64, (cuuint32_t)BN, 3};
-    if (!encode(&h.tm_w, 3, w_tap_major, dims, strides, box)) return 2;
+    if (!encode_tmap_f16(&h.tm_w, 3, w_tap_major, dims, strides, box)) return 2;
   }
   h.out = p.out;
   h.res = p.res;

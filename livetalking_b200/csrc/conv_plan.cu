@@ -89,12 +89,18 @@ ConvParams conv_params(ConvMode mode, int N, ConvSlice in, int IH, int IW, int C
 int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan* out) {
   out->p = p;
   out->halo = false;
+  out->pingpong = false;
   if (p.group_slot) {
     if (p.group_images < 1 || p.N % p.group_images || p.slots < 1 || p.w_slot_stride < 0 || p.bias_slot_stride < 0)
       return LTB_FAIL("conv: grouped weights need N divisible by group_images >= 1, slots >= 1 and non-negative slot strides");
     if (p.zbatch > 1 || p.upconv) return LTB_FAIL("conv: grouped weights cannot be combined with zbatch or the fused upsample");
   }
   if (path == ConvPath::Gather) return 0;
+  if (w_tap && conv_pingpong_supported(p)) {
+    if (conv_pingpong_make_plan(p, w_tap, &out->pp) != 0) return LTB_FAIL("conv: ping-pong plan / tensor map creation failed");
+    out->pingpong = true;
+    return 0;
+  }
   const bool gemm = p.nphases == 1 && p.ph[0].ntaps == 1;   // the halo kernel's GEMM mode reads the K-major rows
   if (!((w_tap || gemm) && conv_halo_supported(p))) {
     if (path == ConvPath::Auto) return 0;
@@ -108,12 +114,23 @@ int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan*
 }
 
 cudaError_t conv_launch(const ConvPlan& pl, cudaStream_t st, float* splitk_ws, size_t ws_floats) {
+  if (pl.pingpong) return launch_conv_pingpong(pl.pp, st);
   return pl.halo ? launch_conv_halo(pl.hp, st) : launch_conv_gather(pl.p, st, splitk_ws, ws_floats);
 }
 
 bool conv_plan_variant(const ConvPlan& pl, bool have_ws, size_t ws_floats, ltb_conv_variant* out) {
   std::memset(out, 0, sizeof(*out));
   out->grouped = pl.p.group_slot != nullptr;
+  if (pl.pingpong) {   // one instance: 3x3, 64 output channels, one 128-pixel tile per warpgroup, resident weights
+    out->kernel = 2;
+    out->taps = 9;
+    out->bn = 64;
+    out->nsub = 1;
+    out->nacc = 1;
+    out->resident_chunks = 1;
+    out->res_halo = 1;
+    return true;
+  }
   if (pl.halo) {
     out->kernel = 1;
     out->taps = pl.hp.TAPS;
@@ -250,7 +267,7 @@ static int conv2d_f16_impl(const ltb_conv_desc* d, const void* in_f16, const flo
     cleanup();
     return 1;
   }
-  const size_t ws_floats = pl.halo ? 0 : (size_t)1 << 22;
+  const size_t ws_floats = (pl.halo || pl.pingpong) ? 0 : (size_t)1 << 22;
   if (ws_floats) {
     CK(cudaMalloc(&dws, ws_floats * sizeof(float)));
     CK(cudaMemset(dws, 0, ws_floats * sizeof(float)));

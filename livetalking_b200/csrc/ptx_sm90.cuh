@@ -109,6 +109,46 @@ __device__ __forceinline__ void ldmatrix_x4(uint32_t& r0, uint32_t& r1, uint32_t
                : "memory");
 }
 
+// the same four matrices transposed: lane l receives column l/4, elements 2(l%4) (+1), i.e. (row 2(l%4) (+1), column l/4)
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3, uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(saddr)
+               : "memory");
+}
+// inverse of ldmatrix_x4_trans: lane l's words are (row 2(l%4) (+1), column l/4) of the four matrices whose row addresses
+// lanes 8k..8k+7 give
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t saddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
+               : "memory");
+}
+
+// ---------------------------------------------------------------- TMA store (bulk async group)
+__device__ __forceinline__ void tma_store_4d(const void* tmap, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(tmap), "r"(src), "r"(c0),
+               "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the shared-memory sources of all but the newest N bulk groups have been read (they may be overwritten)
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// the bulk groups but the newest N have completed their global writes
+template <int N>
+__device__ __forceinline__ void bulk_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+
+// ---------------------------------------------------------------- named barriers (id 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_arrive(uint32_t id, uint32_t threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
 // ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
 // K-major shared-memory matrix descriptor: rows of the swizzle span (128 / 64 / 32 B) packed densely, 8-row core groups SBO
 // bytes apart; LBO is the distance between K-adjacent core matrices (used by SWIZZLE_NONE only).
