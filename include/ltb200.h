@@ -225,7 +225,9 @@ int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d);
  * argument checks and planning; nothing is launched.  kernel: 0 = cp.async gather kernel conv_gather_wgmma_kernel<bn, kb,
  * grouped>, 1 = TMA kernel conv_halo_wgmma_kernel<bn, nsub, nacc, taps, resident_chunks, grouped> (taps: 9 = 3x3 / ConvT,
  * 10 = stride-2 parity planes, 16 = fused upsample, 1 = GEMM mode), 2 = TMA kernel conv_pingpong_kernel (3x3, 64 -> 64
- * channels, residual from the halo; reported as taps 9, bn 64, nsub 1, nacc 1, resident_chunks 1).  ksplit > 1: the gather kernel splits K that many ways
+ * channels, residual from the halo; reported as taps 9, bn 64, nsub 1, nacc 1, resident_chunks 1), 3 = TMA kernel
+ * conv_rowpair_kernel (3x3, 80 -> 32 channels, two output rows per MMA; reported as taps 9, bn 32, nsub 1, nacc 1,
+ * resident_chunks 2).  ksplit > 1: the gather kernel splits K that many ways
  * and a finalize kernel sums the slices.  res_halo = 1: the TMA kernel adds the residual from its shared-memory halo tiles
  * (res is the input slice itself) instead of reading res from global memory.  Fields that do not apply to the kernel are 0. */
 typedef struct ltb_conv_variant {

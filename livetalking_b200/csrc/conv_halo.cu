@@ -650,12 +650,12 @@ static EncodeTiledFn get_encode() {
 }
 
 bool encode_tmap_f16(CUtensorMap* tm, int rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                     const cuuint32_t* box, int spatial_stride) {
+                     const cuuint32_t* box, int spatial_stride, CUtensorMapSwizzle swizzle) {
   EncodeTiledFn fn = get_encode();
   if (!fn) return false;
   cuuint32_t es[5] = {1, (cuuint32_t)spatial_stride, (cuuint32_t)spatial_stride, 1, 1};   // traversal stride of the W and H dimensions
   return fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes, box, es,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+            CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 

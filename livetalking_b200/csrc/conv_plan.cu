@@ -90,6 +90,7 @@ int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan*
   out->p = p;
   out->halo = false;
   out->pingpong = false;
+  out->rowpair = false;
   if (p.group_slot) {
     if (p.group_images < 1 || p.N % p.group_images || p.slots < 1 || p.w_slot_stride < 0 || p.bias_slot_stride < 0)
       return LTB_FAIL("conv: grouped weights need N divisible by group_images >= 1, slots >= 1 and non-negative slot strides");
@@ -99,6 +100,11 @@ int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan*
   if (w_tap && conv_pingpong_supported(p)) {
     if (conv_pingpong_make_plan(p, w_tap, &out->pp) != 0) return LTB_FAIL("conv: ping-pong plan / tensor map creation failed");
     out->pingpong = true;
+    return 0;
+  }
+  if (w_tap && conv_rowpair_supported(p)) {
+    if (conv_rowpair_make_plan(p, w_tap, &out->rp) != 0) return LTB_FAIL("conv: row-pair plan / tensor map creation failed");
+    out->rowpair = true;
     return 0;
   }
   const bool gemm = p.nphases == 1 && p.ph[0].ntaps == 1;   // the halo kernel's GEMM mode reads the K-major rows
@@ -115,6 +121,7 @@ int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan*
 
 cudaError_t conv_launch(const ConvPlan& pl, cudaStream_t st, float* splitk_ws, size_t ws_floats) {
   if (pl.pingpong) return launch_conv_pingpong(pl.pp, st);
+  if (pl.rowpair) return launch_conv_rowpair(pl.rp, st);
   return pl.halo ? launch_conv_halo(pl.hp, st) : launch_conv_gather(pl.p, st, splitk_ws, ws_floats);
 }
 
@@ -129,6 +136,15 @@ bool conv_plan_variant(const ConvPlan& pl, bool have_ws, size_t ws_floats, ltb_c
     out->nacc = 1;
     out->resident_chunks = 1;
     out->res_halo = 1;
+    return true;
+  }
+  if (pl.rowpair) {   // one instance: 3x3, 32 output channels, two resident K chunks
+    out->kernel = 3;
+    out->taps = 9;
+    out->bn = 32;
+    out->nsub = 1;
+    out->nacc = 1;
+    out->resident_chunks = 2;
     return true;
   }
   if (pl.halo) {
@@ -160,6 +176,12 @@ bool conv_plan_fuse_gn_stats(ConvPlan* pl, float* stats, int groups, int hw) {
 }
 
 bool conv_plan_fuse_head(ConvPlan* pl, const float* w, const float* b, float* out) {
+  if (pl->rowpair) {
+    pl->rp.head_w = w;
+    pl->rp.head_b = b;
+    pl->rp.head_out = out;
+    return true;
+  }
   if (!pl->halo || pl->hp.grouped || pl->hp.BN != 32 || pl->p.Cout != 32) return false;
   pl->hp.hp.head_w = w;
   pl->hp.hp.head_b = b;
@@ -267,7 +289,7 @@ static int conv2d_f16_impl(const ltb_conv_desc* d, const void* in_f16, const flo
     cleanup();
     return 1;
   }
-  const size_t ws_floats = (pl.halo || pl.pingpong) ? 0 : (size_t)1 << 22;
+  const size_t ws_floats = (pl.halo || pl.pingpong || pl.rowpair) ? 0 : (size_t)1 << 22;
   if (ws_floats) {
     CK(cudaMalloc(&dws, ws_floats * sizeof(float)));
     CK(cudaMemset(dws, 0, ws_floats * sizeof(float)));

@@ -1,11 +1,13 @@
 // Conv planning: the one place that turns a convolution into ConvParams, picks the kernel that runs it (the TMA halo kernel
-// of conv_halo.cu, the ping-pong kernel of conv_pingpong.cu for the 64-channel residual 3x3 convs, or the cp.async gather
-// kernel of conv_gather.cu), fuses epilogue extras and launches it.
+// of conv_halo.cu, the ping-pong kernel of conv_pingpong.cu for the 64-channel residual 3x3 convs, the row-pair kernel of
+// conv_rowpair.cu for the 80 -> 32 channel output conv, or the cp.async gather kernel of conv_gather.cu), fuses epilogue extras
+// and launches it.
 #pragma once
 #include <cuda_runtime.h>
 
 #include "conv_halo.h"
 #include "conv_pingpong.h"
+#include "conv_rowpair.h"
 
 struct ltb_conv_variant;   // include/ltb200.h
 
@@ -33,7 +35,7 @@ ConvParams conv_params(ConvMode mode, int N, ConvSlice in, int IH, int IW, int C
                        ConvSlice res, const __half* w, int Ktot, int w_koff, const float* bias, bool relu, ConvTaps taps = {});
 
 enum class ConvPath {
-  Auto,    // a TMA kernel (ping-pong or halo) when one supports the geometry and has its weights (w_tap, or none needed in
+  Auto,    // a TMA kernel (ping-pong, row-pair or halo) when one supports the geometry and has its weights (w_tap, or none needed in
            // GEMM mode), else gather
   Gather,  // gather kernel
   Halo,    // a TMA kernel, or fail
@@ -44,6 +46,8 @@ struct ConvPlan {
   HaloPlan hp{};  // halo == true only
   bool pingpong = false;
   PingpongParams pp{};  // pingpong == true only
+  bool rowpair = false;
+  RowpairParams rp{};   // rowpair == true only
 };
 
 // w_tap: device copy of the weights in the halo kernel's tap-major layout (see launch_w_tap_major*); null if there is none.

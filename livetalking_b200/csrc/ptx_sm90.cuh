@@ -165,6 +165,8 @@ __device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t lbo_byte
 }
 // high word of a SWIZZLE_128B K-major descriptor with the given SBO; the low word is (addr >> 4) | (1 << 16) (LBO = 16 B)
 __host__ __device__ constexpr uint32_t wgmma_hi_128b(uint32_t sbo_bytes) { return (sbo_bytes >> 4) | (1u << 30); }
+// the same for SWIZZLE_32B (32-byte rows: one k16 step of fp16 per row)
+__host__ __device__ constexpr uint32_t wgmma_hi_32b(uint32_t sbo_bytes) { return (sbo_bytes >> 4) | (3u << 30); }
 __device__ __forceinline__ uint32_t wgmma_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
 __device__ __forceinline__ uint64_t wgmma_lohi(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
 

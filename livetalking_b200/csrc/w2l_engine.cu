@@ -348,7 +348,7 @@ static int build_plan(ltb_w2l_session* s) {
   auto push_conv = [&](int li, const ConvParams& p) -> int {
     Op o;
     if (conv_plan(p, m->wt[li], path, &o.conv)) return LTB_FAIL("plan: layer " + std::to_string(li) + ": " + g_last_error);
-    o.type = (o.conv.halo || o.conv.pingpong) ? 4 : 0;   // 4: a TMA conv kernel
+    o.type = (o.conv.halo || o.conv.pingpong || o.conv.rowpair) ? 4 : 0;   // 4: a TMA conv kernel
     s->ops.push_back(o);
     return 0;
   };

@@ -1,0 +1,45 @@
+"""CPU: the row-pair conv kernel (conv_rowpair.cu) as ptxas builds it for sm_90a.
+
+It keeps its accumulators and epilogue in registers (no local-memory spills), ptxas does not serialise its wgmma pipeline (no
+C75xx advisory), the halo tiles and resident weights arrive by TMA (UTMALDG), the MMAs are m64n128k16 (two output rows of 32
+channels x 16 row pairs of 8 pixels), and the epilogue goes through stmatrix (STSM) into the staging tile and out with a TMA
+tensor store (UTMASTG)."""
+import os
+import re
+import shutil
+import subprocess
+
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+SRC = os.path.join(ROOT, "livetalking_b200", "csrc", "conv_rowpair.cu")
+
+
+@pytest.fixture(scope="module")
+def compiled(tmp_path_factory):
+    from livetalking_b200 import build
+    nvcc = build._nvcc()
+    cuobjdump = shutil.which("cuobjdump") or os.path.join(os.path.dirname(nvcc), "cuobjdump")
+    if not os.path.exists(cuobjdump):
+        pytest.skip("cuobjdump not available")
+    obj = str(tmp_path_factory.mktemp("rowpair") / "conv_rowpair.o")
+    r = subprocess.run([nvcc, *build.NVCC_FLAGS, "-Xptxas", "-v", "-c", SRC, "-o", obj], capture_output=True, text=True)
+    assert r.returncode == 0, r.stdout + r.stderr
+    sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
+    return r.stdout + r.stderr, sass
+
+
+def test_rowpair_kernel_has_no_spills_or_wgmma_serialisation(compiled):
+    log, sass = compiled
+    assert "conv_rowpair_kernel" in log, log
+    assert re.search(r"\b0 bytes spill stores, 0 bytes spill loads", log), log
+    assert not re.search(r"C75\d\d", log), log
+    assert not re.search(r"\b(STL|LDL)\b", sass)
+
+
+def test_rowpair_uses_tma_wgmma_and_stmatrix(compiled):
+    _, sass = compiled
+    assert "UTMALDG" in sass
+    assert "UTMASTG" in sass
+    assert "STSM" in sass
+    assert len(re.findall(r"HGMMA\.64x128x16\.F32", sass)) == 60   # 4 views x (4 + 1) K steps x 3 tap columns

@@ -7,7 +7,9 @@
 For every shape: full kernel, then with one role knocked out (LTB_HALO_DIAG bits: 1 no epilogue global I/O, 2 no epilogue,
 4 no MMAs, 8 no A (halo) loads, 16 no B (weight) loads) — what the remaining time is tells which resource bounds the layer.
 --forward: per-op event timings (median of 5 eager profiling passes) of the wav2lip256 batch-16 forward, fused 1x1 head and
-all, under LTB_HALO_DIAG 0 / 1 / 2, and the sum over the halo-kernel ops of (dbg0 - dbg1) and (dbg0 - dbg2)."""
+all, under LTB_HALO_DIAG 0 / 1 / 2, and the sum over the halo-kernel ops of (dbg0 - dbg1) and (dbg0 - dbg2).
+--forward --ab VAR: the same per-op timings with the A/B switch VAR (e.g. LTB_CONV_ROWPAIR) on and off, in one process
+(with LTB_DIAG_NORMAL_LIB=1 the product library runs)."""
 import os
 import sys
 
@@ -65,8 +67,10 @@ def forward(engine):
     model = engine.W2LModel(pack_state_dict(synth.random_state_dict(0)))
     av = engine.W2LAvatar(*synth.synthetic_avatar(n=16, H=720, W=1280, bbox=(200, 520, 480, 800)))
     med = {}
-    for v in (0, 1, 2):
-        os.environ["LTB_HALO_DIAG"] = str(v)    # read when the session plans its convs
+    ab = sys.argv[sys.argv.index("--ab") + 1] if "--ab" in sys.argv else None
+    settings = [(ab, "1"), (ab, "0")] if ab else [("LTB_HALO_DIAG", str(v)) for v in (0, 1, 2)]
+    for v, (var, val) in enumerate(settings):
+        os.environ[var] = val    # read when the session plans its convs
         sess = engine.W2LSession(model, av, 16)
         sess.mel_step(synth.sine_audio(2.0)[:(10 + 10 + 2 * 16) * 320], want_output=False)   # one step's PCM window
         sess.profile_ops(0)
@@ -74,7 +78,14 @@ def forward(engine):
         kinds, flops = passes[0][2], passes[0][1]
         med[v] = np.median(np.stack([ms for ms, _, _ in passes]), axis=0)
         sess.close()
-    halo = kinds == 4   # kind 4: halo kernel (3x3 / ConvT / GEMM mode)
+    halo = kinds == 4   # kind 4: a TMA conv kernel (halo, ping-pong or row-pair)
+    if ab:
+        print(f"op kind GFLOP  {ab}=1_us {ab}=0_us")
+        for i in range(len(kinds)):
+            if halo[i]:
+                print(f"{i:3d} {kinds[i]} {flops[i] / 1e9:7.1f} {med[0][i] * 1e3:7.1f} {med[1][i] * 1e3:7.1f}")
+        print(f"all ops {ab}=1 {med[0].sum() * 1e3:.1f} us | {ab}=0 {med[1].sum() * 1e3:.1f} us", flush=True)
+        return
     print("op kind GFLOP  dbg0_us dbg1_us dbg2_us")
     for i in range(len(kinds)):
         if halo[i]:
