@@ -330,6 +330,14 @@ int ltb_op_whisper_logmel(ltb_ctx* c, const void* pcm_f32, int n, const void* fb
  * frame i <- encoder steps int((i+start)*mult) + 0..9 (clamped) of the 5 hidden states -> out[i][50 rows][D]. */
 int ltb_op_whisper_slice(ltb_ctx* c, const void* const* hidden5, int T, int D, int B, float start, float mult, void* out,
                          int out_rows_per_frame);
+/* The two Whisper ops above over G windows (cross-session batching: one encoder forward for G sessions).  logmel: pcm_f32 [G][n],
+ * logspec_ws >= G*80*3000 floats, gmax_ws [G] ints (each window clamped to its own maximum), out_f16 [G][3000][80], out_f32 [G][80][3000];
+ * window g is what ltb_op_whisper_logmel computes for it alone.  slice: each hidden state is [G*T][D], window g reads rows
+ * [g*T, (g+1)*T) -> out[G][B][out_rows_per_frame][D].  G = 1 is the op above. */
+int ltb_op_whisper_logmel_grouped(ltb_ctx* c, const void* pcm_f32, int G, int n, const void* fb_f32, void* logspec_ws, void* gmax_ws,
+                                  void* out_f16, void* out_f32);
+int ltb_op_whisper_slice_grouped(ltb_ctx* c, const void* const* hidden5, int G, int T, int D, int B, float start, float mult, void* out,
+                                 int out_rows_per_frame);
 /* MuseReal.paste_back_frame + get_image_blending (avatars/musetalk_avatar.py:154-164, avatars/musetalk/myutil.py:4-25) */
 typedef struct ltb_mt_paste_op {
   const void* frames; const void* coords; const void* crop; const void* masks; const void* mask_off; const void* pred; void* out;

@@ -154,6 +154,10 @@ _SIGS = {
     "ltb_op_whisper_logmel": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ltb_op_whisper_slice": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p,
                                        C.c_int]),
+    "ltb_op_whisper_logmel_grouped": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p]),
+    "ltb_op_whisper_slice_grouped": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                               C.c_void_p, C.c_int]),
     "ltb_op_mt_paste": (C.c_int, [C.c_void_p, C.POINTER(MtPasteOp)]),
     "ltb_op_s3fd_prep": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "ltb_op_maxpool2x2": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),

@@ -64,10 +64,10 @@ cudaError_t launch_stamp_pixels(uint8_t* frames, int N, int H, int W, const int*
 cudaError_t launch_vae_pre(const uint8_t* img, int N, int H, int W, int half_mask, __half* out, cudaStream_t st);
 cudaError_t launch_gather_rows(const __half* table, int n, const int* d_index, int B, size_t row_elems, __half* out, cudaStream_t st);
 
-// Whisper front-end (whisper.cu)
-cudaError_t launch_whisper_logmel(const float* pcm, int n, const float* fb, float* logspec_ws, int* gmax, __half* out16, float* out32,
+// Whisper front-end (whisper.cu), over G windows (G = 1: one window)
+cudaError_t launch_whisper_logmel(const float* pcm, int G, int n, const float* fb, float* logspec_ws, int* gmax, __half* out16, float* out32,
                                   cudaStream_t st);
-cudaError_t launch_whisper_slice(const __half* const* hidden5, int T, int D, int B, float start, float mult, __half* out,
+cudaError_t launch_whisper_slice(const __half* const* hidden5, int G, int T, int D, int B, float start, float mult, __half* out,
                                  int out_rows_per_frame, cudaStream_t st);
 
 // MuseTalk paste-back (mt_paste.cu): resize + insert + blendLinear, `count` frames per launch

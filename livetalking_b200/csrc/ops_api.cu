@@ -658,27 +658,35 @@ int ltb_op_gather_rows(ltb_ctx* c, const void* table, int n, const void* d_index
   c->launches += 1;
   return 0;
 }
-int ltb_op_whisper_logmel(ltb_ctx* c, const void* pcm_f32, int n, const void* fb_f32, void* logspec_ws, void* gmax_ws, void* out_f16,
-                          void* out_f32) {
+int ltb_op_whisper_logmel_grouped(ltb_ctx* c, const void* pcm_f32, int G, int n, const void* fb_f32, void* logspec_ws, void* gmax_ws,
+                                  void* out_f16, void* out_f32) {
   if (!c || !pcm_f32 || !fb_f32 || !logspec_ws || !gmax_ws || !out_f16) return LTB_FAIL("whisper_logmel: null argument");
   LTB_CTX_ENTER(c);
-  cudaError_t e = launch_whisper_logmel(static_cast<const float*>(pcm_f32), n, static_cast<const float*>(fb_f32),
+  cudaError_t e = launch_whisper_logmel(static_cast<const float*>(pcm_f32), G, n, static_cast<const float*>(fb_f32),
                                         static_cast<float*>(logspec_ws), static_cast<int*>(gmax_ws), static_cast<__half*>(out_f16),
                                         static_cast<float*>(out_f32), c->st);
-  if (e != cudaSuccess) return LTB_FAIL(std::string("whisper_logmel: ") + cudaGetErrorString(e));
+  if (e != cudaSuccess) return LTB_FAIL(std::string("whisper_logmel (1 <= n <= 480000, 1 <= G <= 65535): ") + cudaGetErrorString(e));
   c->launches += 3;
+  return 0;
+}
+int ltb_op_whisper_logmel(ltb_ctx* c, const void* pcm_f32, int n, const void* fb_f32, void* logspec_ws, void* gmax_ws, void* out_f16,
+                          void* out_f32) {
+  return ltb_op_whisper_logmel_grouped(c, pcm_f32, 1, n, fb_f32, logspec_ws, gmax_ws, out_f16, out_f32);
+}
+int ltb_op_whisper_slice_grouped(ltb_ctx* c, const void* const* hidden5, int G, int T, int D, int B, float start, float mult, void* out,
+                                 int out_rows_per_frame) {
+  if (!c || !hidden5 || !out) return LTB_FAIL("whisper_slice: null argument");
+  LTB_CTX_ENTER(c);
+  if (D % 8 != 0 || out_rows_per_frame < 50) return LTB_FAIL("whisper_slice: bad shape");
+  cudaError_t e = launch_whisper_slice(reinterpret_cast<const __half* const*>(hidden5), G, T, D, B, start, mult, static_cast<__half*>(out),
+                                       out_rows_per_frame, c->st);
+  if (e != cudaSuccess) return LTB_FAIL(std::string("whisper_slice (T >= 1, 1 <= B, G <= 65535): ") + cudaGetErrorString(e));
+  c->launches += 1;
   return 0;
 }
 int ltb_op_whisper_slice(ltb_ctx* c, const void* const* hidden5, int T, int D, int B, float start, float mult, void* out,
                          int out_rows_per_frame) {
-  if (!c || !hidden5 || !out) return LTB_FAIL("whisper_slice: null argument");
-  LTB_CTX_ENTER(c);
-  if (D % 8 != 0 || out_rows_per_frame < 50) return LTB_FAIL("whisper_slice: bad shape");
-  cudaError_t e = launch_whisper_slice(reinterpret_cast<const __half* const*>(hidden5), T, D, B, start, mult, static_cast<__half*>(out),
-                                       out_rows_per_frame, c->st);
-  if (e != cudaSuccess) return LTB_FAIL(std::string("whisper_slice: ") + cudaGetErrorString(e));
-  c->launches += 1;
-  return 0;
+  return ltb_op_whisper_slice_grouped(c, hidden5, 1, T, D, B, start, mult, out, out_rows_per_frame);
 }
 int ltb_op_mt_paste(ltb_ctx* c, const ltb_mt_paste_op* d) {
   if (!c || !d) return LTB_FAIL("mt_paste: null argument");

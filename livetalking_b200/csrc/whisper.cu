@@ -8,6 +8,10 @@
 //             log10(1e-10) = -10 (before the global-max clamp), exactly what the reference computes for silence.
 //   slicing : video frame i takes encoder steps c..c+9, c = int((i + start) * 2), clamped to [0, T-1], from all 5 hidden
 //             states -> (50, 384) rows ordered (step-major, layer-minor).
+//
+// Every kernel takes a window count G (cross-session batching: one encoder forward for G sessions): PCM [G][n], log-mel
+// [G][3000][80], hidden states [G*T][D], features [G][B][rows][D].  Window g reads and writes only its own slices, and has its own
+// global maximum (WhisperFeatureExtractor clamps each utterance on its own).  G = 1 is the single-window layout.
 #include "ops.h"
 
 namespace ltb {
@@ -27,14 +31,18 @@ __device__ __forceinline__ int float_ordered(float f) {
 }
 __device__ __forceinline__ float ordered_float(int i) { return __int_as_float((i >= 0) ? i : (i ^ 0x7FFFFFFF)); }
 
-// one block per active frame; writes log10 mel power to logspec[m * t_active + t] and folds the global maximum
+// one block per active frame (blockIdx.x) of window blockIdx.y; writes log10 mel power to logspec[g][m * t_active + t] and folds
+// the window's maximum into gmax[g]
 __global__ void __launch_bounds__(256) whisper_stft_mel_kernel(const float* __restrict__ pcm, int n, const float* __restrict__ fb,
                                                                int t_active, float* __restrict__ logspec, int* __restrict__ gmax) {
   __shared__ double fr[kWNfft];
   __shared__ double tc[kWNfft], ts[kWNfft];
   __shared__ double pw[kWBins];
   __shared__ float red[8];
-  const int t = blockIdx.x;
+  const int t = blockIdx.x, g = blockIdx.y;
+  pcm += (size_t)g * n;
+  logspec += (size_t)g * kWMels * t_active;
+  gmax += g;
   for (int i = threadIdx.x; i < kWNfft; i += 256) {
     const double w = 0.5 - 0.5 * cospi((double)i / 200.0);  // torch.hann_window(400) (periodic)
     fr[i] = (double)w_sample(pcm, n, t * kWHop + i - kWNfft / 2) * (double)(float)w;
@@ -74,14 +82,19 @@ __global__ void __launch_bounds__(256) whisper_stft_mel_kernel(const float* __re
   }
 }
 
-__global__ void whisper_init_max_kernel(int* gmax, int t_active) {
-  *gmax = float_ordered(t_active < kWFrames ? -10.f : -INFINITY);
+__global__ void whisper_init_max_kernel(int* gmax, int G, int t_active) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < G) gmax[g] = float_ordered(t_active < kWFrames ? -10.f : -INFINITY);
 }
 
-// out16: fp16 [3000][80] (the NHWC input of conv1) ; out32 (optional): float [80][3000] = input_features
+// window blockIdx.y -> out16: fp16 [3000][80] (the NHWC input of conv1) ; out32 (optional): float [80][3000] = input_features
 __global__ void __launch_bounds__(256) whisper_finalize_kernel(const float* __restrict__ logspec, int t_active, const int* __restrict__ gmax,
                                                                __half* __restrict__ out16, float* __restrict__ out32) {
-  const float floor_v = ordered_float(*gmax) - 8.0f;
+  const int g = blockIdx.y;
+  logspec += (size_t)g * kWMels * t_active;
+  out16 += (size_t)g * kWFrames * kWMels;
+  if (out32) out32 += (size_t)g * kWMels * kWFrames;
+  const float floor_v = ordered_float(gmax[g]) - 8.0f;
   const int total = kWFrames * kWMels;
   for (int i = blockIdx.x * 256 + threadIdx.x; i < total; i += gridDim.x * 256) {
     const int t = i / kWMels, m = i % kWMels;
@@ -92,14 +105,14 @@ __global__ void __launch_bounds__(256) whisper_finalize_kernel(const float* __re
   }
 }
 
-cudaError_t launch_whisper_logmel(const float* pcm, int n, const float* fb, float* logspec_ws, int* gmax, __half* out16, float* out32,
+cudaError_t launch_whisper_logmel(const float* pcm, int G, int n, const float* fb, float* logspec_ws, int* gmax, __half* out16, float* out32,
                                   cudaStream_t st) {
-  if (n < 1 || n > kWSamples) return cudaErrorInvalidValue;
+  if (n < 1 || n > kWSamples || G < 1 || G > 65535) return cudaErrorInvalidValue;
   int t_active = (n + kWNfft / 2 + kWHop - 1) / kWHop + 1;
   if (t_active > kWFrames) t_active = kWFrames;
-  whisper_init_max_kernel<<<1, 1, 0, st>>>(gmax, t_active);
-  whisper_stft_mel_kernel<<<t_active, 256, 0, st>>>(pcm, n, fb, t_active, logspec_ws, gmax);
-  whisper_finalize_kernel<<<240, 256, 0, st>>>(logspec_ws, t_active, gmax, out16, out32);
+  whisper_init_max_kernel<<<(G + 255) / 256, 256, 0, st>>>(gmax, G, t_active);
+  whisper_stft_mel_kernel<<<dim3(t_active, G), 256, 0, st>>>(pcm, n, fb, t_active, logspec_ws, gmax);
+  whisper_finalize_kernel<<<dim3(240, G), 256, 0, st>>>(logspec_ws, t_active, gmax, out16, out32);
   return cudaGetLastError();
 }
 
@@ -110,20 +123,22 @@ __global__ void __launch_bounds__(128) whisper_slice_kernel(HiddenPtrs hp, int T
                                                             int out_rows_per_frame) {
   const int i = blockIdx.y;         // video frame
   const int r = blockIdx.x;         // 0..49 : step j = r / 5, layer = r % 5
+  const int g = blockIdx.z;         // window: its hidden rows [g*T, (g+1)*T), its B frames of out
   const int j = r / 5, layer = r % 5;
   const int center = (int)((float)(i + start) * mult);   // int(vid_idx * feature_idx_multiplier)
   int idx = center + j;                                   // window [0, 5] video frames * 2 = 10 steps
   idx = max(0, min(T - 1, idx));
-  const uint4* src = reinterpret_cast<const uint4*>(hp.h[layer] + (size_t)idx * D);
-  uint4* dst = reinterpret_cast<uint4*>(out + ((size_t)i * out_rows_per_frame + r) * D);
+  const uint4* src = reinterpret_cast<const uint4*>(hp.h[layer] + ((size_t)g * T + idx) * D);
+  uint4* dst = reinterpret_cast<uint4*>(out + (((size_t)g * B + i) * out_rows_per_frame + r) * D);
   for (int v = threadIdx.x; v < D / 8; v += 128) dst[v] = src[v];
 }
 
-cudaError_t launch_whisper_slice(const __half* const* hidden5, int T, int D, int B, float start, float mult, __half* out,
+cudaError_t launch_whisper_slice(const __half* const* hidden5, int G, int T, int D, int B, float start, float mult, __half* out,
                                  int out_rows_per_frame, cudaStream_t st) {
+  if (G < 1 || G > 65535 || B < 1 || B > 65535 || T < 1) return cudaErrorInvalidValue;
   HiddenPtrs hp;
   for (int i = 0; i < 5; ++i) hp.h[i] = hidden5[i];
-  whisper_slice_kernel<<<dim3(50, B), 128, 0, st>>>(hp, T, D, B, start, mult, out, out_rows_per_frame);
+  whisper_slice_kernel<<<dim3(50, B, G), 128, 0, st>>>(hp, T, D, B, start, mult, out, out_rows_per_frame);
   return cudaGetLastError();
 }
 

@@ -334,18 +334,21 @@ class Ctx:
     def mt_paste(self, op: MtPasteOp):
         check(lib().ltb_op_mt_paste(self._h, C.byref(op)))
 
-    # ---- Whisper front end and feature slicing (livetalking_b200/whisper.py)
+    # ---- Whisper front end and feature slicing (livetalking_b200/whisper.py), over G windows (each clamped and sliced on its own)
     def whisper_logmel(self, pcm: DevTensor, n: int, fb: DevTensor, logspec: DevTensor, gmax: DevTensor, feats16: DevTensor,
-                       feats32: Optional[DevTensor] = None):
-        check(lib().ltb_op_whisper_logmel(self._h, C.c_void_p(pcm.ptr), n, C.c_void_p(fb.ptr), C.c_void_p(logspec.ptr), C.c_void_p(gmax.ptr),
-                                          C.c_void_p(feats16.ptr), C.c_void_p(feats32.ptr) if feats32 is not None else None))
+                       feats32: Optional[DevTensor] = None, G: int = 1):
+        check(lib().ltb_op_whisper_logmel_grouped(self._h, C.c_void_p(pcm.ptr), G, n, C.c_void_p(fb.ptr), C.c_void_p(logspec.ptr),
+                                                  C.c_void_p(gmax.ptr), C.c_void_p(feats16.ptr),
+                                                  C.c_void_p(feats32.ptr) if feats32 is not None else None))
 
-    def whisper_slice(self, hidden: Sequence[DevTensor], T: int, D: int, B: int, start: float, mult: float, out: DevTensor, out_rows: int):
-        """hidden: the five (T, D) fp16 encoder states; frame i of B takes steps int((i + start) * mult) + 0..9 -> out[i][out_rows][D]."""
+    def whisper_slice(self, hidden: Sequence[DevTensor], T: int, D: int, B: int, start: float, mult: float, out: DevTensor, out_rows: int,
+                      G: int = 1):
+        """hidden: the five (G*T, D) fp16 encoder states; frame i of B of window g takes steps int((i + start) * mult) + 0..9 of rows
+        [g*T, (g+1)*T) -> out[g][i][out_rows][D]."""
         if len(hidden) != 5:
             raise ValueError(f"whisper_slice reads 5 hidden states, got {len(hidden)}")
         ptrs = (C.c_void_p * 5)(*[h.ptr for h in hidden])
-        check(lib().ltb_op_whisper_slice(self._h, ptrs, T, D, B, float(start), float(mult), C.c_void_p(out.ptr), out_rows))
+        check(lib().ltb_op_whisper_slice_grouped(self._h, ptrs, G, T, D, B, float(start), float(mult), C.c_void_p(out.ptr), out_rows))
 
     # ---- S3FD face detector (livetalking_b200/s3fd.py)
     def s3fd_prep(self, frames_u8: DevTensor, N: int, H: int, W: int, out: DevTensor):

@@ -109,3 +109,17 @@ class CrossSessionBatcher:
             t.error = RuntimeError("CrossSessionBatcher closed")
             t.done.set()
         self._thread.join(timeout=5)
+
+
+class SharedFeatures:
+    """An ASR's feature extractor in cross-session mode (HubertASR, WhisperASR): run(pcm) is one group request of a shared feature
+    scheduler and blocks until its round is served.  The scheduler and its graph belong to the model, so close() releases nothing."""
+
+    def __init__(self, batcher: CrossSessionBatcher):
+        self.batcher = batcher
+
+    def run(self, pcm: np.ndarray) -> np.ndarray:
+        return self.batcher.submit([pcm])[0]
+
+    def close(self):
+        pass

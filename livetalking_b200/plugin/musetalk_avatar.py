@@ -5,6 +5,11 @@ and the class registered as ``("avatar", "musetalk")``.  ``MuseReal`` keeps the 
 
     inference_batch(index, audiofeat_batch) -> (B,256,256,3) uint8 BGR predictions      (musetalk_avatar.py:130-152)
     paste_back_frame(pred_frame, idx)       -> H x W x 3 uint8 BGR, fresh and writable   (musetalk_avatar.py:154-164)
+
+Cross-session mode (``opt.ltb_cross_session`` / ``LTB_CROSS_SESSION=1``): ``inference_batch`` submits one group request to a shared
+``MuseTalkBatchSession`` (``LTB_MT_GROUPS`` sessions per UNet + VAE launch, default 4), and ``WhisperASR.run_step`` submits its PCM
+window as one group request to a shared ``WhisperBatchFeatures`` (up to ``LTB_MT_GROUPS`` windows per encoder forward).  Both
+schedulers dispatch a round when it is full or its oldest request is ``LTB_MUX_WAIT_MS`` old.
 """
 from __future__ import annotations
 
@@ -18,8 +23,8 @@ import numpy as np
 from .. import engine
 from ..musetalk import MuseTalkAvatar, MuseTalkBatchSession, MuseTalkModel, MuseTalkSession
 from ..ops import Ctx
-from ..whisper import WhisperEncoder, WhisperFeatures
-from .batcher import CrossSessionBatcher
+from ..whisper import WhisperBatchFeatures, WhisperEncoder, WhisperFeatures
+from .batcher import CrossSessionBatcher, SharedFeatures
 from .whisper_asr import WhisperASR
 
 try:
@@ -122,6 +127,21 @@ def shared_batcher(model: EngineModel, lat_hw: int, frames_per_session: int) -> 
         return table[key]
 
 
+def shared_feature_batcher(model: EngineModel, batch: int, stride_left: int, stride_right: int) -> CrossSessionBatcher:
+    """Cross-session mode: one Whisper scheduler per (model, window layout), created by the first session that asks.  Its mux is a
+    WhisperBatchFeatures of LTB_MT_GROUPS windows: sessions whose steps fall in the same round share one encoder forward."""
+    with _BATCHER_LOCK:
+        table = getattr(model, "_ltb_feature_batchers", None)
+        if table is None:
+            table = model._ltb_feature_batchers = {}
+        key = (int(batch), int(stride_left), int(stride_right))
+        if key not in table:
+            groups = int(os.environ.get("LTB_MT_GROUPS", "4"))
+            mux = WhisperBatchFeatures(model.whisper, batch, groups, stride_left, stride_right)
+            table[key] = CrossSessionBatcher(mux, float(os.environ.get("LTB_MUX_WAIT_MS", "4")))
+        return table[key]
+
+
 @register("avatar", "musetalk")
 class MuseReal(BaseAvatar):
     def __init__(self, opt, model, avatar):
@@ -142,7 +162,11 @@ class MuseReal(BaseAvatar):
         # every session owns its stream + scratch (two: UNet/VAE graph, Whisper graph); weights / avatar assets are shared.
         # Cross-session mode: the session keeps only a paste-back context, its UNet/VAE pass runs in the shared batch.
         self.engine_session = MuseTalkSession(model.net, eng_avatar, self.batch_size, paste_only=cross)
-        self.audio_processor = WhisperFeatures(model.whisper, self.batch_size, opt.l, opt.r)
+        # cross-session mode shares one grouped Whisper forward per round; a stand-in encoder (no device weights) keeps its own extractor
+        if cross and isinstance(model.whisper, WhisperEncoder):
+            self.audio_processor = SharedFeatures(shared_feature_batcher(model, self.batch_size, opt.l, opt.r))
+        else:
+            self.audio_processor = WhisperFeatures(model.whisper, self.batch_size, opt.l, opt.r)
         self.asr = WhisperASR(opt, self, self.audio_processor)
         self.asr.warm_up()
 

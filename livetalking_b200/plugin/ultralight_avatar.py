@@ -28,7 +28,7 @@ from .. import engine
 from ..hubert import HubertBatchFeatures, HubertEncoder, HubertFeatures
 from ..ops import Ctx
 from ..ultralight import FACE, UltraLightAvatar, UltraLightBatchSession, UltraLightModel, UltraLightSession
-from .batcher import CrossSessionBatcher
+from .batcher import CrossSessionBatcher, SharedFeatures
 from .hubert_asr import HubertASR
 
 try:
@@ -133,20 +133,6 @@ def shared_feature_batcher(audio: EngineAudio, batch: int, stride_left: int, str
             mux = HubertBatchFeatures(audio.encoder, batch, groups, stride_left, stride_right)
             table[key] = CrossSessionBatcher(mux, float(os.environ.get("LTB_MUX_WAIT_MS", "4")))
         return table[key]
-
-
-class SharedFeatures:
-    """HubertASR's extractor in cross-session mode: run(pcm) is one group request of the shared HuBERT scheduler and blocks until its
-    round is served.  The scheduler and its graph belong to the model, so close() releases nothing."""
-
-    def __init__(self, batcher: CrossSessionBatcher):
-        self.batcher = batcher
-
-    def run(self, pcm: np.ndarray) -> np.ndarray:
-        return self.batcher.submit([pcm])[0]
-
-    def close(self):
-        pass
 
 
 @register("avatar", "ultralight")

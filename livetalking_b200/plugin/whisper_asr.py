@@ -13,7 +13,7 @@ from .base_asr import BaseASR, fixed_chunk
 class WhisperASR(BaseASR):
     def __init__(self, opt, parent, audio_processor):
         super().__init__(opt, parent)
-        self.audio_processor = audio_processor          # livetalking_b200.whisper.WhisperFeatures
+        self.audio_processor = audio_processor          # whisper.WhisperFeatures, or batcher.SharedFeatures in cross-session mode
         if audio_processor is None:
             raise RuntimeError("WhisperASR needs an engine WhisperFeatures object (no CPU fallback)")
 

@@ -4,10 +4,12 @@ output_hidden_states=True)``) and the slicing of ``WhisperASR.run_step`` (avatar
 
 Weights come from the HF ``WhisperModel`` state_dict (``encoder.*`` keys).  The encoder (2 conv1d + 4 pre-LN transformer
 layers over 1500 steps) is assembled from the same engine ops as the UNet and captured into one CUDA graph together with
-the log-mel kernels and the per-frame (50, 384) slicing."""
+the log-mel kernels and the per-frame (50, 384) slicing.
+
+``WhisperBatchFeatures`` is the cross-session form: G sessions' windows stacked on the row dimension, one encoder forward for all."""
 from __future__ import annotations
 
-from typing import Dict, Optional
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
@@ -73,21 +75,27 @@ class WhisperEncoder:
     def emit(self, b: Builder, feats16: DevTensor):
         """feats16: fp16 (3000, 80) log-mel features -> the 5 hidden states HF returns, each (1500, D) fp16.
         Ops are enqueued on the builder's ctx (the session's own stream); the weights live in self.ctx (read-only)."""
+        return self.emit_grouped(b, feats16, 1)
+
+    def emit_grouped(self, b: Builder, feats16: DevTensor, G: int):
+        """emit() for G windows at once: feats16 fp16 (G, 3000, 80) -> 5 hidden states of (G * 1500, D), window g in rows
+        [g*1500, (g+1)*1500).  The convs run with N = G images of 1 x 3000 (each zero-padded on its own), the positional add repeats
+        per window, row-wise ops run over G*1500 rows and attention with batch G, so no op mixes rows of different windows."""
         ctx, D = b.ctx, self.D
         T = N_FRAMES
-        x = DevTensor(feats16.ptr, (1, 1, T, N_MELS))
-        h = b.new(1, 1, T, D)
-        ctx.conv(x, self.conv1, h, N=1, IH=1, IW=T, OH=1, OW=T, pad=(0, 1))
-        ctx.eltwise(h, None, T * D, 8, 1, h)                                             # GELU
+        x = DevTensor(feats16.ptr, (G, 1, T, N_MELS))
+        h = b.new(G, 1, T, D)
+        ctx.conv(x, self.conv1, h, N=G, IH=1, IW=T, OH=1, OW=T, pad=(0, 1))
+        ctx.eltwise(h, None, G * T * D, 8, 1, h)                                         # GELU
         T2 = T // 2
-        h2 = b.new(1, 1, T2, D)
-        ctx.conv(h, self.conv2, h2, N=1, IH=1, IW=T, OH=1, OW=T2, stride=(1, 2), pad=(0, 1))
-        ctx.eltwise(h2, None, T2 * D, 8, 1, h2)                                          # GELU
-        x = b.new(T2, D)
-        ctx.eltwise(h2, self.pos, T2 * D, T2 * D, 0, x)                                  # + embed_positions
+        h2 = b.new(G, 1, T2, D)
+        ctx.conv(h, self.conv2, h2, N=G, IH=1, IW=T, OH=1, OW=T2, stride=(1, 2), pad=(0, 1))
+        ctx.eltwise(h2, None, G * T2 * D, 8, 1, h2)                                      # GELU
+        x = b.new(G * T2, D)
+        ctx.eltwise(h2, self.pos, G * T2 * D, T2 * D, 0, x)                              # + embed_positions
         hidden = [x]
         for i, L in enumerate(self.layers):
-            x = b.attention(L["attn"], b.layernorm(x, L["ln1"]), 1, T2, res=x)
+            x = b.attention(L["attn"], b.layernorm(x, L["ln1"]), G, T2, res=x)
             f = b.linear(b.layernorm(x, L["ln2"]), L["fc1"])
             ctx.eltwise(f, None, f.rows * f.C, 8, 1, f)
             x = b.linear(f, L["fc2"], res=x)
@@ -143,3 +151,63 @@ class WhisperFeatures(GraphSession):
             self.run_async(pcm)
             full = self.ctx.download(self.out)
         return full[:, :50]
+
+
+class WhisperBatchFeatures(GraphSession):
+    """WhisperFeatures for up to G sessions at once: G PCM windows of the same layout -> G x (B, 50, D) features, ONE CUDA graph
+    (grouped log-mel, one encoder forward over the G windows stacked on the row dimension, grouped slice).  The encoder always
+    runs over the 30-s padded window (1500 tokens), whatever B, so at small B each session's forward is mostly fixed cost: G
+    windows per forward share the weights and fill wider GEMMs.  Each window keeps its own log-mel clamp, conv padding and attention
+    keys, so a session's features do not depend on which other windows share its round.  A call with k < G windows is a partial
+    round: groups [k, G) keep their last window (zeros before the first call) and their output is not read.  `batch` /
+    `infer_slots` make it a mux for plugin.batcher.CrossSessionBatcher (a request is one session's PCM window)."""
+
+    def __init__(self, enc: WhisperEncoder, batch: int, groups: int, stride_left: int = 10, stride_right: int = 10,
+                 ctx: Optional[Ctx] = None):
+        self.enc, self.B, self.G = enc, int(batch), int(groups)
+        if self.G < 1:
+            raise ValueError("groups must be >= 1")
+        self.batch = self.G                                  # CrossSessionBatcher: requests per engine call
+        self.n = (stride_left + stride_right + 2 * self.B) * 320
+        if self.n > N_SAMPLES:
+            raise ValueError("audio window longer than 30 s")
+        super().__init__(ctx)
+        try:
+            ctx = self.ctx
+            self.pcm = self.alloc((self.G, self.n), np.float32, zero=True)
+            self.logspec = self.alloc((self.G, N_MELS * N_FRAMES), np.float32, zero=True)
+            self.gmax = self.alloc((self.G,), np.int32, zero=True)
+            self.feats16 = self.alloc((self.G, N_FRAMES, N_MELS), np.float16, zero=True)
+            self.out = self.alloc((self.G, self.B, 50, enc.D), np.float16, zero=True)
+            self.start = stride_left / 2.0
+
+            def emit(b: Builder):
+                ctx.whisper_logmel(self.pcm, self.n, enc.fb, self.logspec, self.gmax, self.feats16, None, G=self.G)
+                self.hidden = enc.emit_grouped(b, self.feats16, self.G)
+                ctx.whisper_slice(self.hidden, N_FRAMES // 2, enc.D, self.B, self.start, 2.0, self.out, 50, G=self.G)
+
+            self.capture(emit)
+        except BaseException:
+            self.close()
+            raise
+
+    def run_async(self, pcms: Sequence[np.ndarray]) -> int:
+        """Stage windows 0 .. k-1 and launch the graph; -> k."""
+        k = len(pcms)
+        if not 1 <= k <= self.G:
+            raise ValueError(f"1..{self.G} windows per call, got {k}")
+        x = np.stack([np.ascontiguousarray(p, np.float32).reshape(-1) for p in pcms])
+        if x.shape[1] != self.n:
+            raise ValueError(f"expected windows of {self.n} samples, got {x.shape[1]}")
+        self.ctx.h2d(DevTensor(self.pcm.ptr, (k, self.n), np.float32), x, sync=False)
+        self.graph.launch()
+        return k
+
+    def run_groups(self, pcms: Sequence[np.ndarray]) -> List[np.ndarray]:
+        """-> per window its (B, 50, D) float16 features: what WhisperFeatures.run returns for that window alone."""
+        with self.ctx.lock:
+            k = self.run_async(pcms)
+            out = self.ctx.download(DevTensor(self.out.ptr, (k, self.B, 50, self.enc.D), np.float16))
+        return [out[g] for g in range(k)]
+
+    infer_slots = run_groups
