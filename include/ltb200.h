@@ -219,6 +219,9 @@ typedef struct ltb_conv_op {
    * (1,0), (1,1) in turn (the packing of ltb_conv2d_f16); `w_tap`, if given, the same nine [Cout][Cin] slices of `w` in the
    * order 0, 1, 5, 2, 6, 8, 7, 4, 3 for the TMA kernel. */
   int transposed;
+  /* 1: run the layer on the small-map split-K kernel when it supports the geometry (8x8 / 4x4 / 1x1 grids, Cin % 64 == 0,
+   * Cout % 128 == 0; see ltb_conv_variant kernel 4) */
+  int smallmap;
 } ltb_conv_op;
 int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d);
 /* test hook (like ltb_conv2d_f16): the kernel instance ltb_op_conv2d would run for *d on this device, found by the same
@@ -227,7 +230,9 @@ int ltb_op_conv2d(ltb_ctx* c, const ltb_conv_op* d);
  * 10 = stride-2 parity planes, 16 = fused upsample, 1 = GEMM mode), 2 = TMA kernel conv_pingpong_kernel (3x3, 64 -> 64
  * channels, residual from the halo; reported as taps 9, bn 64, nsub 1, nacc 1, resident_chunks 1), 3 = TMA kernel
  * conv_rowpair_kernel (3x3, 80 -> 32 channels, two output rows per MMA; reported as taps 9, bn 32, nsub 1, nacc 1,
- * resident_chunks 2).  ksplit > 1: the gather kernel splits K that many ways
+ * resident_chunks 2), 4 = TMA kernel conv_smallmap_kernel<np> (128 output channels x the pixels of whole images, taps = taps
+ * summed over the phases, bn 128, kb 64, ksplit = the CTAs of one cluster that split K, reduced in distributed shared memory).
+ * ksplit > 1: the gather kernel splits K that many ways
  * and a finalize kernel sums the slices.  res_halo = 1: the TMA kernel adds the residual from its shared-memory halo tiles
  * (res is the input slice itself) instead of reading res from global memory.  Fields that do not apply to the kernel are 0. */
 typedef struct ltb_conv_variant {

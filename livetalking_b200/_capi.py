@@ -28,7 +28,7 @@ class ConvOp(C.Structure):
                 [(n, C.c_longlong) for n in ("in_zo", "in_zi", "w_zo", "w_zi", "out_zo", "out_zi")] +
                 [("gn_stats", C.c_void_p), ("gn_groups", C.c_int), ("gn_hw", C.c_int), ("upsample2x", C.c_int)] +
                 [("group_slot", C.c_void_p), ("group_images", C.c_int), ("slots", C.c_int), ("w_slot_stride", C.c_longlong),
-                 ("bias_slot_stride", C.c_longlong), ("transposed", C.c_int)])
+                 ("bias_slot_stride", C.c_longlong), ("transposed", C.c_int), ("smallmap", C.c_int)])
 
 
 class ConvVariant(C.Structure):

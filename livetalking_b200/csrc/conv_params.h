@@ -62,6 +62,8 @@ struct ConvParams {
   const int* group_slot;
   int group_images, slots;
   long long w_slot_stride, bias_slot_stride;
+  // 1: the caller opts this layer in to the small-map split-K kernel (conv_smallmap.cu) where that kernel supports it
+  int smallmap;
 };
 
 }  // namespace ltb

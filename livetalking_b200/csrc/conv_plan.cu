@@ -91,12 +91,18 @@ int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan*
   out->halo = false;
   out->pingpong = false;
   out->rowpair = false;
+  out->smallmap = false;
   if (p.group_slot) {
     if (p.group_images < 1 || p.N % p.group_images || p.slots < 1 || p.w_slot_stride < 0 || p.bias_slot_stride < 0)
       return LTB_FAIL("conv: grouped weights need N divisible by group_images >= 1, slots >= 1 and non-negative slot strides");
     if (p.zbatch > 1 || p.upconv) return LTB_FAIL("conv: grouped weights cannot be combined with zbatch or the fused upsample");
   }
   if (path == ConvPath::Gather) return 0;
+  if (path == ConvPath::Auto && conv_smallmap_supported(p)) {
+    if (conv_smallmap_make_plan(p, &out->sp) != 0) return LTB_FAIL("conv: small-map plan / tensor map creation failed");
+    out->smallmap = true;
+    return 0;
+  }
   if (w_tap && conv_pingpong_supported(p)) {
     if (conv_pingpong_make_plan(p, w_tap, &out->pp) != 0) return LTB_FAIL("conv: ping-pong plan / tensor map creation failed");
     out->pingpong = true;
@@ -122,6 +128,7 @@ int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan*
 cudaError_t conv_launch(const ConvPlan& pl, cudaStream_t st, float* splitk_ws, size_t ws_floats) {
   if (pl.pingpong) return launch_conv_pingpong(pl.pp, st);
   if (pl.rowpair) return launch_conv_rowpair(pl.rp, st);
+  if (pl.smallmap) return launch_conv_smallmap(pl.sp, st);
   return pl.halo ? launch_conv_halo(pl.hp, st) : launch_conv_gather(pl.p, st, splitk_ws, ws_floats);
 }
 
@@ -145,6 +152,14 @@ bool conv_plan_variant(const ConvPlan& pl, bool have_ws, size_t ws_floats, ltb_c
     out->nsub = 1;
     out->nacc = 1;
     out->resident_chunks = 2;
+    return true;
+  }
+  if (pl.smallmap) {   // 128 output channels per CTA, 64-channel K steps, ksplit CTAs of a cluster per output tile
+    out->kernel = 4;
+    for (int i = 0; i < pl.p.nphases; ++i) out->taps += pl.p.ph[i].ntaps;
+    out->bn = 128;
+    out->kb = 64;
+    out->ksplit = pl.sp.ksplit;
     return true;
   }
   if (pl.halo) {

@@ -1,6 +1,7 @@
 // Conv planning: the one place that turns a convolution into ConvParams, picks the kernel that runs it (the TMA halo kernel
 // of conv_halo.cu, the ping-pong kernel of conv_pingpong.cu for the 64-channel residual 3x3 convs, the row-pair kernel of
-// conv_rowpair.cu for the 80 -> 32 channel output conv, or the cp.async gather kernel of conv_gather.cu), fuses epilogue extras
+// conv_rowpair.cu for the 80 -> 32 channel output conv, the small-map split-K kernel of conv_smallmap.cu for opted-in 8x8 / 4x4 / 1x1
+// layers, or the cp.async gather kernel of conv_gather.cu), fuses epilogue extras
 // and launches it.
 #pragma once
 #include <cuda_runtime.h>
@@ -8,6 +9,7 @@
 #include "conv_halo.h"
 #include "conv_pingpong.h"
 #include "conv_rowpair.h"
+#include "conv_smallmap.h"
 
 struct ltb_conv_variant;   // include/ltb200.h
 
@@ -48,6 +50,8 @@ struct ConvPlan {
   PingpongParams pp{};  // pingpong == true only
   bool rowpair = false;
   RowpairParams rp{};   // rowpair == true only
+  bool smallmap = false;
+  SmallmapParams sp{};  // smallmap == true only
 };
 
 // w_tap: device copy of the weights in the halo kernel's tap-major layout (see launch_w_tap_major*); null if there is none.

@@ -222,6 +222,7 @@ static int conv2d_plan(ltb_ctx* c, const ltb_conv_op* d, ConvPlan* pl) {
   p.w_zi = d->w_zi;
   p.out_zo = d->out_zo;
   p.out_zi = d->out_zi;
+  p.smallmap = d->smallmap;
   if (d->group_slot) {
     if (d->gn_stats) return LTB_FAIL("conv2d: grouped weights cannot produce GroupNorm statistics");
     p.group_slot = static_cast<const int*>(d->group_slot);

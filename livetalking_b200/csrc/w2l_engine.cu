@@ -81,6 +81,9 @@ static const LDef kLayers[54] = {
 constexpr int kNumLayers = 54;
 constexpr size_t kSplitKFloats = (size_t)8 << 20;  // 8M floats: ksplit * M * Cout of the small-spatial layers (<= 10 x 1024 x 512)
 constexpr int kStem = 13, kConvT4 = 34;
+// layers opted in to conv_smallmap.cu: the 4x4 and 1x1 maps L29 - L36 (faster there on H100, DESIGN §3); the 8x8 layers L27,
+// L28, L37 and L38 measured faster on their halo / gather plans and stay there
+constexpr int kFirstSmallmap = 29, kLastSmallmap = 36;
 
 // expected packed sizes (elements) of layer i's weight matrix [rows][K]
 static void packed_dims(int i, int* rows, int* K) {
@@ -345,8 +348,10 @@ static int build_plan(ltb_w2l_session* s) {
     s->louts[li] = LayerOut{v.p, v.H, v.W, v.C, v.Ctot, v.c_off};
   };
   const ConvPath path = (s->flags & LTB_SESSION_NO_HALO) ? ConvPath::Gather : ConvPath::Auto;
-  auto push_conv = [&](int li, const ConvParams& p) -> int {
+  auto push_conv = [&](int li, const ConvParams& p_in) -> int {
     Op o;
+    ConvParams p = p_in;
+    p.smallmap = (li >= kFirstSmallmap && li <= kLastSmallmap) ? 1 : 0;
     if (conv_plan(p, m->wt[li], path, &o.conv)) return LTB_FAIL("plan: layer " + std::to_string(li) + ": " + g_last_error);
     o.type = (o.conv.halo || o.conv.pingpong || o.conv.rowpair) ? 4 : 0;   // 4: a TMA conv kernel
     s->ops.push_back(o);

@@ -172,10 +172,12 @@ class Ctx:
                  zbatch: int = 0, zdiv: int = 1, in_z=(0, 0), w_z=(0, 0), out_z=(0, 0), w_ptr: Optional[int] = None,
                  ktot: Optional[int] = None, cout: Optional[int] = None, in_ptr: Optional[int] = None, out_ptr: Optional[int] = None,
                  gn_stats: Optional[DevTensor] = None, gn_groups: int = 0, gn_hw: int = 0, upsample2x: bool = False,
-                 bias_ptr: Optional[int] = None, group: Optional[tuple] = None, transposed: bool = False) -> ConvOp:
+                 bias_ptr: Optional[int] = None, group: Optional[tuple] = None, transposed: bool = False,
+                 smallmap: bool = False) -> ConvOp:
         """group = (slot table int32 DevTensor, images per group, slots, w slot stride, bias slot stride): grouped weights
         (ltb_conv_op.group_slot) read from w_ptr / bias_ptr.  no_halo: False / True, or 2 to require the TMA kernel.
-        transposed: ConvTranspose2d(k3, s2, p1, op1); w.w / w.w_tap hold the weight layouts of ltb_conv_op.transposed."""
+        transposed: ConvTranspose2d(k3, s2, p1, op1); w.w / w.w_tap hold the weight layouts of ltb_conv_op.transposed.
+        smallmap: opt in to the small-map split-K kernel (ltb_conv_op.smallmap)."""
         d = ConvOp()
         d.in_ = in_ptr if in_ptr is not None else x.ptr
         d.w = w_ptr if w_ptr is not None else w.w.ptr
@@ -210,6 +212,7 @@ class Ctx:
             up = w.upconv(w.ctx)    # beside the weights: a session's ctx may close while the model still uses them
             d.w, d.w_tap, d.Ktot, d.upsample2x = up[0].ptr, up[1].ptr, 16 * w.cin, 1
         d.transposed = int(transposed)
+        d.smallmap = int(smallmap)
         return d
 
     def groupnorm(self, x: DevTensor, N: int, HW: int, groups: int, eps: float, gamma: DevTensor, beta: DevTensor, silu: bool,
