@@ -7,10 +7,16 @@ For every traced call the tracer
   * reads the whole allocation under each output view before and after the op and records every byte outside the view that
     changed (an output whose allocation the tracer did not see being made is checked over the span of its view, pitch gaps
     included);
-  * keeps the dense contents of the input and output views, passed through ``keep`` (e.g. to keep some images of a batch).
+  * keeps the dense contents of the input and output views, passed through ``keep`` (e.g. to keep some images of a batch), or,
+    with ``on_record``, hands each finished record to that callback and then drops its dense data (a traced full-width decoder
+    would otherwise hold many GB of host copies);
+  * with ``data=False`` records only the op sequence (arguments and conv plans): no sync and no read-back.
 Channel-sliced views are read at full pitch and sliced on the host: no kernel runs for a read-back.  Ops that take raw pointers
-(``attention``, ``transpose_heads``) get their views rebuilt from the pointer, pitch and row arguments.  Entering
-``ctx.capture()`` stops tracing (a sync inside stream capture is illegal); ``stop()`` restores the plain methods."""
+(``attention``, ``transpose_heads``, ``softmax``, ...) get their views rebuilt from the pointer, pitch and row arguments.  A
+z-batched conv (``w=None``, ``zbatch > 1``: the GEMMs of the unfused attention) has one view per z slice for its input, its
+weight operand (activation data: K or V^T) and its output; the outside-write check of an allocation uses the union of every
+output view that lies in it.  Entering ``ctx.capture()`` stops tracing (a sync inside stream capture is illegal); ``stop()``
+restores the plain methods."""
 from __future__ import annotations
 
 import inspect
@@ -20,6 +26,10 @@ import numpy as np
 
 UL_OPS = ("conv", "dwconv3x3", "upsample_bilinear2x", "head_sigmoid255", "ul_prep", "ul_prep_grouped")
 HUBERT_OPS = ("conv", "layernorm", "eltwise", "hubert_conv0", "hubert_pos_conv", "transpose_heads", "attention")
+MT_OPS = ("conv", "groupnorm", "groupnorm_apply", "layernorm", "geglu", "eltwise", "softmax", "copy_channels", "upsample2x",
+          "transpose_heads", "attention", "vae_post", "vae_pre", "gather_rows")
+WHISPER_OPS = ("conv", "layernorm", "eltwise", "transpose_heads", "attention", "softmax", "whisper_logmel", "whisper_slice")
+WHISPER_FRAMES, WHISPER_MELS, WHISPER_HOP, WHISPER_NFFT = 3000, 80, 160, 400
 
 
 class OpRecord:
@@ -32,9 +42,25 @@ class OpRecord:
         return f"#{self.index} {self.op}"
 
 
-def _io(op: str, a: dict):
-    """The op's bound arguments -> ({input name: view}, {output name: view}) as DevTensors."""
+def _zviews(v, ptr, n, zdiv, zo, zi, shape=None, pitch=None):
+    """The n z slices of a z-batched conv operand: slice z starts (z // zdiv) zo + (z % zdiv) zi elements after ptr."""
     from livetalking_b200.ops import DevTensor as T
+    return [T(ptr + ((z // zdiv) * zo + (z % zdiv) * zi) * 2, shape or v.shape, pitch=pitch or v.pitch, c_off=0 if shape else v.c_off)
+            for z in range(n)]
+
+
+def _io(op: str, a: dict):
+    """The op's bound arguments -> ({input name: view}, {output name: view}) as DevTensors; a list of views (the z slices of a
+    z-batched conv) is kept as one stacked array."""
+    from livetalking_b200.ops import DevTensor as T
+    if op == "conv" and a["w"] is None and a["kw"].get("zbatch", 0) > 1:
+        kw = a["kw"]
+        x, out, n, zdiv = a["x"], a["out"], kw["zbatch"], kw.get("zdiv", 1)
+        cin, cout = kw["cin"], kw["cout"]
+        assert kw.get("in_ptr") is None and kw.get("out_ptr") is None and kw.get("res") is None, "z-batched conv with extra pointers"
+        return ({"x": _zviews(x, x.ptr + x.c_off * 2, n, zdiv, *kw["in_z"], shape=(x.rows, cin), pitch=x.pitch),
+                 "w": _zviews(None, kw["w_ptr"], n, zdiv, *kw["w_z"], shape=(cout, cin), pitch=kw["ktot"])},
+                {"out": _zviews(out, out.ptr + out.c_off * 2, n, zdiv, *kw["out_z"], shape=(out.rows, cout), pitch=out.pitch)})
     if op == "conv":
         kw = a["kw"]
         x, out = a["x"], a["out"]
@@ -88,6 +114,49 @@ def _io(op: str, a: dict):
         return ({"q": T(a["q_ptr"], (B * a["nq"], hd), pitch=a["q_pitch"]), "k": T(a["k_ptr"], (B * a["kv_rows"], hd), pitch=a["kv_pitch"]),
                  "vt": T(a["vt"].ptr, (B * a["heads"], a["d"], a["n_pad"]))},
                 {"out": T(out.ptr, (B * a["nq"], hd), pitch=out.pitch, c_off=out.c_off)})
+    if op == "groupnorm":
+        return {"x": a["x"]}, {"out": a["out"]}
+    if op == "groupnorm_apply":
+        st = a["stats"]
+        return {"x": a["x"], "stats": T(st.ptr, (a["N"], a["groups"], 2), np.float32)}, {"out": a["out"]}
+    if op == "geglu":
+        rows, H = a["rows"], a["H"]
+        return {"h": T(a["h"].ptr, (rows, 2 * H))}, {"out": T(a["out"].ptr, (rows, H))}
+    if op == "softmax":                                    # in place: the input is read before the op runs
+        v = T(a["x"].ptr, (a["rows"], a["cols"]))
+        return {"x": v}, {"out": v}
+    if op == "copy_channels":
+        src, dst = a["src"], a["dst"]
+        if a["rows"] is not None and a["rows"] != src.rows:
+            src = T(src.ptr, (a["rows"], src.C), pitch=src.pitch, c_off=src.c_off)
+            dst = T(dst.ptr, (a["rows"], dst.C), pitch=dst.pitch, c_off=dst.c_off)
+        return {"src": src}, {"dst": dst}
+    if op == "upsample2x":
+        N, H, W, x = a["N"], a["H"], a["W"], a["x"]
+        return {"x": T(x.ptr, (N, H, W, x.C))}, {"out": T(a["out"].ptr, (N, 2 * H, 2 * W, x.C))}
+    if op == "vae_post":
+        x, n = a["x"], a["npix"]
+        return {"x": T(x.ptr, (n, 3), pitch=x.pitch)}, {"out": T(a["out_u8"].ptr, (n, 3), np.uint8)}
+    if op == "vae_pre":
+        N, H, W = a["N"], a["H"], a["W"]
+        return {"img": T(a["img_u8"].ptr, (N, H, W, 3), np.uint8)}, {"out": T(a["out"].ptr, (N, H, W, 16))}
+    if op == "gather_rows":
+        n, B, r = a["n"], a["B"], a["row_elems"]
+        return ({"table": T(a["table"].ptr, (n, r)), "index": T(a["d_index"].ptr, (1,), np.int32)},
+                {"out": T(a["out"].ptr, (B, r))})
+    if op == "whisper_logmel":
+        G, n = a["G"], a["n"]
+        t_active = min(WHISPER_FRAMES, (n + WHISPER_NFFT // 2 + WHISPER_HOP - 1) // WHISPER_HOP + 1)
+        outs = {"feats16": T(a["feats16"].ptr, (G, WHISPER_FRAMES, WHISPER_MELS)),
+                "logspec": T(a["logspec"].ptr, (G, WHISPER_MELS, t_active), np.float32),
+                "gmax": T(a["gmax"].ptr, (G,), np.int32)}
+        if a["feats32"] is not None:
+            outs["feats32"] = T(a["feats32"].ptr, (G, WHISPER_MELS, WHISPER_FRAMES), np.float32)
+        return {"pcm": T(a["pcm"].ptr, (G, n), np.float32)}, outs
+    if op == "whisper_slice":
+        G, T_, D, B, rows = a["G"], a["T"], a["D"], a["B"], a["out_rows"]
+        ins = {f"h{i}": T(h.ptr, (G * T_, D)) for i, h in enumerate(a["hidden"])}
+        return ins, {"out": T(a["out"].ptr, (G * B, 50 * D), pitch=rows * D)}
     raise ValueError(f"op_trace: no views defined for op {op!r}")
 
 
@@ -112,8 +181,10 @@ def _dense(rows: np.ndarray, v) -> np.ndarray:
 class OpTrace:
     """Trace the ops `ops` of `ctx` until stop().  records: OpRecord per call; errors: writes outside an output view."""
 
-    def __init__(self, ctx, ops=UL_OPS + HUBERT_OPS, keep: Optional[Callable[[np.ndarray], np.ndarray]] = None):
+    def __init__(self, ctx, ops=UL_OPS + HUBERT_OPS, keep: Optional[Callable[[np.ndarray], np.ndarray]] = None,
+                 on_record: Optional[Callable[[OpRecord], None]] = None, data: bool = True):
         self.ctx, self.keep = ctx, keep or (lambda arr: arr)
+        self.on_record, self.data = on_record, data
         self.records: List[OpRecord] = []
         self.errors: List[str] = []
         self._allocs: Dict[int, int] = {}                  # ptr -> nbytes of the allocations made through ctx while tracing
@@ -180,30 +251,44 @@ class OpTrace:
 
     def _record(self, name: str, args: dict, run):
         ctx = self.ctx
-        ins, outs = _io(name, args)
-        ctx.sync()
-        inputs = {k: self.keep(self._read_view(v)) for k, v in ins.items()}
         plan = None
         if name == "conv":
-            plan = ctx.conv_plan(args["x"], args["w"], args["out"], **args["kw"])
-        before = {}
-        for k, v in outs.items():
-            base, size = self._allocation(v)
-            before[k] = (base, size, self._read_bytes(base, size))
+            kw = args["kw"]
+            plan = ctx.conv_plan(args["x"], args["w"], args["out"], **kw)
+        if not self.data:
+            run()
+            self.records.append(OpRecord(len(self.records), name, args, None, None, plan))
+            return
+        ins, outs = _io(name, args)
+        ctx.sync()
+        inputs = {k: (np.stack([self._read_view(u) for u in v]) if isinstance(v, list) else self.keep(self._read_view(v)))
+                  for k, v in ins.items()}
+        # every output view, grouped by the allocation it lies in: each allocation is read once before and once after
+        views = [(k, u) for k, v in outs.items() for u in (v if isinstance(v, list) else [v])]
+        allocs = {}
+        for k, u in views:
+            allocs.setdefault(self._allocation(u), []).append((k, u))
+        before = {key: self._read_bytes(*key) for key in allocs}
         run()
         ctx.sync()
         index = len(self.records)
-        outputs = {}
-        for k, v in outs.items():
-            base, size, old = before[k]
+        dense = {}
+        for (base, size), members in allocs.items():
             new = self._read_bytes(base, size)
-            first = _span(v)[0] - base
             mask = np.zeros(size, bool)
-            _rows_of(mask, first, v)[...] = True
-            changed = (old != new) & ~mask
+            for k, u in members:
+                first = _span(u)[0] - base
+                _rows_of(mask, first, u)[...] = True
+                dense.setdefault(k, []).append(_dense(_rows_of(new, first, u), u))
+            changed = (before[(base, size)] != new) & ~mask
             if changed.any():
                 at = int(np.argmax(changed))
-                self.errors.append(f"#{index} {name}: {int(changed.sum())} bytes outside output {k!r} changed, first at byte {at} of "
-                                   f"the {size}-byte allocation (the view starts at byte {first})")
-            outputs[k] = self.keep(_dense(_rows_of(new, first, v), v))
-        self.records.append(OpRecord(index, name, args, inputs, outputs, plan))
+                names = sorted({k for k, _ in members})
+                self.errors.append(f"#{index} {name}: {int(changed.sum())} bytes outside output {'/'.join(names)!r} changed, first at "
+                                   f"byte {at} of the {size}-byte allocation")
+        outputs = {k: (np.stack(dense[k]) if isinstance(v, list) else self.keep(dense[k][0])) for k, v in outs.items()}
+        rec = OpRecord(index, name, args, inputs, outputs, plan)
+        if self.on_record is not None:
+            self.on_record(rec)
+            rec.inputs = rec.outputs = None
+        self.records.append(rec)

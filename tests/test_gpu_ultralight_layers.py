@@ -766,3 +766,26 @@ def test_tracer_stops_at_capture():
     ctx.sync()
     cap.graph.close()
     ctx.close()
+
+
+def test_tracer_checks_writes_outside_channel_slices():
+    """copy_channels into a channel slice of a wider buffer is traced with a clean report and the data it wrote; when the tracer
+    is handed a narrower output view than the op writes (an ordinary in-bounds write into the neighbouring channels of the same
+    buffer), it reports the bytes outside the view."""
+    from livetalking_b200 import engine
+    from livetalking_b200.ops import Ctx, DevTensor
+    from op_trace import MT_OPS
+    engine.set_device(0)
+    ctx = Ctx()
+    tr = OpTrace(ctx, MT_OPS)
+    src = ctx.upload((np.arange(7 * 16).reshape(7, 16) % 97).astype(np.float16))
+    wide = ctx.alloc((7, 48), np.float16, zero=True)
+    ctx.copy_channels(src, DevTensor(wide.ptr, (7, 16), pitch=48, c_off=16))
+    assert not tr.errors, tr.errors
+    rec = tr.records[0]
+    assert rec.op == "copy_channels" and np.array_equal(_bits(rec.outputs["dst"]), _bits(rec.inputs["src"]))
+    # the op copies src.C = 16 channels, the tracer is told the output is 8 channels wide
+    ctx.copy_channels(src, DevTensor(wide.ptr, (7, 8), pitch=48, c_off=24))
+    tr.stop()
+    assert len(tr.errors) == 1 and "#1 copy_channels" in tr.errors[0] and "outside output 'dst'" in tr.errors[0], tr.errors
+    ctx.close()
