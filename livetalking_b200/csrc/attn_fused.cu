@@ -15,8 +15,7 @@
 // the [B*H][d][keys] buffer transpose_heads writes.  Roles (288 threads): warps 0-7 consumers, warp 8 TMA producer.
 #include <cuda.h>
 
-#include <mutex>
-
+#include "conv_tma.h"
 #include "ltb_internal.h"
 #include "ops.h"
 #include "ptx_sm90.cuh"
@@ -199,33 +198,8 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attn_fused_kernel(const __gri
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn2)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn2 attn_encode_fn() {
-  static EncodeTiledFn2 fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, []() {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn2>(ptr);
-  });
-  return fn;
-}
-
-static bool attn_encode(CUtensorMap* tm, int rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box) {
-  EncodeTiledFn2 fn = attn_encode_fn();
-  if (!fn) return false;
-  cuuint32_t es[5] = {1, 1, 1, 1, 1};
-  return fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, es,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 bool attn_fused_supported(int d, int q_pitch, int kv_pitch, int n_pad) {
-  return d >= 16 && d <= 160 && d % 16 == 0 && q_pitch % 8 == 0 && kv_pitch % 8 == 0 && n_pad % 8 == 0 && attn_encode_fn() != nullptr;
+  return d >= 16 && d <= 160 && d % 16 == 0 && q_pitch % 8 == 0 && kv_pitch % 8 == 0 && n_pad % 8 == 0 && tma_encode_available();
 }
 
 // q: [B][nq] rows of q_pitch elements, head h at columns [h*d, (h+1)*d); k: [B][kv_rows] rows of kv_pitch elements, same head layout;
@@ -240,19 +214,19 @@ cudaError_t launch_attn_fused(const __half* q, int q_pitch, const __half* k, int
     cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)nq, (cuuint64_t)H, (cuuint64_t)B};
     cuuint64_t strides[3] = {(cuuint64_t)q_pitch * 2, (cuuint64_t)d * 2, (cuuint64_t)nq * q_pitch * 2};
     cuuint32_t box[4] = {64, 128, 1, 1};
-    if (!attn_encode(&p.tm_q, 4, q, dims, strides, box)) return cudaErrorInvalidValue;
+    if (!encode_tmap_f16(&p.tm_q, 4, q, dims, strides, box)) return cudaErrorInvalidValue;
   }
   {
     cuuint64_t dims[4] = {(cuuint64_t)d, (cuuint64_t)nk, (cuuint64_t)H, (cuuint64_t)B};
     cuuint64_t strides[3] = {(cuuint64_t)kv_pitch * 2, (cuuint64_t)d * 2, (cuuint64_t)nk * kv_pitch * 2};
     cuuint32_t box[4] = {64, 128, 1, 1};
-    if (!attn_encode(&p.tm_k, 4, k, dims, strides, box)) return cudaErrorInvalidValue;
+    if (!encode_tmap_f16(&p.tm_k, 4, k, dims, strides, box)) return cudaErrorInvalidValue;
   }
   {
     cuuint64_t dims[3] = {(cuuint64_t)n_pad, (cuuint64_t)d, (cuuint64_t)B * H};
     cuuint64_t strides[2] = {(cuuint64_t)n_pad * 2, (cuuint64_t)d * n_pad * 2};
     cuuint32_t box[3] = {64, (cuuint32_t)d, 1};
-    if (!attn_encode(&p.tm_vt, 3, vt, dims, strides, box)) return cudaErrorInvalidValue;
+    if (!encode_tmap_f16(&p.tm_vt, 3, vt, dims, strides, box)) return cudaErrorInvalidValue;
   }
   p.out = out;
   p.out_pitch = out_pitch;

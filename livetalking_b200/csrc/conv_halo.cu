@@ -21,11 +21,10 @@
 // ahead across tiles, so the loads of tile i+1 overlap the epilogue of tile i.
 #include <cuda.h>
 
-#include <atomic>
-#include <mutex>
 #include <utility>
 
 #include "conv_halo.h"
+#include "conv_tma.h"
 #include "ltb_internal.h"
 #include "ptx_sm90.cuh"
 
@@ -632,39 +631,6 @@ __global__ void __launch_bounds__(kHaloThreads, 1) conv_halo_wgmma_kernel(const 
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, []() {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  });
-  return fn;
-}
-
-bool encode_tmap_f16(CUtensorMap* tm, int rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                     const cuuint32_t* box, int spatial_stride, CUtensorMapSwizzle swizzle) {
-  EncodeTiledFn fn = get_encode();
-  if (!fn) return false;
-  cuuint32_t es[5] = {1, (cuuint32_t)spatial_stride, (cuuint32_t)spatial_stride, 1, 1};   // traversal stride of the W and H dimensions
-  return fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes, box, es,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-static bool is_conv3x3(const ConvParams& p) {
-  if (p.nphases != 1 || p.ph[0].ntaps != 9 || p.sy != 1 || p.sx != 1 || p.osy != 1 || p.osx != 1) return false;
-  for (int t = 0; t < 9; ++t)
-    if (p.ph[0].dy[t] != t / 3 - 1 || p.ph[0].dx[t] != t % 3 - 1) return false;
-  return p.IH == p.GH && p.IW == p.GW && p.OH == p.GH && p.OW == p.GW;
-}
 static bool is_convT(const ConvParams& p) {
   if (p.nphases != 4 || p.osy != 2 || p.osx != 2 || p.sy != 1 || p.sx != 1) return false;
   const int nt[4] = {1, 2, 2, 4};
@@ -695,15 +661,15 @@ static bool pick_cfg(const ConvParams& p, int* BN, int* NSUB, int* NACC);
 bool conv_halo_supported(const ConvParams& p) {
   if (p.zbatch > 1) return false;   // the halo kernel runs one GEMM per launch
   // the epilogue writes the output (and reads the residual) 8 channels per 16-byte access
-  if ((p.OCtot % 8) || (p.oc_off % 8) || (reinterpret_cast<uintptr_t>(p.out) % 16)) return false;
-  if (p.res && ((p.RCtot % 8) || (p.rc_off % 8) || (reinterpret_cast<uintptr_t>(p.res) % 16))) return false;
+  if (!tma_slice_ok(p.out, p.OCtot, p.oc_off)) return false;
+  if (p.res && !tma_slice_ok(p.res, p.RCtot, p.rc_off)) return false;
   // grouped weights: GEMM mode only (the weight map's slot stride must be 16-byte aligned); 3x3, stride-2, ConvT and upsample
   // layers go to the gather kernel
   if (p.group_slot && (!is_gemm(p) || (p.w_slot_stride * 2) % 16 != 0)) return false;
   if (is_gemm(p)) {
     // TMA GEMM: K-major rows with 16-byte aligned pitch; worth it from a few M tiles upwards
     return p.Cout % 32 == 0 && p.Cin % 8 == 0 && p.Cin >= 32 && (p.ICtot % 8) == 0 && (p.ic_off % 8) == 0 && (p.Ktot % 8) == 0 &&
-           (p.ph[0].koff % 8) == 0 && p.M >= 512 && get_encode() != nullptr;
+           (p.ph[0].koff % 8) == 0 && p.M >= 512 && tma_encode_available();
   }
   if (is_conv3x3_s2(p)) {
     // parity-plane TMA path: worth it while the 16-row tiles are mostly full (the 8x8 / 4x4 output maps stay on the split-K gather
@@ -711,11 +677,11 @@ bool conv_halo_supported(const ConvParams& p) {
     // 64->128 @64->32: 18.5 -> 14.4 us, 128->256 @32->16: 22.5 -> 14.3 us, but 16->32 @256->128: 38.9 -> 64.1 us (nine K=16
     // instructions per 78 KB of zero-padded plane loads: latency bound) -> Cin >= 64 only.
     return p.Cout % 32 == 0 && p.Cin >= 64 && (p.ICtot % 8) == 0 && (p.ic_off % 8) == 0 && p.Ktot == 9 * p.Cin && p.GH >= 16 &&
-           p.GW >= 8 && get_encode() != nullptr;
+           p.GW >= 8 && tma_encode_available();
   }
   if (is_upconv(p))
-    return p.Cout % 64 == 0 && p.Cin >= 16 && (p.ICtot % 8) == 0 && (p.ic_off % 8) == 0 && p.Ktot == 16 * p.Cin && get_encode() != nullptr;
-  if (!(is_conv3x3(p) || is_convT(p))) return false;
+    return p.Cout % 64 == 0 && p.Cin >= 16 && (p.ICtot % 8) == 0 && (p.ic_off % 8) == 0 && p.Ktot == 16 * p.Cin && tma_encode_available();
+  if (!(conv_is_3x3_same(p) || is_convT(p))) return false;
   // tiles of 16*NSUB x 8 pixels may overhang the map (TMA zero-fills the halo, the epilogue masks the stores): small maps
   // (8x8, 4x4 ...) waste MMA rows but still beat the latency-bound gather kernel
   if (p.Cout % 32 != 0 || p.Cin < 16) return false;
@@ -730,7 +696,7 @@ bool conv_halo_supported(const ConvParams& p) {
     const long waves = (tiles + kSms - 1) / kSms, chunks = (p.Cin + 63) / 64;
     if (waves * chunks > 16) return false;
   }
-  return get_encode() != nullptr;
+  return tma_encode_available();
 }
 
 // picks (BN, NSUB, NACC) ; returns false if unsupported
@@ -816,17 +782,13 @@ int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan
     cuuint64_t wstrides[2] = {(cuuint64_t)p.Ktot * 2, (cuuint64_t)p.w_slot_stride * 2};
     cuuint32_t wbox[3] = {64, (cuuint32_t)BN, 1};
     if (!encode_tmap_f16(&h.tm_w, p.group_slot ? 3 : 2, p.w + p.ph[0].koff, wdims, wstrides, wbox)) return 2;
-  } else
-  // input: 4-D (C, W, H, N) view of the NHWC channel slice
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.IW, (cuuint64_t)p.IH, (cuuint64_t)p.N};
-    cuuint64_t strides[3] = {(cuuint64_t)p.ICtot * 2, (cuuint64_t)p.IW * p.ICtot * 2, (cuuint64_t)p.IH * p.IW * p.ICtot * 2};
+  } else {
     cuuint32_t box[4] = {64, (cuuint32_t)kHaloP, (cuuint32_t)(16 * NSUB + 2), 1};
     if (s2) {   // one parity plane per load: 9 x (16*NSUB + 1) pixels picked with traversal stride 2 (box extent 2n - 1)
       box[1] = 2 * 9 - 1;
       box[2] = 2 * (16 * NSUB + 1) - 1;
     }
-    if (!encode_tmap_f16(&h.tm_in, 4, p.in + p.ic_off, dims, strides, box, s2 ? 2 : 1)) return 2;
+    if (!encode_nhwc_f16(&h.tm_in, p.in + p.ic_off, p.Cin, p.IW, p.IH, p.N, p.ICtot, box, s2 ? 2 : 1)) return 2;
   }
   // weights: 3-D (k = Cin, n = Cout, tap = 9) view of the tap-major copy [9][Cout][Cin]
   if (up) {
@@ -910,19 +872,6 @@ static cudaError_t launch_cfg(const HaloPlan& pl, int sms, cudaStream_t st) {
   return launch_kernel_pdl(conv_halo_wgmma_kernel<BN, NSUB, NACC, TAPS, RC, GRP>, dim3(grid), dim3(kHaloThreads), C::SMEM_BYTES, st, pl.hp);
 }
 
-int conv_halo_sms() {
-  static std::atomic<int> sms_cached{0};
-  int sms = sms_cached.load();
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = kSms;
-    sms_cached.store(sms);
-  }
-  return sms;
-}
-
 // weights-resident variants: 3x3 / ConvT layers with a single N tile, at least two tiles per SM and one or two K chunks of
 // weights (the variants that fit next to the halo ring)
 int conv_halo_resident_chunks(const HaloPlan& pl, int sms) {
@@ -935,7 +884,7 @@ int conv_halo_resident_chunks(const HaloPlan& pl, int sms) {
 }
 
 cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st) {
-  const int sms = conv_halo_sms();
+  const int sms = device_sms();
   if (pl.TAPS == 10) {
     if (pl.NSUB != 1 || pl.NACC != 1) return cudaErrorInvalidValue;
     return pl.BN == 64 ? launch_cfg<64, 1, 1, 10>(pl, sms, st) : (pl.BN == 32 ? launch_cfg<32, 1, 1, 10>(pl, sms, st) : cudaErrorInvalidValue);

@@ -58,12 +58,6 @@ bool conv_halo_supported(const ConvParams& p);
 // w_tap_major: device pointer to the [9][Cout][Cin] copy of the layer's weights (unused in GEMM mode). returns 0 on success.
 int conv_halo_make_plan(const ConvParams& p, const __half* w_tap_major, HaloPlan* out);
 cudaError_t launch_conv_halo(const HaloPlan& pl, cudaStream_t st);
-// fp16 tensor map, out-of-bounds elements read as zero; spatial_stride: traversal stride of dimensions 1 and 2.
-// False if the driver entry point is missing or rejects the map.
-bool encode_tmap_f16(CUtensorMap* tm, int rank, const void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                     const cuuint32_t* box, int spatial_stride = 1, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
-// SM count of the current device (read once), the width of the persistent grid launch_conv_halo sizes
-int conv_halo_sms();
 // K chunks of weights the variant launch_conv_halo runs for pl on `sms` SMs keeps resident (template argument RC); 0: streamed
 int conv_halo_resident_chunks(const HaloPlan& pl, int sms);
 bool conv_halo_gn_fusable(const HaloPlan& pl, int cout_total, int groups, int hw);

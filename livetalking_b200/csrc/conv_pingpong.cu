@@ -26,11 +26,10 @@
 // same sequence of k16 partial sums as on conv_halo_wgmma_kernel<64, 2, 1, 9, 1>.
 #include <cuda.h>
 
-#include <cstdlib>
 #include <cstring>
 
-#include "conv_halo.h"
 #include "conv_pingpong.h"
+#include "conv_tma.h"
 #include "ltb_internal.h"
 #include "ptx_sm90.cuh"
 
@@ -183,54 +182,34 @@ __global__ void __launch_bounds__(kThreads, 1) conv_pingpong_kernel(const __grid
   if (leader) bulk_wait<0>();
 }
 
-static bool pingpong_enabled() {
-  const char* e = std::getenv("LTB_CONV_PINGPONG");   // A/B switch: 0 runs these convs on the halo kernel
-  return !(e && std::strcmp(e, "0") == 0);
-}
-
 bool conv_pingpong_supported(const ConvParams& p) {
-  if (p.zbatch > 1 || p.group_slot || p.upconv || p.nphases != 1 || p.ph[0].ntaps != 9) return false;
-  if (p.sy != 1 || p.sx != 1 || p.osy != 1 || p.osx != 1) return false;
-  for (int t = 0; t < 9; ++t)
-    if (p.ph[0].dy[t] != t / 3 - 1 || p.ph[0].dx[t] != t % 3 - 1) return false;
-  if (p.IH != p.GH || p.IW != p.GW || p.OH != p.GH || p.OW != p.GW) return false;
+  if (p.zbatch > 1 || p.group_slot || p.upconv || !conv_is_3x3_same(p)) return false;
   if (p.Cin != 64 || p.Cout != 64 || p.Ktot != 9 * 64) return false;
   // the residual is the input slice the halo tiles hold
   if (p.res != p.in || p.rc_off != p.ic_off || p.RCtot != p.ICtot) return false;
   // TMA: 16-byte aligned slice starts and pixel pitches
-  if ((p.ICtot % 8) || (p.ic_off % 8) || (p.OCtot % 8) || (p.oc_off % 8) || (reinterpret_cast<uintptr_t>(p.out) % 16) ||
-      (reinterpret_cast<uintptr_t>(p.in) % 16))
-    return false;
+  if (!tma_slice_ok(p.in, p.ICtot, p.ic_off) || !tma_slice_ok(p.out, p.OCtot, p.oc_off)) return false;
   // The kernel clips tiles at any map edge, but only maps whose width is a multiple of the 8-pixel tile are routed here (the
   // wav2lip256 residual layers): other 64-channel maps keep the halo instance their callers were measured and tested on.
   if (p.GW % 8) return false;
   // at least three tiles per SM: each CTA's second warpgroup has a tile whose MMAs run under the first one's epilogue.  Smaller
   // layers stay on the halo kernel, which splits each tile over both warpgroups.
   const long tiles = (long)p.N * ((p.GH + 15) / 16) * ((p.GW + 7) / 8);
-  if (tiles < 3L * conv_halo_sms()) return false;
-  return pingpong_enabled();
+  if (tiles < 3L * device_sms()) return false;
+  return ab_switch_on("LTB_CONV_PINGPONG");   // 0 runs these convs on the halo kernel
 }
 
 int conv_pingpong_make_plan(const ConvParams& p, const __half* w_tap_major, PingpongParams* out) {
   if (!conv_pingpong_supported(p) || !w_tap_major) return 1;
   std::memset(out, 0, sizeof(*out));
-  {
-    const cuuint64_t dims[4] = {64, (cuuint64_t)p.IW, (cuuint64_t)p.IH, (cuuint64_t)p.N};
-    const cuuint64_t strides[3] = {(cuuint64_t)p.ICtot * 2, (cuuint64_t)p.IW * p.ICtot * 2, (cuuint64_t)p.IH * p.IW * p.ICtot * 2};
-    const cuuint32_t box[4] = {64, kP, kHR, 1};
-    if (!encode_tmap_f16(&out->tm_in, 4, p.in + p.ic_off, dims, strides, box)) return 2;
-  }
+  const cuuint32_t in_box[4] = {64, kP, kHR, 1}, out_box[4] = {64, 8, 16, 1};
+  if (!encode_nhwc_f16(&out->tm_in, p.in + p.ic_off, 64, p.IW, p.IH, p.N, p.ICtot, in_box)) return 2;
+  if (!encode_nhwc_f16(&out->tm_out, p.out + p.oc_off, 64, p.OW, p.OH, p.N, p.OCtot, out_box)) return 2;
   {
     const cuuint64_t dims[3] = {64, 64, 9};
     const cuuint64_t strides[2] = {64 * 2, 64 * 64 * 2};
     const cuuint32_t box[3] = {64, 64, 3};
     if (!encode_tmap_f16(&out->tm_w, 3, w_tap_major, dims, strides, box)) return 2;
-  }
-  {
-    const cuuint64_t dims[4] = {64, (cuuint64_t)p.OW, (cuuint64_t)p.OH, (cuuint64_t)p.N};
-    const cuuint64_t strides[3] = {(cuuint64_t)p.OCtot * 2, (cuuint64_t)p.OW * p.OCtot * 2, (cuuint64_t)p.OH * p.OW * p.OCtot * 2};
-    const cuuint32_t box[4] = {64, 8, 16, 1};
-    if (!encode_tmap_f16(&out->tm_out, 4, p.out + p.oc_off, dims, strides, box)) return 2;
   }
   out->bias = p.bias;
   out->relu = p.relu;
@@ -243,7 +222,7 @@ int conv_pingpong_make_plan(const ConvParams& p, const __half* w_tap_major, Ping
 cudaError_t launch_conv_pingpong(const PingpongParams& pp, cudaStream_t st) {
   static SmemConfigOnce once;
   if (cudaError_t e = once.ensure(conv_pingpong_kernel, kSmemBytes); e != cudaSuccess) return e;
-  const int sms = conv_halo_sms();
+  const int sms = device_sms();
   const int grid = pp.total_tiles < sms ? pp.total_tiles : sms;
   return launch_kernel_pdl(conv_pingpong_kernel, dim3(grid), dim3(kThreads), kSmemBytes, st, pp);
 }

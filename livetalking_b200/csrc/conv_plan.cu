@@ -6,6 +6,7 @@
 
 #include "../../include/ltb200.h"
 #include "conv_plan.h"
+#include "conv_tma.h"
 #include "ltb_internal.h"
 
 namespace ltb {
@@ -88,10 +89,7 @@ ConvParams conv_params(ConvMode mode, int N, ConvSlice in, int IH, int IW, int C
 
 int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan* out) {
   out->p = p;
-  out->halo = false;
-  out->pingpong = false;
-  out->rowpair = false;
-  out->smallmap = false;
+  out->kernel = ConvKernel::Gather;
   if (p.group_slot) {
     if (p.group_images < 1 || p.N % p.group_images || p.slots < 1 || p.w_slot_stride < 0 || p.bias_slot_stride < 0)
       return LTB_FAIL("conv: grouped weights need N divisible by group_images >= 1, slots >= 1 and non-negative slot strides");
@@ -100,17 +98,17 @@ int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan*
   if (path == ConvPath::Gather) return 0;
   if (path == ConvPath::Auto && conv_smallmap_supported(p)) {
     if (conv_smallmap_make_plan(p, &out->sp) != 0) return LTB_FAIL("conv: small-map plan / tensor map creation failed");
-    out->smallmap = true;
+    out->kernel = ConvKernel::Smallmap;
     return 0;
   }
   if (w_tap && conv_pingpong_supported(p)) {
     if (conv_pingpong_make_plan(p, w_tap, &out->pp) != 0) return LTB_FAIL("conv: ping-pong plan / tensor map creation failed");
-    out->pingpong = true;
+    out->kernel = ConvKernel::Pingpong;
     return 0;
   }
   if (w_tap && conv_rowpair_supported(p)) {
     if (conv_rowpair_make_plan(p, w_tap, &out->rp) != 0) return LTB_FAIL("conv: row-pair plan / tensor map creation failed");
-    out->rowpair = true;
+    out->kernel = ConvKernel::Rowpair;
     return 0;
   }
   const bool gemm = p.nphases == 1 && p.ph[0].ntaps == 1;   // the halo kernel's GEMM mode reads the K-major rows
@@ -121,56 +119,57 @@ int conv_plan(const ConvParams& p, const __half* w_tap, ConvPath path, ConvPlan*
                     (w_tap || gemm ? "" : " without tap-major weights"));
   }
   if (conv_halo_make_plan(p, w_tap, &out->hp) != 0) return LTB_FAIL("conv: halo plan / tensor map creation failed");
-  out->halo = true;
+  out->kernel = ConvKernel::Halo;
   return 0;
 }
 
 cudaError_t conv_launch(const ConvPlan& pl, cudaStream_t st, float* splitk_ws, size_t ws_floats) {
-  if (pl.pingpong) return launch_conv_pingpong(pl.pp, st);
-  if (pl.rowpair) return launch_conv_rowpair(pl.rp, st);
-  if (pl.smallmap) return launch_conv_smallmap(pl.sp, st);
-  return pl.halo ? launch_conv_halo(pl.hp, st) : launch_conv_gather(pl.p, st, splitk_ws, ws_floats);
+  switch (pl.kernel) {
+    case ConvKernel::Gather: return launch_conv_gather(pl.p, st, splitk_ws, ws_floats);
+    case ConvKernel::Halo: return launch_conv_halo(pl.hp, st);
+    case ConvKernel::Pingpong: return launch_conv_pingpong(pl.pp, st);
+    case ConvKernel::Rowpair: return launch_conv_rowpair(pl.rp, st);
+    case ConvKernel::Smallmap: return launch_conv_smallmap(pl.sp, st);
+  }
+  return cudaErrorInvalidValue;
 }
 
 bool conv_plan_variant(const ConvPlan& pl, bool have_ws, size_t ws_floats, ltb_conv_variant* out) {
   std::memset(out, 0, sizeof(*out));
+  out->kernel = int(pl.kernel);
   out->grouped = pl.p.group_slot != nullptr;
-  if (pl.pingpong) {   // one instance: 3x3, 64 output channels, one 128-pixel tile per warpgroup, resident weights
-    out->kernel = 2;
-    out->taps = 9;
-    out->bn = 64;
-    out->nsub = 1;
-    out->nacc = 1;
-    out->resident_chunks = 1;
-    out->res_halo = 1;
-    return true;
-  }
-  if (pl.rowpair) {   // one instance: 3x3, 32 output channels, two resident K chunks
-    out->kernel = 3;
-    out->taps = 9;
-    out->bn = 32;
-    out->nsub = 1;
-    out->nacc = 1;
-    out->resident_chunks = 2;
-    return true;
-  }
-  if (pl.smallmap) {   // 128 output channels per CTA, 64-channel K steps, ksplit CTAs of a cluster per output tile
-    out->kernel = 4;
-    for (int i = 0; i < pl.p.nphases; ++i) out->taps += pl.p.ph[i].ntaps;
-    out->bn = 128;
-    out->kb = 64;
-    out->ksplit = pl.sp.ksplit;
-    return true;
-  }
-  if (pl.halo) {
-    out->kernel = 1;
-    out->taps = pl.hp.TAPS;
-    out->bn = pl.hp.BN;
-    out->nsub = pl.hp.NSUB;
-    out->nacc = pl.hp.NACC;
-    out->resident_chunks = conv_halo_resident_chunks(pl.hp, conv_halo_sms());
-    out->res_halo = pl.hp.hp.res_halo;
-    return true;
+  switch (pl.kernel) {
+    case ConvKernel::Pingpong:   // one instance: 3x3, 64 output channels, one 128-pixel tile per warpgroup, resident weights
+      out->taps = 9;
+      out->bn = 64;
+      out->nsub = 1;
+      out->nacc = 1;
+      out->resident_chunks = 1;
+      out->res_halo = 1;
+      return true;
+    case ConvKernel::Rowpair:   // one instance: 3x3, 32 output channels, two resident K chunks
+      out->taps = 9;
+      out->bn = 32;
+      out->nsub = 1;
+      out->nacc = 1;
+      out->resident_chunks = 2;
+      return true;
+    case ConvKernel::Smallmap:   // 128 output channels per CTA, 64-channel K steps, ksplit CTAs of a cluster per output tile
+      for (int i = 0; i < pl.p.nphases; ++i) out->taps += pl.p.ph[i].ntaps;
+      out->bn = 128;
+      out->kb = 64;
+      out->ksplit = pl.sp.ksplit;
+      return true;
+    case ConvKernel::Halo:
+      out->taps = pl.hp.TAPS;
+      out->bn = pl.hp.BN;
+      out->nsub = pl.hp.NSUB;
+      out->nacc = pl.hp.NACC;
+      out->resident_chunks = conv_halo_resident_chunks(pl.hp, device_sms());
+      out->res_halo = pl.hp.hp.res_halo;
+      return true;
+    case ConvKernel::Gather:
+      break;
   }
   int ksplit = 0;
   if (!conv_gather_pick(pl.p, have_ws, ws_floats, &out->bn, &out->kb, &ksplit)) return false;
@@ -180,7 +179,9 @@ bool conv_plan_variant(const ConvPlan& pl, bool have_ws, size_t ws_floats, ltb_c
 
 bool conv_plan_fuse_gn_stats(ConvPlan* pl, float* stats, int groups, int hw) {
   const ConvParams& p = pl->p;
-  if (!pl->halo || pl->hp.grouped || p.oc_off != 0 || p.OCtot != p.Cout || !conv_halo_gn_fusable(pl->hp, p.Cout, groups, hw)) return false;
+  if (pl->kernel != ConvKernel::Halo || pl->hp.grouped || p.oc_off != 0 || p.OCtot != p.Cout ||
+      !conv_halo_gn_fusable(pl->hp, p.Cout, groups, hw))
+    return false;
   HaloParams& h = pl->hp.hp;
   h.gn_stats = stats;
   h.gn_groups = groups;
@@ -191,13 +192,13 @@ bool conv_plan_fuse_gn_stats(ConvPlan* pl, float* stats, int groups, int hw) {
 }
 
 bool conv_plan_fuse_head(ConvPlan* pl, const float* w, const float* b, float* out) {
-  if (pl->rowpair) {
+  if (pl->kernel == ConvKernel::Rowpair) {
     pl->rp.head_w = w;
     pl->rp.head_b = b;
     pl->rp.head_out = out;
     return true;
   }
-  if (!pl->halo || pl->hp.grouped || pl->hp.BN != 32 || pl->p.Cout != 32) return false;
+  if (pl->kernel != ConvKernel::Halo || pl->hp.grouped || pl->hp.BN != 32 || pl->p.Cout != 32) return false;
   pl->hp.hp.head_w = w;
   pl->hp.hp.head_b = b;
   pl->hp.hp.head_out = out;
@@ -304,7 +305,7 @@ static int conv2d_f16_impl(const ltb_conv_desc* d, const void* in_f16, const flo
     cleanup();
     return 1;
   }
-  const size_t ws_floats = (pl.halo || pl.pingpong || pl.rowpair) ? 0 : (size_t)1 << 22;
+  const size_t ws_floats = pl.kernel == ConvKernel::Gather ? (size_t)1 << 22 : 0;   // split-K workspace of the gather kernel
   if (ws_floats) {
     CK(cudaMalloc(&dws, ws_floats * sizeof(float)));
     CK(cudaMemset(dws, 0, ws_floats * sizeof(float)));

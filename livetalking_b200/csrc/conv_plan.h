@@ -37,21 +37,20 @@ ConvParams conv_params(ConvMode mode, int N, ConvSlice in, int IH, int IW, int C
                        ConvSlice res, const __half* w, int Ktot, int w_koff, const float* bias, bool relu, ConvTaps taps = {});
 
 enum class ConvPath {
-  Auto,    // a TMA kernel (ping-pong, row-pair or halo) when one supports the geometry and has its weights (w_tap, or none needed in
-           // GEMM mode), else gather
+  Auto,    // the small-map kernel for a layer that opts in (ConvParams::smallmap) and fits it, else a TMA kernel (ping-pong,
+           // row-pair or halo) when one supports the geometry and has its weights (w_tap, or none needed in GEMM mode), else gather
   Gather,  // gather kernel
-  Halo,    // a TMA kernel, or fail
+  Halo,    // a TMA kernel (ping-pong, row-pair or halo), or fail
 };
+// the kernel a plan runs; the values are those ltb_conv_variant::kernel reports
+enum class ConvKernel { Gather = 0, Halo = 1, Pingpong = 2, Rowpair = 3, Smallmap = 4 };
 struct ConvPlan {
   ConvParams p{};
-  bool halo = false;
-  HaloPlan hp{};  // halo == true only
-  bool pingpong = false;
-  PingpongParams pp{};  // pingpong == true only
-  bool rowpair = false;
-  RowpairParams rp{};   // rowpair == true only
-  bool smallmap = false;
-  SmallmapParams sp{};  // smallmap == true only
+  ConvKernel kernel = ConvKernel::Gather;
+  HaloPlan hp{};        // Halo only
+  PingpongParams pp{};  // Pingpong only
+  RowpairParams rp{};   // Rowpair only
+  SmallmapParams sp{};  // Smallmap only
 };
 
 // w_tap: device copy of the weights in the halo kernel's tap-major layout (see launch_w_tap_major*); null if there is none.

@@ -28,11 +28,10 @@
 // conv_halo_wgmma_kernel<32, 2, 1, 9, 2>: the outputs are bit-identical.
 #include <cuda.h>
 
-#include <cstdlib>
 #include <cstring>
 
-#include "conv_halo.h"
 #include "conv_rowpair.h"
+#include "conv_tma.h"
 #include "ltb_internal.h"
 #include "ptx_sm90.cuh"
 
@@ -241,39 +240,26 @@ __global__ void __launch_bounds__(kThreads, 1) conv_rowpair_kernel(const __grid_
   if (leader) bulk_wait<0>();
 }
 
-static bool rowpair_enabled() {
-  const char* e = std::getenv("LTB_CONV_ROWPAIR");   // A/B switch: 0 runs these convs on the halo kernel
-  return !(e && std::strcmp(e, "0") == 0);
-}
-
 bool conv_rowpair_supported(const ConvParams& p) {
-  if (p.zbatch > 1 || p.group_slot || p.upconv || p.nphases != 1 || p.ph[0].ntaps != 9) return false;
-  if (p.sy != 1 || p.sx != 1 || p.osy != 1 || p.osx != 1) return false;
-  for (int t = 0; t < 9; ++t)
-    if (p.ph[0].dy[t] != t / 3 - 1 || p.ph[0].dx[t] != t % 3 - 1) return false;
-  if (p.IH != p.GH || p.IW != p.GW || p.OH != p.GH || p.OW != p.GW) return false;
+  if (p.zbatch > 1 || p.group_slot || p.upconv || !conv_is_3x3_same(p)) return false;
   // The kernel takes any Cin in 65..80 (the second chunk is one K step of 16 channels), but only the wav2lip256 output conv's
   // 80 channels are routed here: other narrow convs keep the halo instances their callers were measured and tested on.
   if (p.Cin != 80 || p.Cout != 32 || p.Ktot != 9 * 80 || p.res) return false;
   // TMA: 16-byte aligned slice starts and pixel pitches
-  if ((p.ICtot % 8) || (p.ic_off % 8) || (p.OCtot % 8) || (p.oc_off % 8) || (reinterpret_cast<uintptr_t>(p.out) % 16) ||
-      (reinterpret_cast<uintptr_t>(p.in) % 16))
-    return false;
+  if (!tma_slice_ok(p.in, p.ICtot, p.ic_off) || !tma_slice_ok(p.out, p.OCtot, p.oc_off)) return false;
   // at least three tiles per SM: each CTA's second warpgroup has a tile whose MMAs run under the first one's epilogue
   const long tiles = (long)p.N * ((p.GH + kTH - 1) / kTH) * ((p.GW + 7) / 8);
-  if (tiles < 3L * conv_halo_sms()) return false;
-  return rowpair_enabled();
+  if (tiles < 3L * device_sms()) return false;
+  return ab_switch_on("LTB_CONV_ROWPAIR");   // 0 runs these convs on the halo kernel
 }
 
 int conv_rowpair_make_plan(const ConvParams& p, const __half* w_tap_major, RowpairParams* out) {
   if (!conv_rowpair_supported(p) || !w_tap_major) return 1;
   std::memset(out, 0, sizeof(*out));
   {
-    const cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.IW, (cuuint64_t)p.IH, (cuuint64_t)p.N};
-    const cuuint64_t strides[3] = {(cuuint64_t)p.ICtot * 2, (cuuint64_t)p.IW * p.ICtot * 2, (cuuint64_t)p.IH * p.IW * p.ICtot * 2};
     const cuuint32_t box0[4] = {64, kP, kHR, 1}, box1[4] = {16, kP, kHR, 1};
-    if (!encode_tmap_f16(&out->tm_x0, 4, p.in + p.ic_off, dims, strides, box0)) return 2;
-    if (!encode_tmap_f16(&out->tm_x1, 4, p.in + p.ic_off, dims, strides, box1, 1, CU_TENSOR_MAP_SWIZZLE_32B)) return 2;
+    if (!encode_nhwc_f16(&out->tm_x0, p.in + p.ic_off, p.Cin, p.IW, p.IH, p.N, p.ICtot, box0)) return 2;
+    if (!encode_nhwc_f16(&out->tm_x1, p.in + p.ic_off, p.Cin, p.IW, p.IH, p.N, p.ICtot, box1, 1, CU_TENSOR_MAP_SWIZZLE_32B)) return 2;
   }
   {
     const cuuint64_t dims[3] = {(cuuint64_t)p.Cin, 32, 9};
@@ -283,10 +269,8 @@ int conv_rowpair_make_plan(const ConvParams& p, const __half* w_tap_major, Rowpa
     if (!encode_tmap_f16(&out->tm_w1, 3, w_tap_major, dims, strides, box1, 1, CU_TENSOR_MAP_SWIZZLE_32B)) return 2;
   }
   {
-    const cuuint64_t dims[4] = {32, (cuuint64_t)p.OW, (cuuint64_t)p.OH, (cuuint64_t)p.N};
-    const cuuint64_t strides[3] = {(cuuint64_t)p.OCtot * 2, (cuuint64_t)p.OW * p.OCtot * 2, (cuuint64_t)p.OH * p.OW * p.OCtot * 2};
     const cuuint32_t box[4] = {32, 8, kTH, 1};
-    if (!encode_tmap_f16(&out->tm_out, 4, p.out + p.oc_off, dims, strides, box, 1, CU_TENSOR_MAP_SWIZZLE_64B)) return 2;
+    if (!encode_nhwc_f16(&out->tm_out, p.out + p.oc_off, 32, p.OW, p.OH, p.N, p.OCtot, box, 1, CU_TENSOR_MAP_SWIZZLE_64B)) return 2;
   }
   out->bias = p.bias;
   out->relu = p.relu;
@@ -301,7 +285,7 @@ int conv_rowpair_make_plan(const ConvParams& p, const __half* w_tap_major, Rowpa
 cudaError_t launch_conv_rowpair(const RowpairParams& rp, cudaStream_t st) {
   static SmemConfigOnce once;
   if (cudaError_t e = once.ensure(conv_rowpair_kernel, kSmemBytes); e != cudaSuccess) return e;
-  const int sms = conv_halo_sms();
+  const int sms = device_sms();
   const int grid = rp.total_tiles < sms ? rp.total_tiles : sms;
   return launch_kernel_pdl(conv_rowpair_kernel, dim3(grid), dim3(kThreads), kSmemBytes, st, rp);
 }

@@ -17,11 +17,10 @@
 // Roles (288 threads): warpgroups 0 and 1 consume (MMAs), warp 8 is the TMA producer; all nine warps reduce.
 #include <cuda.h>
 
-#include <cstdlib>
 #include <cstring>
 
-#include "conv_halo.h"
 #include "conv_smallmap.h"
+#include "conv_tma.h"
 #include "ltb_internal.h"
 #include "ptx_sm90.cuh"
 
@@ -179,11 +178,6 @@ __global__ void __launch_bounds__(kThreads, 1) conv_smallmap_kernel(const __grid
   cluster_sync();   // no CTA leaves while another still reads its shared memory
 }
 
-static bool smallmap_enabled() {
-  const char* e = std::getenv("LTB_CONV_SMALLMAP");   // A/B switch: 0 keeps these layers on the halo / gather kernels
-  return !(e && std::strcmp(e, "0") == 0);
-}
-
 static int pick_np(const ConvParams& p) {
   const int g = p.GH * p.GW;
   return (p.GH == 8 && p.GW == 8) ? 256 : (p.GH == 4 && p.GW == 4) ? 64 : g == 1 ? 16 : 0;
@@ -204,7 +198,7 @@ bool conv_smallmap_supported(const ConvParams& p) {
     return false;
   for (int i = 0; i < p.nphases; ++i)
     if (p.ph[i].koff % 8 || p.ph[i].ntaps < 1) return false;
-  return smallmap_enabled();
+  return ab_switch_on("LTB_CONV_SMALLMAP");   // 0 keeps these layers on the halo / gather kernels
 }
 
 int conv_smallmap_make_plan(const ConvParams& p, SmallmapParams* out) {
@@ -229,10 +223,8 @@ int conv_smallmap_make_plan(const ConvParams& p, SmallmapParams* out) {
   out->ksplit = ks;
   {
     const int sx = p.nphases == 1 ? p.sx : 1;
-    const cuuint64_t dims[4] = {(cuuint64_t)p.Cin, (cuuint64_t)p.IW, (cuuint64_t)p.IH, (cuuint64_t)p.N};
-    const cuuint64_t strides[3] = {(cuuint64_t)p.ICtot * 2, (cuuint64_t)p.IW * p.ICtot * 2, (cuuint64_t)p.IH * p.IW * p.ICtot * 2};
     const cuuint32_t box[4] = {64, (cuuint32_t)((p.GW - 1) * sx + 1), (cuuint32_t)((p.GH - 1) * sx + 1), (cuuint32_t)out->bimg};
-    if (!encode_tmap_f16(&out->tm_in, 4, p.in + p.ic_off, dims, strides, box, sx)) return 2;
+    if (!encode_nhwc_f16(&out->tm_in, p.in + p.ic_off, p.Cin, p.IW, p.IH, p.N, p.ICtot, box, sx)) return 2;
   }
   {
     const cuuint64_t dims[2] = {(cuuint64_t)p.Ktot, (cuuint64_t)p.Cout};

@@ -11,8 +11,8 @@
 #include <cuda.h>
 
 #include <cstring>
-#include <mutex>
 
+#include "conv_tma.h"
 #include "ltb_internal.h"
 #include "ptx_sm90.cuh"
 #include "stem_umma.h"
@@ -117,38 +117,20 @@ __global__ void __launch_bounds__(kStemThreads, 1) stem_umma_kernel(const __grid
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 int stem_make_plan(const __half* img_pad, int B, const __half* w_tap_major, const float* bias, __half* out, int OCtot, int oc_off,
                    StemParams* sp) {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, []() {
-    void* q = nullptr;
-    cudaDriverEntryPointQueryResult r;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &q, cudaEnableDefault, &r) == cudaSuccess && r == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(q);
-  });
-  if (!fn) return 1;
   std::memset(sp, 0, sizeof(*sp));
-  cuuint32_t es[4] = {1, 1, 1, 1};
   {
     cuuint64_t dims[4] = {8, 264, 262, (cuuint64_t)B};
     cuuint64_t strides[3] = {16, 264 * 16, (cuuint64_t)262 * 264 * 16};
     cuuint32_t box[4] = {8, 16, 22, 1};
-    if (fn(&sp->tm_in, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(img_pad), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return 2;
+    if (!encode_tmap_f16(&sp->tm_in, 4, img_pad, dims, strides, box, 1, CU_TENSOR_MAP_SWIZZLE_NONE)) return 2;
   }
   {
     cuuint64_t dims[3] = {64, 16, 7};
     cuuint64_t strides[2] = {128, 16 * 128};
     cuuint32_t box[3] = {64, 16, 7};
-    if (fn(&sp->tm_w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(w_tap_major), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return 2;
+    if (!encode_tmap_f16(&sp->tm_w, 3, w_tap_major, dims, strides, box)) return 2;
   }
   sp->out = out;
   sp->bias = bias;
@@ -160,17 +142,9 @@ int stem_make_plan(const __half* img_pad, int B, const __half* w_tap_major, cons
 
 cudaError_t launch_stem(const StemParams& sp, cudaStream_t st) {
   static SmemConfigOnce once;
-  static std::atomic<int> sms_cached{0};
   constexpr int smem = kStemWBytes + kStemStages * kStemAStride + 1024;
   if (cudaError_t e = once.ensure(stem_umma_kernel, smem); e != cudaSuccess) return e;
-  int sms = sms_cached.load();
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 132;
-    sms_cached.store(sms);
-  }
+  const int sms = device_sms();
   const int grid = sp.total_tiles < sms ? sp.total_tiles : sms;
   return launch_kernel_pdl(stem_umma_kernel, dim3(grid), dim3(kStemThreads), smem, st, sp);
 }

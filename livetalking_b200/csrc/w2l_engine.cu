@@ -353,7 +353,10 @@ static int build_plan(ltb_w2l_session* s) {
     ConvParams p = p_in;
     p.smallmap = (li >= kFirstSmallmap && li <= kLastSmallmap) ? 1 : 0;
     if (conv_plan(p, m->wt[li], path, &o.conv)) return LTB_FAIL("plan: layer " + std::to_string(li) + ": " + g_last_error);
-    o.type = (o.conv.halo || o.conv.pingpong || o.conv.rowpair) ? 4 : 0;   // 4: a TMA conv kernel
+    // 4: a TMA conv kernel.  The small-map kernel reports kind 0, as the gather kernel does: bench.py and the layer tests read
+    // these kinds.
+    const ConvKernel k = o.conv.kernel;
+    o.type = (k == ConvKernel::Halo || k == ConvKernel::Pingpong || k == ConvKernel::Rowpair) ? 4 : 0;
     s->ops.push_back(o);
     return 0;
   };

@@ -6,10 +6,9 @@ channels x 16 row pairs of 8 pixels), and the epilogue goes through stmatrix (ST
 tensor store (UTMASTG)."""
 import os
 import re
-import shutil
-import subprocess
 
 import pytest
+from sass_build import compile_sass
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "livetalking_b200", "csrc", "conv_rowpair.cu")
@@ -17,16 +16,7 @@ SRC = os.path.join(ROOT, "livetalking_b200", "csrc", "conv_rowpair.cu")
 
 @pytest.fixture(scope="module")
 def compiled(tmp_path_factory):
-    from livetalking_b200 import build
-    nvcc = build._nvcc()
-    cuobjdump = shutil.which("cuobjdump") or os.path.join(os.path.dirname(nvcc), "cuobjdump")
-    if not os.path.exists(cuobjdump):
-        pytest.skip("cuobjdump not available")
-    obj = str(tmp_path_factory.mktemp("rowpair") / "conv_rowpair.o")
-    r = subprocess.run([nvcc, *build.NVCC_FLAGS, "-Xptxas", "-v", "-c", SRC, "-o", obj], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
-    return r.stdout + r.stderr, sass
+    return compile_sass(SRC, tmp_path_factory.mktemp("rowpair"))
 
 
 def test_rowpair_kernel_has_no_spills_or_wgmma_serialisation(compiled):

@@ -5,10 +5,9 @@ not serialise their wgmma pipeline (no C75xx advisory), operands arrive by TMA (
 N, and the split-K partials are reduced across the CTAs of a cluster between cluster barriers."""
 import os
 import re
-import shutil
-import subprocess
 
 import pytest
+from sass_build import compile_sass
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "livetalking_b200", "csrc", "conv_smallmap.cu")
@@ -16,16 +15,7 @@ SRC = os.path.join(ROOT, "livetalking_b200", "csrc", "conv_smallmap.cu")
 
 @pytest.fixture(scope="module")
 def compiled(tmp_path_factory):
-    from livetalking_b200 import build
-    nvcc = build._nvcc()
-    cuobjdump = shutil.which("cuobjdump") or os.path.join(os.path.dirname(nvcc), "cuobjdump")
-    if not os.path.exists(cuobjdump):
-        pytest.skip("cuobjdump not available")
-    obj = str(tmp_path_factory.mktemp("smallmap") / "conv_smallmap.o")
-    r = subprocess.run([nvcc, *build.NVCC_FLAGS, "-Xptxas", "-v", "-c", SRC, "-o", obj], capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
-    return r.stdout + r.stderr, sass
+    return compile_sass(SRC, tmp_path_factory.mktemp("smallmap"))
 
 
 def test_smallmap_kernels_have_no_spills_or_wgmma_serialisation(compiled):

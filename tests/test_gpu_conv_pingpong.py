@@ -8,12 +8,11 @@ neighbours hold sentinels, outputs go into a channel slice of a wider buffer, an
 
 Convs without a residual, or whose residual is another tensor, stay on the halo kernel (the S3FD, BiSeNet and UltraLight plans
 pin that), as do maps whose width is not a multiple of 8 and layers with fewer tiles (the wav2lip256 audio encoder)."""
-import types
-
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
+from conv_cases import bits, ctx, slice_buf, weights
 
 pytestmark = pytest.mark.gpu
 
@@ -25,44 +24,11 @@ PINGPONG = dict(kernel=2, taps=9, bn=64, nsub=1, nacc=1, resident_chunks=1, kb=0
 CASES = [(16, 64, 64), (16, 72, 80), (3, 150, 152)]
 
 
-@pytest.fixture(scope="module")
-def ctx():
-    from livetalking_b200 import engine
-    from livetalking_b200.ops import Ctx
-    engine.set_device(0)
-    c = Ctx()
-    yield c
-    c.close()
-
-
 @pytest.fixture
 def switch(monkeypatch):
     def set_(on):
         monkeypatch.setenv("LTB_CONV_PINGPONG", "1" if on else "0")
     return set_
-
-
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint16)
-
-
-def _slice_buf(ctx, dense, pitch, off, fill):
-    from livetalking_b200.ops import DevTensor
-    buf = np.full(dense.shape[:-1] + (pitch,), fill, np.float16)
-    buf[..., off:off + dense.shape[-1]] = dense
-    t = ctx.upload(buf)
-    return DevTensor(t.ptr, dense.shape, pitch=pitch, c_off=off), t, buf
-
-
-def _weights(ctx, g, C=64):
-    w = (torch.randn(C, C, 3, 3, generator=g) * (2.0 / (C * 9)) ** 0.5).half()
-    b = torch.randn(C, generator=g) * 0.2
-    wt = ctx.upload(w.permute(0, 2, 3, 1).reshape(C, 9 * C).numpy())
-    bt = ctx.upload(b.numpy().astype(np.float32))
-    wtap = ctx.alloc((9, C, C))
-    ctx.w_tap_major(wt, wtap, C, C)
-    cw = types.SimpleNamespace(cout=C, cin=C, kh=3, kw=3, ktot=9 * C, w=wt, w_tap=wtap, bias=bt)
-    return w, b, cw, [wt, bt, wtap]
 
 
 @pytest.mark.parametrize("relu", [True, False], ids=["relu", "no_relu"])
@@ -71,14 +37,14 @@ def test_pingpong_equals_halo_kernel(ctx, switch, shape, relu):
     N, H, W = shape
     g = torch.Generator().manual_seed(N * 1000 + H + W + relu)
     x = (torch.randn(N, H, W, 64, generator=g) * 0.7 + 0.2 + torch.randn(64, generator=g) * 0.3).half()
-    w, b, cw, temps = _weights(ctx, g)
-    xv, xt, xbuf = _slice_buf(ctx, x.numpy(), 88, 8, SENT_IN)
+    w, b, cw, temps = weights(ctx, g, 64, 64)
+    xv, xt, xbuf = slice_buf(ctx, x.numpy(), 88, 8, SENT_IN)
     temps.append(xt)
     outs = {}
     try:
         for on in (False, True):
             switch(on)
-            ov, ot, obuf = _slice_buf(ctx, np.full((N, H, W, 64), np.nan, np.float16), 80, 8, SENT_OUT)
+            ov, ot, obuf = slice_buf(ctx, np.full((N, H, W, 64), np.nan, np.float16), 80, 8, SENT_OUT)
             temps.append(ot)
             geo = dict(N=N, IH=H, IW=W, OH=H, OW=W, pad=(1, 1), relu=relu, res=xv)
             variant = ctx.conv_plan(xv, cw, ov, **geo)
@@ -90,11 +56,11 @@ def test_pingpong_equals_halo_kernel(ctx, switch, shape, relu):
             full = ctx.download(ot)
             outside = np.ones(obuf.shape, bool)
             outside[..., 8:72] = False
-            assert np.array_equal(_bits(full)[outside], _bits(obuf)[outside]), f"pingpong={on}: wrote outside the output slice"
+            assert np.array_equal(bits(full)[outside], bits(obuf)[outside]), f"pingpong={on}: wrote outside the output slice"
             outs[on] = full[..., 8:72]
-        assert np.array_equal(_bits(ctx.download(xt)), _bits(xbuf)), "the conv changed its input buffer"
+        assert np.array_equal(bits(ctx.download(xt)), bits(xbuf)), "the conv changed its input buffer"
         assert np.isfinite(outs[True].astype(np.float32)).all(), "unwritten outputs"
-        diff = _bits(outs[True]) != _bits(outs[False])
+        diff = bits(outs[True]) != bits(outs[False])
         assert not diff.any(), f"{int(diff.sum())} of {diff.size} outputs differ from the halo kernel, first at {np.argwhere(diff)[0]}"
         # and both against float64 (the tolerance of test_gpu_conv_res_halo)
         x64 = x[:1].double().permute(0, 3, 1, 2)
@@ -112,7 +78,7 @@ def test_wav2lip_decoder_layers_plan_pingpong(ctx, switch):
     256 x 256, each with its input as residual, plan the ping-pong kernel; with the switch off, the halo kernel."""
     from livetalking_b200.ops import DevTensor
     g = torch.Generator().manual_seed(51)
-    _, _, cw, temps = _weights(ctx, g)
+    _, _, cw, temps = weights(ctx, g, 64, 64)
     N, S = 16, 256
     a = ctx.alloc((N, S, S, 64))
     cat7 = ctx.alloc((N, S, S, 80))

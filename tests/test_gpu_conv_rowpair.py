@@ -6,12 +6,11 @@ on the same inputs and weights both ways in one process and requires bit-identic
 the halo kernel's order (its extra products are exact zeros) and rounds in the halo kernel's order.  The input is an 80-channel
 slice whose neighbours hold sentinels, the output goes into a channel slice of a wider buffer, and nothing outside it may
 change.  The fused head is checked through the whole wav2lip256 forward, whose pred it writes."""
-import types
-
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
+from conv_cases import bits, ctx, slice_buf, weights
 
 pytestmark = pytest.mark.gpu
 
@@ -23,44 +22,11 @@ ROWPAIR = dict(kernel=3, taps=9, bn=32, nsub=1, nacc=1, resident_chunks=2, kb=0,
 CASES = [(16, 72, 80), (16, 96, 72), (3, 200, 204)]
 
 
-@pytest.fixture(scope="module")
-def ctx():
-    from livetalking_b200 import engine
-    from livetalking_b200.ops import Ctx
-    engine.set_device(0)
-    c = Ctx()
-    yield c
-    c.close()
-
-
 @pytest.fixture
 def switch(monkeypatch):
     def set_(on):
         monkeypatch.setenv("LTB_CONV_ROWPAIR", "1" if on else "0")
     return set_
-
-
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint16)
-
-
-def _slice_buf(ctx, dense, pitch, off, fill):
-    from livetalking_b200.ops import DevTensor
-    buf = np.full(dense.shape[:-1] + (pitch,), fill, np.float16)
-    buf[..., off:off + dense.shape[-1]] = dense
-    t = ctx.upload(buf)
-    return DevTensor(t.ptr, dense.shape, pitch=pitch, c_off=off), t, buf
-
-
-def _weights(ctx, g, cin=80, cout=32):
-    w = (torch.randn(cout, cin, 3, 3, generator=g) * (2.0 / (cin * 9)) ** 0.5).half()
-    b = torch.randn(cout, generator=g) * 0.2
-    wt = ctx.upload(w.permute(0, 2, 3, 1).reshape(cout, 9 * cin).numpy())
-    bt = ctx.upload(b.numpy().astype(np.float32))
-    wtap = ctx.alloc((9, cout, cin))
-    ctx.w_tap_major(wt, wtap, cout, cin)
-    cw = types.SimpleNamespace(cout=cout, cin=cin, kh=3, kw=3, ktot=9 * cin, w=wt, w_tap=wtap, bias=bt)
-    return w, b, cw, [wt, bt, wtap]
 
 
 @pytest.mark.parametrize("relu", [True, False], ids=["relu", "no_relu"])
@@ -69,14 +35,14 @@ def test_rowpair_equals_halo_kernel(ctx, switch, shape, relu):
     N, H, W = shape
     g = torch.Generator().manual_seed(N * 1000 + H + W + relu)
     x = (torch.randn(N, H, W, 80, generator=g) * 0.7 + 0.2 + torch.randn(80, generator=g) * 0.3).half()
-    w, b, cw, temps = _weights(ctx, g)
-    xv, xt, xbuf = _slice_buf(ctx, x.numpy(), 96, 8, SENT_IN)
+    w, b, cw, temps = weights(ctx, g, 80, 32)
+    xv, xt, xbuf = slice_buf(ctx, x.numpy(), 96, 8, SENT_IN)
     temps.append(xt)
     outs = {}
     try:
         for on in (False, True):
             switch(on)
-            ov, ot, obuf = _slice_buf(ctx, np.full((N, H, W, 32), np.nan, np.float16), 48, 8, SENT_OUT)
+            ov, ot, obuf = slice_buf(ctx, np.full((N, H, W, 32), np.nan, np.float16), 48, 8, SENT_OUT)
             temps.append(ot)
             geo = dict(N=N, IH=H, IW=W, OH=H, OW=W, pad=(1, 1), relu=relu)
             variant = ctx.conv_plan(xv, cw, ov, **geo)
@@ -88,11 +54,11 @@ def test_rowpair_equals_halo_kernel(ctx, switch, shape, relu):
             full = ctx.download(ot)
             outside = np.ones(obuf.shape, bool)
             outside[..., 8:40] = False
-            assert np.array_equal(_bits(full)[outside], _bits(obuf)[outside]), f"rowpair={on}: wrote outside the output slice"
+            assert np.array_equal(bits(full)[outside], bits(obuf)[outside]), f"rowpair={on}: wrote outside the output slice"
             outs[on] = full[..., 8:40]
-        assert np.array_equal(_bits(ctx.download(xt)), _bits(xbuf)), "the conv changed its input buffer"
+        assert np.array_equal(bits(ctx.download(xt)), bits(xbuf)), "the conv changed its input buffer"
         assert np.isfinite(outs[True].astype(np.float32)).all(), "unwritten outputs"
-        diff = _bits(outs[True]) != _bits(outs[False])
+        diff = bits(outs[True]) != bits(outs[False])
         assert not diff.any(), f"{int(diff.sum())} of {diff.size} outputs differ from the halo kernel, first at {np.argwhere(diff)[0]}"
         # and against float64 (the tolerance of test_gpu_conv_pingpong)
         x64 = x[:1].double().permute(0, 3, 1, 2)
@@ -111,7 +77,7 @@ def test_plans_route_only_the_output_conv(ctx, switch):
     keep their halo plans."""
     from livetalking_b200.ops import DevTensor
     g = torch.Generator().manual_seed(53)
-    _, _, cw, temps = _weights(ctx, g)
+    _, _, cw, temps = weights(ctx, g, 80, 32)
     N, S = 16, 256
     cat7 = ctx.alloc((N, S, S, 80))
     h = ctx.alloc((N, S, S, 32))

@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
+from conv_cases import bits, ctx, slice_buf
 
 pytestmark = pytest.mark.gpu
 
@@ -34,28 +35,6 @@ CASES = {
 }
 # ConvTranspose2d(k3, s2, p1, op1) sub-pixel packing (conv_plan.cu kTk / kTn): phase (a, b) reads kernel rows kTk[a][:kTn[a]]
 KTK, KTN = ((1, 0), (2, 0)), (1, 2)
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from livetalking_b200 import engine
-    from livetalking_b200.ops import Ctx
-    engine.set_device(0)
-    c = Ctx()
-    yield c
-    c.close()
-
-
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint16)
-
-
-def _slice(ctx, dense, pitch, off, fill):
-    from livetalking_b200.ops import DevTensor
-    buf = np.full(dense.shape[:-1] + (pitch,), fill, np.float16)
-    buf[..., off:off + dense.shape[-1]] = dense
-    t = ctx.upload(buf)
-    return DevTensor(t.ptr, dense.shape, pitch=pitch, c_off=off), t, buf
 
 
 def _pack(w, transposed):
@@ -93,9 +72,9 @@ def _launch(ctx, P, B, smallmap=True, plan_only=False, slices=True):
     ic = (cin + 64, 32) if slices else (cin, 0)
     oc = (cout + 128, 64) if slices else (cout, 0)
     rc = (cout + 32, 16) if slices else (cout, 0)
-    xv, xt, xbuf = _slice(ctx, P["x"].numpy(), ic[0], ic[1], 512.0)
-    ov, ot, obuf = _slice(ctx, np.full((B, P["OH"], P["OH"], cout), SENT, np.float16), oc[0], oc[1], SENT)
-    rv = _slice(ctx, P["r"].numpy(), rc[0], rc[1], 512.0)[0] if P["r"] is not None else None
+    xv, xt, xbuf = slice_buf(ctx, P["x"].numpy(), ic[0], ic[1], 512.0)
+    ov, ot, obuf = slice_buf(ctx, np.full((B, P["OH"], P["OH"], cout), SENT, np.float16), oc[0], oc[1], SENT)
+    rv = slice_buf(ctx, P["r"].numpy(), rc[0], rc[1], 512.0)[0] if P["r"] is not None else None
     k = P["k"]
     wt = SimpleNamespace(w=ctx.upload(_pack(P["w"].float(), P["tr"])), w_tap=None, bias=ctx.upload(P["b"].float().numpy()),
                          cin=cin, cout=cout, kh=k, kw=k, ktot=k * k * cin)
@@ -107,8 +86,8 @@ def _launch(ctx, P, B, smallmap=True, plan_only=False, slices=True):
     full = ctx.download(ot)
     outside = np.ones(obuf.shape, bool)
     outside[..., oc[1]:oc[1] + cout] = False
-    assert np.array_equal(_bits(full)[outside], _bits(obuf)[outside]), "the conv wrote outside its output slice"
-    assert np.array_equal(_bits(ctx.download(xt)), _bits(xbuf)), "the conv changed its input buffer"
+    assert np.array_equal(bits(full)[outside], bits(obuf)[outside]), "the conv wrote outside its output slice"
+    assert np.array_equal(bits(ctx.download(xt)), bits(xbuf)), "the conv changed its input buffer"
     return full[..., oc[1]:oc[1] + cout]
 
 
@@ -145,7 +124,7 @@ def test_two_launches_bit_identical(ctx, name):
     P = _problem(name, 16, seed=7)
     a = _launch(ctx, P, 16)
     b = _launch(ctx, P, 16)
-    assert np.array_equal(_bits(a), _bits(b))
+    assert np.array_equal(bits(a), bits(b))
 
 
 def test_routing_is_opt_in(ctx):
