@@ -296,20 +296,17 @@ int ltb_op_head_sigmoid255_grouped(ltb_ctx* c, const void* x, const float* w3x32
  * explicit_idx (>= 0) or mirror_index(nf, index + j).  Bit-exact with OpenCV. */
 int ltb_op_ul_paste(ltb_ctx* c, const void* frames, const void* faces, const void* coords, const float* pred, void* out, int nf, int H, int W,
                     int index, int explicit_idx, int slot0, int count);
-/* Audio2Feature.get_hubert_from_16k_speech front end, avatars/ultralight/audio2feature.py:14-20: Wav2Vec2 processor normalisation
- * (stats[2] = mean, 1/sqrt(var + 1e-7)) fused with HubertModel's conv layer 0 (w fp32 [C][10], stride 5) -> fp16 [(n-10)/5+1][C] */
-int ltb_op_hubert_conv0(ltb_ctx* c, const float* pcm, int n, const float* w, const float* bias, int C, float* stats, void* out);
-/* HubertPositionalConvEmbedding + residual: out = h + gelu(conv1d(h, k 128, pad 64, groups)[:T]); w fp16 [D][128][D/groups] */
-int ltb_op_hubert_pos_conv(ltb_ctx* c, const void* h, int T, int D, int groups, int K, const void* w, const float* bias, void* out);
-/* trim / pad to T rows (audio2feature.py:50-55) + BaseASR._feature2chunks (avatars/audio_features/base_asr.py:91-157) as
- * HubertASR.run_step calls it (hubert.py:42-45): out_f32 [B][R][D] and / or out_nhwc fp16 [B][D][R] */
-int ltb_op_hubert_slice(ltb_ctx* c, const void* hidden, int Tc, int T, int D, int B, int R, float start, float mult, int win_l, float* out_f32,
-                        void* out_nhwc);
-/* The three HuBERT ops above over G windows stacked on the row dimension (cross-session batching: one encoder forward for G sessions).
- * pcm f32 [G][n], stats [G][4] (each window normalised with its own mean / variance), conv0 out [G][(n-10)/5+1][C]; pos_conv h / out
- * [G][T][D], zero padding per window; slice hidden [G][Tc][D] -> out_f32 [G][B][R][D] / out_nhwc [G][B][D][R].  G = 1 is the op above. */
+/* The HuBERT ops run over G >= 1 windows stacked on the row dimension (cross-session batching: one encoder forward for G sessions);
+ * every window is computed as if it were alone.
+ * conv0: Audio2Feature.get_hubert_from_16k_speech front end, avatars/ultralight/audio2feature.py:14-20: Wav2Vec2 processor normalisation
+ * (stats[g][2] = mean, 1/sqrt(var + 1e-7) of window g) fused with HubertModel's conv layer 0 (w fp32 [C][10], stride 5):
+ * pcm f32 [G][n] -> fp16 [G][(n-10)/5+1][C] */
 int ltb_op_hubert_conv0_grouped(ltb_ctx* c, const float* pcm, int G, int n, const float* w, const float* bias, int C, float* stats, void* out);
+/* HubertPositionalConvEmbedding + residual: out = h + gelu(conv1d(h, k 128, pad 64, groups)[:T]); w fp16 [D][128][D/groups];
+ * h / out [G][T][D], zero padding per window */
 int ltb_op_hubert_pos_conv_grouped(ltb_ctx* c, const void* h, int G, int T, int D, int groups, int K, const void* w, const float* bias, void* out);
+/* trim / pad to T rows (audio2feature.py:50-55) + BaseASR._feature2chunks (avatars/audio_features/base_asr.py:91-157) as
+ * HubertASR.run_step calls it (hubert.py:42-45): hidden [G][Tc][D] -> out_f32 [G][B][R][D] and / or out_nhwc fp16 [G][B][D][R] */
 int ltb_op_hubert_slice_grouped(ltb_ctx* c, const void* hidden, int G, int Tc, int T, int D, int B, int R, float start, float mult, int win_l,
                                 float* out_f32, void* out_nhwc);
 /* VAE.decode_latents post-processing, avatars/musetalk/models/vae.py:104-107 -> uint8 BGR NHWC */
@@ -326,19 +323,14 @@ int ltb_op_stamp_pixels(ltb_ctx* c, void* frames_u8, int N, int H, int W, const 
 int ltb_op_vae_pre(ltb_ctx* c, const void* img_u8, int N, int H, int W, int half_mask, void* out);
 /* out[i] = table[mirror_index(n, *d_index + i)], i < B  (latent gather of MuseReal.inference_batch, musetalk_avatar.py:134-139) */
 int ltb_op_gather_rows(ltb_ctx* c, const void* table, int n, const void* d_index, int B, long long row_elems, void* out);
-/* transformers.WhisperFeatureExtractor as used by Audio2Feature.audio2feat (avatars/musetalk/whisper/audio2feature.py:106-111):
- * float32 PCM [n <= 480000] -> log-mel features; out_f16 = fp16 [3000][80] (conv1 input), out_f32 (optional) = float [80][3000].
- * fb_f32: the 80 x 201 Slaney mel filterbank; logspec_ws: >= 80*3000 floats; gmax_ws: one int. */
-int ltb_op_whisper_logmel(ltb_ctx* c, const void* pcm_f32, int n, const void* fb_f32, void* logspec_ws, void* gmax_ws, void* out_f16,
-                          void* out_f32);
-/* WhisperASR._feature2chunks / BaseASR._get_sliced_feature (avatars/audio_features/whisper.py:35-56, base_asr.py:91-133):
- * frame i <- encoder steps int((i+start)*mult) + 0..9 (clamped) of the 5 hidden states -> out[i][50 rows][D]. */
-int ltb_op_whisper_slice(ltb_ctx* c, const void* const* hidden5, int T, int D, int B, float start, float mult, void* out,
-                         int out_rows_per_frame);
-/* The two Whisper ops above over G windows (cross-session batching: one encoder forward for G sessions).  logmel: pcm_f32 [G][n],
- * logspec_ws >= G*80*3000 floats, gmax_ws [G] ints (each window clamped to its own maximum), out_f16 [G][3000][80], out_f32 [G][80][3000];
- * window g is what ltb_op_whisper_logmel computes for it alone.  slice: each hidden state is [G*T][D], window g reads rows
- * [g*T, (g+1)*T) -> out[G][B][out_rows_per_frame][D].  G = 1 is the op above. */
+/* The Whisper ops run over G >= 1 windows (cross-session batching: one encoder forward for G sessions); every window is computed
+ * as if it were alone.
+ * logmel: transformers.WhisperFeatureExtractor as used by Audio2Feature.audio2feat (avatars/musetalk/whisper/audio2feature.py:106-111):
+ * float32 PCM [G][n <= 480000] -> log-mel features; out_f16 = fp16 [G][3000][80] (conv1 input), out_f32 (optional) = float [G][80][3000].
+ * fb_f32: the 80 x 201 Slaney mel filterbank; logspec_ws: >= G*80*3000 floats; gmax_ws: G ints (each window clamped to its own maximum).
+ * slice: WhisperASR._feature2chunks / BaseASR._get_sliced_feature (avatars/audio_features/whisper.py:35-56, base_asr.py:91-133):
+ * each hidden state is [G*T][D]; frame i of window g <- steps int((i+start)*mult) + 0..9 (clamped) of rows [g*T, (g+1)*T) of the 5
+ * hidden states -> out[G][B][out_rows_per_frame][D], 50 rows written per frame. */
 int ltb_op_whisper_logmel_grouped(ltb_ctx* c, const void* pcm_f32, int G, int n, const void* fb_f32, void* logspec_ws, void* gmax_ws,
                                   void* out_f16, void* out_f32);
 int ltb_op_whisper_slice_grouped(ltb_ctx* c, const void* const* hidden5, int G, int T, int D, int B, float start, float mult, void* out,

@@ -457,9 +457,6 @@ int ltb_op_hubert_conv0_grouped(ltb_ctx* c, const float* pcm, int G, int n, cons
   c->launches += 2;
   return 0;
 }
-int ltb_op_hubert_conv0(ltb_ctx* c, const float* pcm, int n, const float* w, const float* bias, int C, float* stats, void* out) {
-  return ltb_op_hubert_conv0_grouped(c, pcm, 1, n, w, bias, C, stats, out);
-}
 int ltb_op_hubert_pos_conv_grouped(ltb_ctx* c, const void* h, int G, int T, int D, int groups, int K, const void* w, const float* bias, void* out) {
   if (!c || !h || !w || !bias || !out) return LTB_FAIL("hubert_pos_conv: null argument");
   LTB_CTX_ENTER(c);
@@ -470,9 +467,6 @@ int ltb_op_hubert_pos_conv_grouped(ltb_ctx* c, const void* h, int G, int T, int 
   c->launches += 1;
   return 0;
 }
-int ltb_op_hubert_pos_conv(ltb_ctx* c, const void* h, int T, int D, int groups, int K, const void* w, const float* bias, void* out) {
-  return ltb_op_hubert_pos_conv_grouped(c, h, 1, T, D, groups, K, w, bias, out);
-}
 int ltb_op_hubert_slice_grouped(ltb_ctx* c, const void* hidden, int G, int Tc, int T, int D, int B, int R, float start, float mult, int win_l,
                                 float* out_f32, void* out_nhwc) {
   if (!c || !hidden || (!out_f32 && !out_nhwc)) return LTB_FAIL("hubert_slice: null argument");
@@ -482,10 +476,6 @@ int ltb_op_hubert_slice_grouped(ltb_ctx* c, const void* hidden, int G, int Tc, i
   if (e != cudaSuccess) return LTB_FAIL(std::string("hubert_slice: ") + cudaGetErrorString(e));
   c->launches += 1;
   return 0;
-}
-int ltb_op_hubert_slice(ltb_ctx* c, const void* hidden, int Tc, int T, int D, int B, int R, float start, float mult, int win_l, float* out_f32,
-                        void* out_nhwc) {
-  return ltb_op_hubert_slice_grouped(c, hidden, 1, Tc, T, D, B, R, start, mult, win_l, out_f32, out_nhwc);
 }
 int ltb_op_vae_post(ltb_ctx* c, const void* x, long long npix, int Ctot, void* out_u8) {
   if (!c || !x || !out_u8) return LTB_FAIL("vae_post: null argument");
@@ -670,10 +660,6 @@ int ltb_op_whisper_logmel_grouped(ltb_ctx* c, const void* pcm_f32, int G, int n,
   c->launches += 3;
   return 0;
 }
-int ltb_op_whisper_logmel(ltb_ctx* c, const void* pcm_f32, int n, const void* fb_f32, void* logspec_ws, void* gmax_ws, void* out_f16,
-                          void* out_f32) {
-  return ltb_op_whisper_logmel_grouped(c, pcm_f32, 1, n, fb_f32, logspec_ws, gmax_ws, out_f16, out_f32);
-}
 int ltb_op_whisper_slice_grouped(ltb_ctx* c, const void* const* hidden5, int G, int T, int D, int B, float start, float mult, void* out,
                                  int out_rows_per_frame) {
   if (!c || !hidden5 || !out) return LTB_FAIL("whisper_slice: null argument");
@@ -684,10 +670,6 @@ int ltb_op_whisper_slice_grouped(ltb_ctx* c, const void* const* hidden5, int G, 
   if (e != cudaSuccess) return LTB_FAIL(std::string("whisper_slice (T >= 1, 1 <= B, G <= 65535): ") + cudaGetErrorString(e));
   c->launches += 1;
   return 0;
-}
-int ltb_op_whisper_slice(ltb_ctx* c, const void* const* hidden5, int T, int D, int B, float start, float mult, void* out,
-                         int out_rows_per_frame) {
-  return ltb_op_whisper_slice_grouped(c, hidden5, 1, T, D, B, start, mult, out, out_rows_per_frame);
 }
 int ltb_op_mt_paste(ltb_ctx* c, const ltb_mt_paste_op* d) {
   if (!c || !d) return LTB_FAIL("mt_paste: null argument");

@@ -7,7 +7,8 @@ per-layer LayerNorm and bias, 1024-d stable-LayerNorm transformer, 16-group posi
 projections, attention and MLPs run on the tcgen05 conv / fused-attention kernels; conv layer 0 (+ the processor's utterance
 normalisation), the grouped positional conv and the window gather are csrc/hubert.cu.  One CUDA graph per extractor.
 
-``HubertBatchFeatures`` is the cross-session form: G sessions' windows stacked on the row dimension, one encoder forward for all."""
+``HubertBatchFeatures`` runs G sessions' windows stacked on the row dimension, one encoder forward for all (cross-session mode);
+``HubertFeatures`` is its one-window form, one session's own extractor."""
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence
@@ -92,15 +93,11 @@ class HubertEncoder:
         self.ln_post = _Norm(ctx, sd, "encoder.layer_norm")
         ctx.sync()
 
-    def emit(self, b: Builder, pcm: DevTensor, n: int, stats: DevTensor) -> DevTensor:
-        """pcm: float32 [n] raw 16 kHz samples -> last_hidden_state (conv_frames(n), D) fp16 (HubertModel.forward on the
-        processor-normalised input; stable-LayerNorm encoder: hidden += pos_conv(hidden); pre-LN layers; final LayerNorm)."""
-        return self.emit_grouped(b, pcm, 1, n, stats)
-
-    def emit_grouped(self, b: Builder, pcm: DevTensor, G: int, n: int, stats: DevTensor) -> DevTensor:
-        """emit() for G windows at once: pcm float32 [G][n], stats [G][4] -> (G * conv_frames(n), D) fp16, window g in rows
-        [g*T, (g+1)*T).  Each window is normalised with its own statistics, the conv stack runs with N = G images, row-wise ops
-        run over G*T rows and attention with batch G, so no window sees another's samples or keys."""
+    def emit(self, b: Builder, pcm: DevTensor, n: int, stats: DevTensor, G: int = 1) -> DevTensor:
+        """pcm: float32 [G][n] raw 16 kHz samples of G windows, stats [G][4] -> last_hidden_state (G * conv_frames(n), D) fp16, window g
+        in rows [g*T, (g+1)*T) (HubertModel.forward on the processor-normalised input; stable-LayerNorm encoder: hidden +=
+        pos_conv(hidden); pre-LN layers; final LayerNorm).  Each window is normalised with its own statistics, the conv stack runs
+        with N = G images, row-wise ops run over G*T rows and attention with batch G, so no window sees another's samples or keys."""
         ctx, C, D = b.ctx, self.C, self.D
         T = (n - CONV_KERNEL[0]) // CONV_STRIDE[0] + 1
         h = b.new(G, 1, T, C)
@@ -141,62 +138,19 @@ def window_samples(batch: int, stride_left: int, stride_right: int) -> tuple:
     return n, Tc, T
 
 
-class HubertFeatures(GraphSession):
-    """get_hubert_from_16k_speech + HubertASR's window gather for one session: PCM buffer -> (B, 16, D) features, one CUDA graph.
-    The window is (stride_left + stride_right + 2 * batch) 20 ms chunks (HubertASR keeps exactly that many, hubert.py:30-48)."""
-
-    def __init__(self, enc: HubertEncoder, batch: int, stride_left: int = 10, stride_right: int = 10, out_nhwc: Optional[DevTensor] = None,
-                 ctx: Optional[Ctx] = None):
-        super().__init__(ctx)
-        self.enc, self.B = enc, int(batch)
-        try:
-            ctx = self.ctx
-            self.n, self.Tc, self.T = window_samples(self.B, stride_left, stride_right)
-            self.pcm = self.alloc((self.n,), np.float32, zero=True)
-            self.stats = self.alloc((4,), np.float32, zero=True)
-            self.out = self.alloc((self.B, ROWS, enc.D), np.float32, zero=True)
-            self.out_nhwc = out_nhwc
-            self.start = stride_left / 2.0
-
-            def emit(b: Builder):
-                self.hidden = enc.emit(b, self.pcm, self.n, self.stats)
-                ctx.hubert_slice(self.hidden, self.Tc, self.T, enc.D, self.B, ROWS, self.start, 2.0, WIN[0], self.out, self.out_nhwc)
-
-            self.capture(emit)
-        except BaseException:
-            self.close()
-            raise
-
-    def run_async(self, pcm: Optional[np.ndarray] = None):
-        if pcm is not None:
-            pcm = np.ascontiguousarray(pcm, np.float32).reshape(-1)
-            if pcm.size != self.n:
-                raise ValueError(f"expected {self.n} samples, got {pcm.size}")
-            self.ctx.h2d(self.pcm, pcm, sync=False)
-        self.graph.launch()
-
-    def run(self, pcm: np.ndarray) -> np.ndarray:
-        """-> (B, 16, D) float32: the list HubertASR.run_step queues (stacked)."""
-        with self.ctx.lock:
-            self.run_async(pcm)
-            return self.ctx.download(self.out)
-
-    def hidden_states(self) -> np.ndarray:
-        with self.ctx.lock:
-            return self.ctx.download(self.hidden)
-
-
 class HubertBatchFeatures(GraphSession):
-    """HubertFeatures for up to G sessions at once: G PCM windows of the same layout -> G x (B, 16, D) features, ONE CUDA graph of
-    one encoder forward over the G windows stacked on the row dimension (HubertEncoder.emit_grouped).  At B = 16 a window is ~51
-    tokens, under half of one 128-row GEMM tile, and every window re-reads the encoder's weights: G windows per forward share
+    """get_hubert_from_16k_speech + HubertASR's window gather for up to G sessions at once: G PCM windows of the same layout -> G x
+    (B, 16, D) features, ONE CUDA graph of one encoder forward over the G windows stacked on the row dimension.  The window is
+    (stride_left + stride_right + 2 * batch) 20 ms chunks (HubertASR keeps exactly that many, hubert.py:30-48).  At B = 16 a window
+    is ~51 tokens, under half of one 128-row GEMM tile, and every window re-reads the encoder's weights: G windows per forward share
     both.  Each window keeps its own normalisation statistics, positional-conv padding and attention keys, so a session's features do
     not depend on which other windows share its round.  A call with k < G windows is a partial round: groups [k, G) keep their
-    last window (zeros before the first call) and their output is not read.  `batch` / `infer_slots` make it a mux for
-    plugin.batcher.CrossSessionBatcher (a request is one session's PCM window)."""
+    last window (zeros before the first call) and their output is not read.  out_nhwc (optional): fp16 [G][B][D][16], written
+    besides the float32 features.  `batch` / `infer_slots` make it a mux for plugin.batcher.CrossSessionBatcher (a request is one
+    session's PCM window)."""
 
-    def __init__(self, enc: HubertEncoder, batch: int, groups: int, stride_left: int = 10, stride_right: int = 10,
-                 ctx: Optional[Ctx] = None):
+    def __init__(self, enc: HubertEncoder, batch: int, groups: int, stride_left: int = 10, stride_right: int = 10, *,
+                 out_nhwc: Optional[DevTensor] = None, ctx: Optional[Ctx] = None):
         self.enc, self.B, self.G = enc, int(batch), int(groups)
         if self.G < 1:
             raise ValueError("groups must be >= 1")
@@ -208,19 +162,21 @@ class HubertBatchFeatures(GraphSession):
             self.pcm = self.alloc((self.G, self.n), np.float32, zero=True)
             self.stats = self.alloc((self.G, 4), np.float32, zero=True)
             self.out = self.alloc((self.G, self.B, ROWS, enc.D), np.float32, zero=True)
+            self.out_nhwc = out_nhwc
             self.start = stride_left / 2.0
 
             def emit(b: Builder):
-                self.hidden = enc.emit_grouped(b, self.pcm, self.G, self.n, self.stats)
-                ctx.hubert_slice(self.hidden, self.Tc, self.T, enc.D, self.B, ROWS, self.start, 2.0, WIN[0], self.out, None, G=self.G)
+                self.hidden = enc.emit(b, self.pcm, self.n, self.stats, G=self.G)
+                ctx.hubert_slice(self.hidden, self.Tc, self.T, enc.D, self.B, ROWS, self.start, 2.0, WIN[0], self.out, self.out_nhwc,
+                                 G=self.G)
 
             self.capture(emit)
         except BaseException:
             self.close()
             raise
 
-    def run_async(self, pcms: Sequence[np.ndarray]) -> int:
-        """Stage windows 0 .. k-1 and launch the graph; -> k."""
+    def _stage(self, pcms: Sequence[np.ndarray]) -> int:
+        """Copy windows 0 .. k-1 to the device; -> k."""
         k = len(pcms)
         if not 1 <= k <= self.G:
             raise ValueError(f"1..{self.G} windows per call, got {k}")
@@ -228,17 +184,46 @@ class HubertBatchFeatures(GraphSession):
         if x.shape[1] != self.n:
             raise ValueError(f"expected windows of {self.n} samples, got {x.shape[1]}")
         self.ctx.h2d(DevTensor(self.pcm.ptr, (k, self.n), np.float32), x, sync=False)
+        return k
+
+    def run_async(self, pcms: Sequence[np.ndarray]) -> int:
+        """Stage windows 0 .. k-1 and launch the graph; -> k."""
+        k = self._stage(pcms)
         self.graph.launch()
         return k
 
     def run_groups(self, pcms: Sequence[np.ndarray]) -> List[np.ndarray]:
-        """-> per window its (B, 16, D) float32 features: what HubertFeatures.run returns for that window alone."""
+        """-> per window its (B, 16, D) float32 features: the list HubertASR.run_step queues (stacked) for that window alone."""
         with self.ctx.lock:
-            k = self.run_async(pcms)
+            k = self._stage(pcms)
+            self.graph.launch()
             out = self.ctx.download(DevTensor(self.out.ptr, (k, self.B, ROWS, self.enc.D), np.float32))
         return [out[g] for g in range(k)]
 
     infer_slots = run_groups
+
+    def hidden_states(self) -> np.ndarray:
+        """-> the encoder's last hidden state (G * Tc, D) fp16 of the last launch."""
+        with self.ctx.lock:
+            return self.ctx.download(self.hidden)
+
+
+class HubertFeatures(HubertBatchFeatures):
+    """HubertBatchFeatures for one session (G = 1): PCM buffer -> (B, 16, D) features, one CUDA graph."""
+
+    def __init__(self, enc: HubertEncoder, batch: int, stride_left: int = 10, stride_right: int = 10, out_nhwc: Optional[DevTensor] = None,
+                 ctx: Optional[Ctx] = None):
+        super().__init__(enc, batch, 1, stride_left, stride_right, out_nhwc=out_nhwc, ctx=ctx)
+
+    def run_async(self, pcm: Optional[np.ndarray] = None):
+        """Stage `pcm` (None: keep the last window) and launch the graph."""
+        if pcm is not None:
+            self._stage([pcm])
+        self.graph.launch()
+
+    def run(self, pcm: np.ndarray) -> np.ndarray:
+        """-> (B, 16, D) float32: the list HubertASR.run_step queues (stacked)."""
+        return self.run_groups([pcm])[0]
 
 
 def gflop_per_window(n_samples: int, layers: int = 24, d_model: int = 1024, ffn: int = 4096, conv_dim: int = 512) -> float:

@@ -13,6 +13,7 @@ never held back for longer than that.  Requests of one ``submit`` call keep thei
 than the necessary number of batches."""
 from __future__ import annotations
 
+import os
 import threading
 import time
 from collections import deque
@@ -109,6 +110,23 @@ class CrossSessionBatcher:
             t.error = RuntimeError("CrossSessionBatcher closed")
             t.done.set()
         self._thread.join(timeout=5)
+
+
+_SHARED_LOCK = threading.Lock()
+
+
+def shared_scheduler(owner, table_attr: str, key, make_mux) -> CrossSessionBatcher:
+    """The CrossSessionBatcher of `key` in the table ``owner.<table_attr>``, created by the first session that asks and shared by all
+    later ones.  make_mux() builds its engine mux; its dispatch deadline is LTB_MUX_WAIT_MS (default 4 ms).  The owner is the model
+    whose weights the mux runs, so its schedulers live as long as it does."""
+    with _SHARED_LOCK:
+        table = getattr(owner, table_attr, None)
+        if table is None:
+            table = {}
+            setattr(owner, table_attr, table)
+        if key not in table:
+            table[key] = CrossSessionBatcher(make_mux(), float(os.environ.get("LTB_MUX_WAIT_MS", "4")))
+        return table[key]
 
 
 class SharedFeatures:

@@ -24,7 +24,7 @@ from .. import engine
 from ..musetalk import MuseTalkAvatar, MuseTalkBatchSession, MuseTalkModel, MuseTalkSession
 from ..ops import Ctx
 from ..whisper import WhisperBatchFeatures, WhisperEncoder, WhisperFeatures
-from .batcher import CrossSessionBatcher, SharedFeatures
+from .batcher import CrossSessionBatcher, SharedFeatures, shared_scheduler
 from .whisper_asr import WhisperASR
 
 try:
@@ -110,36 +110,19 @@ def warm_up(batch_size, model):
     logger.info("warmup model... (engine sessions warm up at creation)")
 
 
-_BATCHER_LOCK = __import__("threading").Lock()
-
-
 def shared_batcher(model: EngineModel, lat_hw: int, frames_per_session: int) -> CrossSessionBatcher:
     """Cross-session mode (SURVEY 8(f) rank 1): one scheduler per (model, latent size, session batch size), created by the first
     session that asks.  Its mux is a MuseTalkBatchSession: up to LTB_MT_GROUPS sessions' B frames run as ONE UNet + VAE graph."""
-    with _BATCHER_LOCK:
-        table = getattr(model, "_ltb_batchers", None)
-        if table is None:
-            table = model._ltb_batchers = {}
-        key = (int(lat_hw), int(frames_per_session))
-        if key not in table:
-            mux = MuseTalkBatchSession(model.net, lat_hw, int(os.environ.get("LTB_MT_GROUPS", "4")), frames_per_session)
-            table[key] = CrossSessionBatcher(mux, float(os.environ.get("LTB_MUX_WAIT_MS", "4")))
-        return table[key]
+    return shared_scheduler(model, "_ltb_batchers", (int(lat_hw), int(frames_per_session)),
+                            lambda: MuseTalkBatchSession(model.net, lat_hw, int(os.environ.get("LTB_MT_GROUPS", "4")), frames_per_session))
 
 
 def shared_feature_batcher(model: EngineModel, batch: int, stride_left: int, stride_right: int) -> CrossSessionBatcher:
     """Cross-session mode: one Whisper scheduler per (model, window layout), created by the first session that asks.  Its mux is a
     WhisperBatchFeatures of LTB_MT_GROUPS windows: sessions whose steps fall in the same round share one encoder forward."""
-    with _BATCHER_LOCK:
-        table = getattr(model, "_ltb_feature_batchers", None)
-        if table is None:
-            table = model._ltb_feature_batchers = {}
-        key = (int(batch), int(stride_left), int(stride_right))
-        if key not in table:
-            groups = int(os.environ.get("LTB_MT_GROUPS", "4"))
-            mux = WhisperBatchFeatures(model.whisper, batch, groups, stride_left, stride_right)
-            table[key] = CrossSessionBatcher(mux, float(os.environ.get("LTB_MUX_WAIT_MS", "4")))
-        return table[key]
+    groups = int(os.environ.get("LTB_MT_GROUPS", "4"))
+    return shared_scheduler(model, "_ltb_feature_batchers", (int(batch), int(stride_left), int(stride_right)),
+                            lambda: WhisperBatchFeatures(model.whisper, batch, groups, stride_left, stride_right))
 
 
 @register("avatar", "musetalk")

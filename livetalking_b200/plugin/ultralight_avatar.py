@@ -20,7 +20,6 @@ from __future__ import annotations
 import glob
 import os
 import pickle
-import threading
 
 import numpy as np
 
@@ -28,7 +27,7 @@ from .. import engine
 from ..hubert import HubertBatchFeatures, HubertEncoder, HubertFeatures
 from ..ops import Ctx
 from ..ultralight import FACE, UltraLightAvatar, UltraLightBatchSession, UltraLightModel, UltraLightSession
-from .batcher import CrossSessionBatcher, SharedFeatures
+from .batcher import CrossSessionBatcher, SharedFeatures, shared_scheduler
 from .hubert_asr import HubertASR
 
 try:
@@ -101,38 +100,21 @@ def warm_up(batch_size, avatar, modelres):
     logger.info("warmup model... (engine sessions warm up at creation)")
 
 
-_BATCHER_LOCK = threading.Lock()
-
-
 def shared_batcher(audio: EngineAudio, template: UltraLightModel, frames_per_session: int, return_pred: bool) -> CrossSessionBatcher:
     """Cross-session mode: one scheduler per (HuBERT model, session batch size), created by the first session that asks.  Its mux is
     an UltraLightBatchSession of LTB_UL_GROUPS groups whose graph takes its shapes from `template` (every UltraLight network has the
     same layout) and whose bank holds 2 x groups avatar networks."""
-    with _BATCHER_LOCK:
-        table = getattr(audio, "_ltb_batchers", None)
-        if table is None:
-            table = audio._ltb_batchers = {}
-        key = (int(frames_per_session), bool(return_pred))
-        if key not in table:
-            groups = int(os.environ.get("LTB_UL_GROUPS", "4"))
-            mux = UltraLightBatchSession(template, groups, frames_per_session, slots=2 * groups, return_pred=return_pred)
-            table[key] = CrossSessionBatcher(mux, float(os.environ.get("LTB_MUX_WAIT_MS", "4")))
-        return table[key]
+    groups = int(os.environ.get("LTB_UL_GROUPS", "4"))
+    return shared_scheduler(audio, "_ltb_batchers", (int(frames_per_session), bool(return_pred)),
+                            lambda: UltraLightBatchSession(template, groups, frames_per_session, slots=2 * groups, return_pred=return_pred))
 
 
 def shared_feature_batcher(audio: EngineAudio, batch: int, stride_left: int, stride_right: int) -> CrossSessionBatcher:
     """Cross-session mode: one HuBERT scheduler per (HuBERT model, window layout), created by the first session that asks.  Its mux
     is a HubertBatchFeatures of LTB_UL_GROUPS windows: sessions whose steps fall in the same round share one encoder forward."""
-    with _BATCHER_LOCK:
-        table = getattr(audio, "_ltb_feature_batchers", None)
-        if table is None:
-            table = audio._ltb_feature_batchers = {}
-        key = (int(batch), int(stride_left), int(stride_right))
-        if key not in table:
-            groups = int(os.environ.get("LTB_UL_GROUPS", "4"))
-            mux = HubertBatchFeatures(audio.encoder, batch, groups, stride_left, stride_right)
-            table[key] = CrossSessionBatcher(mux, float(os.environ.get("LTB_MUX_WAIT_MS", "4")))
-        return table[key]
+    groups = int(os.environ.get("LTB_UL_GROUPS", "4"))
+    return shared_scheduler(audio, "_ltb_feature_batchers", (int(batch), int(stride_left), int(stride_right)),
+                            lambda: HubertBatchFeatures(audio.encoder, batch, groups, stride_left, stride_right))
 
 
 @register("avatar", "ultralight")

@@ -26,7 +26,7 @@ import pickle
 import numpy as np
 
 from .. import avatar_pack, engine
-from .batcher import CrossSessionBatcher
+from .batcher import CrossSessionBatcher, shared_scheduler
 from .mel_asr import MelASR
 
 try:
@@ -88,20 +88,10 @@ def warm_up(batch_size, model, modelres):
     logger.info("warmup model... (engine sessions warm up at creation)")
 
 
-_BATCHER_LOCK = __import__("threading").Lock()
-
-
 def shared_batcher(model, eng_avatar) -> CrossSessionBatcher:
     """One scheduler per (model, frame size): created by the first session that asks, shared by all later ones."""
-    with _BATCHER_LOCK:
-        table = getattr(model, "_ltb_batchers", None)
-        if table is None:
-            table = model._ltb_batchers = {}
-        key = (eng_avatar.H, eng_avatar.W)
-        if key not in table:
-            mux = engine.W2LSession(model, eng_avatar, int(os.environ.get("LTB_MUX_BATCH", "16")), slots=True)
-            table[key] = CrossSessionBatcher(mux, float(os.environ.get("LTB_MUX_WAIT_MS", "4")))
-        return table[key]
+    return shared_scheduler(model, "_ltb_batchers", (eng_avatar.H, eng_avatar.W),
+                            lambda: engine.W2LSession(model, eng_avatar, int(os.environ.get("LTB_MUX_BATCH", "16")), slots=True))
 
 
 @register("avatar", "wav2lip")

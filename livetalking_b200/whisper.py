@@ -6,7 +6,8 @@ Weights come from the HF ``WhisperModel`` state_dict (``encoder.*`` keys).  The 
 layers over 1500 steps) is assembled from the same engine ops as the UNet and captured into one CUDA graph together with
 the log-mel kernels and the per-frame (50, 384) slicing.
 
-``WhisperBatchFeatures`` is the cross-session form: G sessions' windows stacked on the row dimension, one encoder forward for all."""
+``WhisperBatchFeatures`` runs G sessions' windows stacked on the row dimension, one encoder forward for all (cross-session mode);
+``WhisperFeatures`` is its one-window form, one session's own extractor."""
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence
@@ -72,15 +73,11 @@ class WhisperEncoder:
         self.fb = ctx.upload(slaney_mel_filterbank())
         ctx.sync()
 
-    def emit(self, b: Builder, feats16: DevTensor):
-        """feats16: fp16 (3000, 80) log-mel features -> the 5 hidden states HF returns, each (1500, D) fp16.
+    def emit(self, b: Builder, feats16: DevTensor, G: int = 1):
+        """feats16: fp16 (G, 3000, 80) log-mel features of G windows -> the 5 hidden states HF returns, each (G * 1500, D) fp16, window
+        g in rows [g*1500, (g+1)*1500).  The convs run with N = G images of 1 x 3000 (each zero-padded on its own), the positional add
+        repeats per window, row-wise ops run over G*1500 rows and attention with batch G, so no op mixes rows of different windows.
         Ops are enqueued on the builder's ctx (the session's own stream); the weights live in self.ctx (read-only)."""
-        return self.emit_grouped(b, feats16, 1)
-
-    def emit_grouped(self, b: Builder, feats16: DevTensor, G: int):
-        """emit() for G windows at once: feats16 fp16 (G, 3000, 80) -> 5 hidden states of (G * 1500, D), window g in rows
-        [g*1500, (g+1)*1500).  The convs run with N = G images of 1 x 3000 (each zero-padded on its own), the positional add repeats
-        per window, row-wise ops run over G*1500 rows and attention with batch G, so no op mixes rows of different windows."""
         ctx, D = b.ctx, self.D
         T = N_FRAMES
         x = DevTensor(feats16.ptr, (G, 1, T, N_MELS))
@@ -104,66 +101,23 @@ class WhisperEncoder:
         return hidden
 
 
-class WhisperFeatures(GraphSession):
-    """audio2feat + WhisperASR slicing for one session: PCM buffer -> (B, 50, D) features, one CUDA graph."""
-
-    def __init__(self, enc: WhisperEncoder, batch: int, stride_left: int = 10, stride_right: int = 10, out: Optional[DevTensor] = None,
-                 out_rows: int = 50, keep_hidden: bool = False, ctx: Optional[Ctx] = None):
-        """ctx: this extractor's own stream + scratch (created here unless given): WhisperASR.run_step runs on the render
-        thread concurrently with inference_batch on the inference thread (avatars/base_avatar.py:483-489 vs :366)."""
-        self.enc, self.B = enc, int(batch)
-        self.n = (stride_left + stride_right + 2 * self.B) * 320
-        if self.n > N_SAMPLES:
-            raise ValueError("audio window longer than 30 s")
-        super().__init__(ctx)
-        try:
-            ctx = self.ctx
-            self.pcm = self.alloc((self.n,), np.float32, zero=True)
-            self.logspec = self.alloc((N_MELS * N_FRAMES,), np.float32, zero=True)
-            self.gmax = self.alloc((4,), np.int32, zero=True)
-            self.feats16 = self.alloc((N_FRAMES, N_MELS), np.float16, zero=True)
-            self.feats32 = self.alloc((N_MELS, N_FRAMES), np.float32, zero=True) if keep_hidden else None
-            self.out_rows = out_rows
-            self.out = out if out is not None else self.alloc((self.B, out_rows, enc.D), np.float16, zero=True)
-            self.start = stride_left / 2.0
-
-            def emit(b: Builder):
-                ctx.whisper_logmel(self.pcm, self.n, enc.fb, self.logspec, self.gmax, self.feats16, self.feats32)
-                self.hidden = enc.emit(b, self.feats16)
-                ctx.whisper_slice(self.hidden, N_FRAMES // 2, enc.D, self.B, self.start, 2.0, self.out, self.out_rows)
-
-            self.capture(emit)
-        except BaseException:
-            self.close()
-            raise
-
-    def run_async(self, pcm: Optional[np.ndarray] = None):
-        if pcm is not None:
-            pcm = np.ascontiguousarray(pcm, np.float32).reshape(-1)
-            if pcm.size != self.n:
-                raise ValueError(f"expected {self.n} samples, got {pcm.size}")
-            self.ctx.h2d(self.pcm, pcm, sync=False)
-        self.graph.launch()
-
-    def run(self, pcm: np.ndarray) -> np.ndarray:
-        """-> (B, 50, D) float16, the list WhisperASR.run_step queues (stacked)."""
-        with self.ctx.lock:
-            self.run_async(pcm)
-            full = self.ctx.download(self.out)
-        return full[:, :50]
-
-
 class WhisperBatchFeatures(GraphSession):
-    """WhisperFeatures for up to G sessions at once: G PCM windows of the same layout -> G x (B, 50, D) features, ONE CUDA graph
-    (grouped log-mel, one encoder forward over the G windows stacked on the row dimension, grouped slice).  The encoder always
-    runs over the 30-s padded window (1500 tokens), whatever B, so at small B each session's forward is mostly fixed cost: G
-    windows per forward share the weights and fill wider GEMMs.  Each window keeps its own log-mel clamp, conv padding and attention
-    keys, so a session's features do not depend on which other windows share its round.  A call with k < G windows is a partial
-    round: groups [k, G) keep their last window (zeros before the first call) and their output is not read.  `batch` /
-    `infer_slots` make it a mux for plugin.batcher.CrossSessionBatcher (a request is one session's PCM window)."""
+    """audio2feat + WhisperASR slicing for up to G sessions at once: G PCM windows of the same layout -> G x (B, 50, D) features, ONE
+    CUDA graph (log-mel, one encoder forward over the G windows stacked on the row dimension, slice).  The encoder always runs over
+    the 30-s padded window (1500 tokens), whatever B, so at small B each session's forward is mostly fixed cost: G windows per forward
+    share the weights and fill wider GEMMs.  Each window keeps its own log-mel clamp, conv padding and attention keys, so a session's
+    features do not depend on which other windows share its round.  A call with k < G windows is a partial round: groups [k, G) keep
+    their last window (zeros before the first call) and their output is not read.  `batch` / `infer_slots` make it a mux for
+    plugin.batcher.CrossSessionBatcher (a request is one session's PCM window).
 
-    def __init__(self, enc: WhisperEncoder, batch: int, groups: int, stride_left: int = 10, stride_right: int = 10,
-                 ctx: Optional[Ctx] = None):
+    out (optional): fp16 [G][B][out_rows][D] the features are written to (50 of every out_rows rows), allocated here unless given.
+    keep_hidden: also keep the float32 log-mel features in feats32, (G * 80, 3000) with window g in rows [g*80, (g+1)*80) like the
+    hidden states (which are in `hidden` either way).
+    ctx: this extractor's own stream + scratch (created here unless given): WhisperASR.run_step runs on the render thread
+    concurrently with inference_batch on the inference thread (avatars/base_avatar.py:483-489 vs :366)."""
+
+    def __init__(self, enc: WhisperEncoder, batch: int, groups: int, stride_left: int = 10, stride_right: int = 10, *,
+                 out: Optional[DevTensor] = None, out_rows: int = 50, keep_hidden: bool = False, ctx: Optional[Ctx] = None):
         self.enc, self.B, self.G = enc, int(batch), int(groups)
         if self.G < 1:
             raise ValueError("groups must be >= 1")
@@ -178,21 +132,23 @@ class WhisperBatchFeatures(GraphSession):
             self.logspec = self.alloc((self.G, N_MELS * N_FRAMES), np.float32, zero=True)
             self.gmax = self.alloc((self.G,), np.int32, zero=True)
             self.feats16 = self.alloc((self.G, N_FRAMES, N_MELS), np.float16, zero=True)
-            self.out = self.alloc((self.G, self.B, 50, enc.D), np.float16, zero=True)
+            self.feats32 = self.alloc((self.G * N_MELS, N_FRAMES), np.float32, zero=True) if keep_hidden else None
+            self.out_rows = out_rows
+            self.out = out if out is not None else self.alloc((self.G, self.B, out_rows, enc.D), np.float16, zero=True)
             self.start = stride_left / 2.0
 
             def emit(b: Builder):
-                ctx.whisper_logmel(self.pcm, self.n, enc.fb, self.logspec, self.gmax, self.feats16, None, G=self.G)
-                self.hidden = enc.emit_grouped(b, self.feats16, self.G)
-                ctx.whisper_slice(self.hidden, N_FRAMES // 2, enc.D, self.B, self.start, 2.0, self.out, 50, G=self.G)
+                ctx.whisper_logmel(self.pcm, self.n, enc.fb, self.logspec, self.gmax, self.feats16, self.feats32, G=self.G)
+                self.hidden = enc.emit(b, self.feats16, G=self.G)
+                ctx.whisper_slice(self.hidden, N_FRAMES // 2, enc.D, self.B, self.start, 2.0, self.out, self.out_rows, G=self.G)
 
             self.capture(emit)
         except BaseException:
             self.close()
             raise
 
-    def run_async(self, pcms: Sequence[np.ndarray]) -> int:
-        """Stage windows 0 .. k-1 and launch the graph; -> k."""
+    def _stage(self, pcms: Sequence[np.ndarray]) -> int:
+        """Copy windows 0 .. k-1 to the device; -> k."""
         k = len(pcms)
         if not 1 <= k <= self.G:
             raise ValueError(f"1..{self.G} windows per call, got {k}")
@@ -200,14 +156,38 @@ class WhisperBatchFeatures(GraphSession):
         if x.shape[1] != self.n:
             raise ValueError(f"expected windows of {self.n} samples, got {x.shape[1]}")
         self.ctx.h2d(DevTensor(self.pcm.ptr, (k, self.n), np.float32), x, sync=False)
+        return k
+
+    def run_async(self, pcms: Sequence[np.ndarray]) -> int:
+        """Stage windows 0 .. k-1 and launch the graph; -> k."""
+        k = self._stage(pcms)
         self.graph.launch()
         return k
 
     def run_groups(self, pcms: Sequence[np.ndarray]) -> List[np.ndarray]:
-        """-> per window its (B, 50, D) float16 features: what WhisperFeatures.run returns for that window alone."""
+        """-> per window its (B, 50, D) float16 features: the list WhisperASR.run_step queues (stacked) for that window alone."""
         with self.ctx.lock:
-            k = self.run_async(pcms)
-            out = self.ctx.download(DevTensor(self.out.ptr, (k, self.B, 50, self.enc.D), np.float16))
-        return [out[g] for g in range(k)]
+            k = self._stage(pcms)
+            self.graph.launch()
+            out = self.ctx.download(DevTensor(self.out.ptr, (k, self.B, self.out_rows, self.enc.D), np.float16))
+        return [out[g, :, :50] for g in range(k)]
 
     infer_slots = run_groups
+
+
+class WhisperFeatures(WhisperBatchFeatures):
+    """WhisperBatchFeatures for one session (G = 1): PCM buffer -> (B, 50, D) features, one CUDA graph."""
+
+    def __init__(self, enc: WhisperEncoder, batch: int, stride_left: int = 10, stride_right: int = 10, out: Optional[DevTensor] = None,
+                 out_rows: int = 50, keep_hidden: bool = False, ctx: Optional[Ctx] = None):
+        super().__init__(enc, batch, 1, stride_left, stride_right, out=out, out_rows=out_rows, keep_hidden=keep_hidden, ctx=ctx)
+
+    def run_async(self, pcm: Optional[np.ndarray] = None):
+        """Stage `pcm` (None: keep the last window) and launch the graph."""
+        if pcm is not None:
+            self._stage([pcm])
+        self.graph.launch()
+
+    def run(self, pcm: np.ndarray) -> np.ndarray:
+        """-> (B, 50, D) float16, the list WhisperASR.run_step queues (stacked)."""
+        return self.run_groups([pcm])[0]

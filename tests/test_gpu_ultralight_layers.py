@@ -709,7 +709,7 @@ def _check_hubert(run, recs, W, G, T):
 
 @pytest.mark.parametrize("run", list(HUBERT_RUNS))
 def test_hubert_every_op_against_float64(hubert, run):
-    """HubertEncoder.emit (G = 1) / emit_grouped (G = 3) over B = 16 windows traced eagerly, every op on every row against float64;
+    """HubertEncoder.emit with G = 1 / G = 3 over B = 16 windows traced eagerly, every op on every row against float64;
     the production graph (HubertFeatures / HubertBatchFeatures) must give the traced hidden states bit for bit."""
     from livetalking_b200.hubert import HubertBatchFeatures, HubertFeatures, window_samples
     from livetalking_b200.graph import Builder
@@ -725,7 +725,7 @@ def test_hubert_every_op_against_float64(hubert, run):
     pcm = ctx.alloc((G, n), np.float32, zero=True)
     stats = ctx.alloc((G, 4), np.float32, zero=True)
     ctx.h2d(pcm, pcms)
-    hidden = enc.emit_grouped(Builder(ctx), pcm, G, n, stats) if G > 1 else enc.emit(Builder(ctx), pcm, n, stats)
+    hidden = enc.emit(Builder(ctx), pcm, n, stats, G=G)
     tr.stop()
     traced = ctx.download(hidden)
     assert not tr.errors, tr.errors[:5]

@@ -1,4 +1,4 @@
-"""GPU: every op of the Whisper-tiny feature path — log-mel, the encoder (WhisperEncoder.emit / emit_grouped) and the per-frame
+"""GPU: every op of the Whisper-tiny feature path — log-mel, the encoder (WhisperEncoder.emit) and the per-frame
 slicing — against float64, each op recomputed from the input the GPU read.
 
 The test drives an eager pass on a fresh Ctx whose op methods are wrapped by `op_trace.OpTrace` (see
@@ -26,7 +26,7 @@ as ConvWeight holds them.  Every op is checked on every row of every window:
     below the clamp floor carries the floor's error (the dlog of the window's maximum + the fp32 rounding of max - 8), any
     other the larger of its own and the floor's; the fp32 add and divide add 2^-23 (|v| + 4) / 4; fp16 adds u |ref| + 2^-25.
 
-Runs: g1_b8 (WhisperEncoder.emit, one window, B = 8 frames) and g4_b2 (emit_grouped over G = 4 windows: a tone, digital silence,
+Runs: g1_b8 (WhisperEncoder.emit, one window, B = 8 frames) and g4_b2 (emit over G = 4 windows: a tone, digital silence,
 a window near full scale with clipped peaks, and a quiet one).  The Whisper path has no float atomics (the only atomic is the
 integer atomicMax of the log-mel maximum), so WhisperFeatures.run / WhisperBatchFeatures.run_groups must reproduce the traced
 features bit for bit."""
@@ -242,7 +242,7 @@ def whisper():
 
 @pytest.mark.parametrize("run", list(RUNS))
 def test_whisper_every_op_against_float64(whisper, run):
-    """log-mel + WhisperEncoder.emit (G = 1) / emit_grouped (G = 4) + whisper_slice traced eagerly, every op on every row against
+    """log-mel + WhisperEncoder.emit (G = 1 / G = 4) + whisper_slice traced eagerly, every op on every row against
     float64; WhisperFeatures / WhisperBatchFeatures must give the traced features bit for bit."""
     from livetalking_b200.graph import Builder
     from livetalking_b200.ops import Ctx
@@ -264,7 +264,7 @@ def test_whisper_every_op_against_float64(whisper, run):
     ctx.h2d(pcm, pcms)
     ctx.whisper_logmel(pcm, n, enc.fb, logspec, gmax, feats16, feats32, G=G)
     b = Builder(ctx)
-    hidden = enc.emit(b, feats16) if G == 1 else enc.emit_grouped(b, feats16, G)
+    hidden = enc.emit(b, feats16, G=G)
     ctx.whisper_slice(hidden, T2, enc.D, B, STRIDE_L / 2.0, 2.0, out, 50, G=G)
     tr.stop()
     traced = ctx.download(out)
