@@ -3,15 +3,18 @@ test_gpu_conv.py never reaches: channel-sliced input / output / residual, asymme
 larger than the taps times Cin with a NULL bias, and the GroupNorm statistics output (fused into the conv epilogue or a separate
 pass) consumed by ltb_op_groupnorm_apply.
 
-References are float64 PyTorch on the same fp16 inputs and fp16-rounded weights.  Conv outputs: |err| <= 2e-2 + 1e-2 |ref| and
-mean < 2e-3 (as test_gpu_conv.py).  Slice neighbours of inputs hold 512 and of outputs a second sentinel; a kernel that reads a
-neighbour channel or writes one fails the comparison or the bit check."""
+References are float64 PyTorch on the same fp16 inputs and fp16 weights.  Conv outputs are held to conv_check.py: the hard error
+bound and the rounding model of the kernel Ctx.conv_plan reports (K = kh kw Cin, 4 Cin for the fused upsample, the padded head
+dim or key count for the batched GEMMs).  Slice neighbours of inputs hold 512 and of outputs a second sentinel; a kernel that
+reads a neighbour channel or writes one fails the comparison or the bit check."""
 import ctypes as C
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
+
+import conv_check as cc
 
 pytestmark = pytest.mark.gpu
 
@@ -41,13 +44,11 @@ def _slice_buf(ctx, dense, pitch, off, fill):
     return DevTensor(t.ptr, dense.shape, pitch=pitch, c_off=off), t, buf
 
 
-def _check_conv(got, ref, what):
-    got = got.astype(np.float64)
-    assert np.isfinite(got).all(), f"{what}: unwritten / non-finite outputs"
-    err = np.abs(got - ref)
-    tol = 2e-2 + 1e-2 * np.abs(ref)
-    assert (err <= tol).all(), f"{what}: max err {err.max():.4f} at {np.unravel_index(err.argmax(), err.shape)}; mean {err.mean():.5f}"
-    assert err.mean() < 2e-3, f"{what}: mean err {err.mean():.5f}"
+def _check_conv(r, what):
+    """conv_check.check on a _run_conv result."""
+    return cc.check(r["out"], r["conv"], r["A"], r["b"], K=r["K"], order=cc.order_of(r["variant"]), relu=r["relu"], r=r["res"],
+                    ks=cc.ksplit_of(r["variant"]), conv_model=r["conv_model"], upsample=r["conv_model"] is not None,
+                    what=f"{what} (planned {r['variant']})")
 
 
 def _run_conv(ctx, *, N, IH, IW, Cin, Cout, k=3, stride=1, pad=(1, 1), ref_pad=None, ic=None, oc=None, rc=None, no_halo=False,
@@ -55,38 +56,38 @@ def _run_conv(ctx, *, N, IH, IW, Cin, Cout, k=3, stride=1, pad=(1, 1), ref_pad=N
     """One ltb_op_conv2d through ops.Ctx.conv.  ic / oc / rc = (pitch, offset) of the input / output / residual slice (None: dense,
     no residual).  gn = (groups, guard_floats) asks for GroupNorm statistics.  ref_pad: F.pad (left, right, top, bottom) of the
     reference (default: the symmetric `pad`).  Returns a dict with the dense output, the float64 reference, the launch count and
-    the downloaded statistics buffer."""
+    the downloaded statistics buffer; conv, A, b, res, K, conv_model and variant for _check_conv."""
     from livetalking_b200.ops import ConvWeight, DevTensor
     g = torch.Generator().manual_seed(seed)
     x = (torch.randn(N, IH, IW, Cin, generator=g) * 0.7 + torch.randn(Cin, generator=g) * 0.3).half()
-    w = torch.randn(Cout, Cin, k, k, generator=g) * (2.0 / (Cin * k * k)) ** 0.5
+    w = (torch.randn(Cout, Cin, k, k, generator=g) * (2.0 / (Cin * k * k)) ** 0.5).half()
     b = torch.randn(Cout, generator=g) * 0.2
-    xd = x.double().permute(0, 3, 1, 2)
-    if upsample:
-        xd = F.interpolate(xd, scale_factor=2, mode="nearest")
+    x0 = x.double().permute(0, 3, 1, 2)
+    xd = F.interpolate(x0, scale_factor=2, mode="nearest") if upsample else x0
     if ref_pad is None:
         ref_pad = (pad[1], pad[1], pad[0], pad[0])
-    ref = F.conv2d(F.pad(xd, ref_pad), w.half().double(), b.double(), stride=stride)
-    OH, OW = ref.shape[2], ref.shape[3]
-    ref = ref.permute(0, 2, 3, 1)
+    conv = F.conv2d(F.pad(xd, ref_pad), w.double(), stride=stride)
+    A = F.conv2d(F.pad(xd.abs(), ref_pad), w.double().abs(), stride=stride).permute(0, 2, 3, 1).numpy()
+    conv_model = cc.upsample_presummed(x0, w.float().numpy()).permute(0, 2, 3, 1).numpy() if upsample else None
+    OH, OW = conv.shape[2], conv.shape[3]
+    conv = conv.permute(0, 2, 3, 1).numpy()
     ic, oc = ic or (Cin, 0), oc or (Cout, 0)
     xv, xt, xbuf = _slice_buf(ctx, x.numpy(), ic[0], ic[1], SENT_IN)
     ov, ot, obuf = _slice_buf(ctx, np.full((N, OH, OW, Cout), SENT_OUT, np.float16), oc[0], oc[1], SENT_OUT)
-    rv = None
+    rv = r = None
     if rc is not None:
-        r = (torch.randn(N, OH, OW, Cout, generator=g) * 0.5).half()
-        rv, _rt, _rbuf = _slice_buf(ctx, r.numpy(), rc[0], rc[1], SENT_IN)
-        ref = ref + r.double()
-    if relu:
-        ref = F.relu(ref)
-    cw = ConvWeight(ctx, w.numpy(), b.numpy())
+        r = (torch.randn(N, OH, OW, Cout, generator=g) * 0.5).half().numpy()
+        rv, _rt, _rbuf = _slice_buf(ctx, r, rc[0], rc[1], SENT_IN)
+    cw = ConvWeight(ctx, w.float().numpy(), b.numpy())
     st = None
     if gn is not None:
         groups, guard = gn
         st = ctx.upload(np.full(N * groups * 2 + guard, -0.0, np.float32))
+    geo = dict(N=N, IH=IH, IW=IW, OH=OH, OW=OW, stride=(stride, stride), pad=pad, res=rv, relu=relu, no_halo=no_halo,
+               upsample2x=upsample)
+    variant = ctx.conv_plan(xv, cw, ov, **geo)
     before = ctx.launch_count
-    ctx.conv(xv, cw, ov, N=N, IH=IH, IW=IW, OH=OH, OW=OW, stride=(stride, stride), pad=pad, res=rv, relu=relu, no_halo=no_halo,
-             upsample2x=upsample, gn_stats=st, gn_groups=gn[0] if gn else 0, gn_hw=OH * OW if gn else 0)
+    ctx.conv(xv, cw, ov, gn_stats=st, gn_groups=gn[0] if gn else 0, gn_hw=OH * OW if gn else 0, **geo)
     launches = ctx.launch_count - before
     full = ctx.download(ot)
     written = np.zeros(obuf.shape, bool)
@@ -94,8 +95,9 @@ def _run_conv(ctx, *, N, IH, IW, Cin, Cout, k=3, stride=1, pad=(1, 1), ref_pad=N
     changed = (_bits(full) != _bits(obuf)) & ~written
     assert not changed.any(), f"conv wrote {int(changed.sum())} elements outside its output slice, first at {np.argwhere(changed)[0]}"
     assert np.array_equal(_bits(ctx.download(xt)), _bits(xbuf)), "conv changed its input buffer"
-    return dict(out=full[..., oc[1]:oc[1] + Cout], ref=ref.numpy(), launches=launches, stats=ctx.download(st) if st is not None else None,
-                view=ov, OH=OH, OW=OW)
+    return dict(out=full[..., oc[1]:oc[1] + Cout], conv=conv, A=A, b=b.numpy(), res=r, relu=relu, variant=variant,
+                K=4 * Cin if upsample else k * k * Cin, conv_model=conv_model, launches=launches,
+                stats=ctx.download(st) if st is not None else None, view=ov, OH=OH, OW=OW)
 
 
 # ------------------------------------------------------------------------------------------------ slices, padding
@@ -125,7 +127,7 @@ SLICE_CASES = [
 @pytest.mark.parametrize("name,kw", SLICE_CASES, ids=[c[0] for c in SLICE_CASES])
 def test_conv_op_slices_and_padding(ctx, name, kw):
     r = _run_conv(ctx, seed=len(name), **kw)
-    _check_conv(r["out"], r["ref"], name)
+    _check_conv(r, name)
 
 
 # ------------------------------------------------------------------------------------------------ Ktot > taps * Cin, NULL bias
@@ -149,8 +151,10 @@ def test_conv_op_weight_koff_and_null_bias(ctx, rows):
     d.Ktot, d.w_koff, d.zdiv = Ktot, koff, 1
     check(lib().ltb_op_conv2d(ctx._h, C.byref(d)))
     got = ctx.download(ot)
-    ref = x.astype(np.float64) @ w[:, koff:koff + Cin].astype(np.float64).T
-    _check_conv(got, ref, f"koff rows={rows}")
+    wk = w[:, koff:koff + Cin].astype(np.float64).T
+    x64 = x.astype(np.float64)
+    # no residual: the gather and the halo GEMM epilogue both round acc + 0 once
+    cc.check(got, x64 @ wk, np.abs(x64) @ np.abs(wk), 0.0, K=Cin, order="gather", ks=cc.ks_ceiling(Cin), what=f"koff rows={rows}")
 
 
 # ------------------------------------------------------------------------------------------------ batched GEMMs (attention, unfused)
@@ -196,8 +200,11 @@ def test_batched_gemms_of_unfused_attention(ctx, mode):
         Kh = K[:nk].astype(np.float64).reshape(1, nk, H, dp).transpose(0, 2, 1, 3)           # rows 40..47: the zero padding rows
     else:
         Kh = K.astype(np.float64).reshape(B, nk, H, dp).transpose(0, 2, 1, 3)
-    ref_s = torch.bmm(torch.from_numpy(Qh.reshape(B * H, nq, dp)), torch.from_numpy(Kh.reshape(B * H, nk, dp)).transpose(1, 2)).numpy()
-    _check_conv(got_s, ref_s, "Q K^T")
+    def bmm(a, b):
+        return torch.bmm(torch.from_numpy(a), torch.from_numpy(b).transpose(1, 2)).numpy()
+    Qh, Kh = Qh.reshape(B * H, nq, dp), Kh.reshape(B * H, nk, dp)
+    # no bias, no residual: one rounding of the exact sum over the padded head dim
+    cc.check(got_s, bmm(Qh, Kh), bmm(np.abs(Qh), np.abs(Kh)), 0.0, K=dp, order="gather", ks=cc.ks_ceiling(dp), what=f"{mode} Q K^T")
     # P V: probabilities (zero in padded key columns) times V^T laid out [B, H, dp, nk] by transpose_heads
     P = rng.uniform(0, 1, (B * H, nq, nk))
     P[..., 50 if mode != "self_padded_keys" else nq:] = 0
@@ -210,9 +217,11 @@ def test_batched_gemms_of_unfused_attention(ctx, mode):
     ctx.conv(sv2, None, ov, N=1, IH=1, IW=nq, OH=1, OW=nq, cin=nk, cout=dp, w_ptr=VTt.ptr, ktot=nk,
              zbatch=B * H, zdiv=H, in_z=(H * nq * nk, nq * nk), w_z=(H * dp * nk, dp * nk), out_z=(nq * Hdp, dp))
     got_o = ctx.download(O).astype(np.float64)
-    ref_o = torch.bmm(torch.from_numpy(P.astype(np.float64)), torch.from_numpy(VT.astype(np.float64)).transpose(1, 2)).numpy()
-    ref_o = ref_o.reshape(B, H, nq, dp).transpose(0, 2, 1, 3).reshape(B * nq, Hdp)
-    _check_conv(got_o, ref_o, "P V")
+    def heads(a):
+        return a.reshape(B, H, nq, dp).transpose(0, 2, 1, 3).reshape(B * nq, Hdp)
+    P64, VT64 = P.astype(np.float64), VT.astype(np.float64)
+    cc.check(got_o, heads(bmm(P64, VT64)), heads(bmm(np.abs(P64), np.abs(VT64))), 0.0, K=nk, order="gather", ks=cc.ks_ceiling(nk),
+             what=f"{mode} P V")
 
 
 # ------------------------------------------------------------------------------------------------ GroupNorm statistics
@@ -268,7 +277,7 @@ def test_conv_op_groupnorm_statistics(ctx, name, kw, groups, fused):
     groupnorm_apply on them against F.group_norm.  The launch count tells the fused epilogue (1) from the separate pass (2).
     The 2*groups floats after the table hold -0.0 and must keep their bits."""
     r = _run_conv(ctx, seed=len(name) + 100, gn=(groups, 2 * groups), **kw)
-    _check_conv(r["out"], r["ref"], name)
+    _check_conv(r, name)
     assert r["launches"] == (1 if fused else 2), f"{name}: {r['launches']} launches"
     N = kw["N"]
     guard = r["stats"][N * groups * 2:]
@@ -283,7 +292,7 @@ def test_fused_gemm_statistics_stay_inside_the_table(ctx):
     sums at image index 19, one table past the end; the -0.0 guard would turn +0.0 there."""
     groups = 80
     r = _run_conv(ctx, seed=19, N=19, IH=16, IW=24, Cin=64, Cout=320, k=1, pad=(0, 0), gn=(groups, 2 * groups))
-    _check_conv(r["out"], r["ref"], "gemm nsub2")
+    _check_conv(r, "gemm nsub2")
     assert r["launches"] == 1, "expected the statistics fused into the GEMM epilogue"
     guard = r["stats"][19 * groups * 2:]
     bad = np.flatnonzero(guard.view(np.uint32) != 0x80000000)

@@ -14,6 +14,8 @@ import torch
 import torch.nn.functional as F
 from conv_cases import bits, ctx, slice_buf, weights
 
+import conv_check as cc
+
 pytestmark = pytest.mark.gpu
 
 SENT_IN = 512.0
@@ -62,12 +64,12 @@ def test_pingpong_equals_halo_kernel(ctx, switch, shape, relu):
         assert np.isfinite(outs[True].astype(np.float32)).all(), "unwritten outputs"
         diff = bits(outs[True]) != bits(outs[False])
         assert not diff.any(), f"{int(diff.sum())} of {diff.size} outputs differ from the halo kernel, first at {np.argwhere(diff)[0]}"
-        # and both against float64 (the tolerance of test_gpu_conv_res_halo)
+        # and both against float64 on the first image, with the halo kernel's rounding order (conv_check.py)
         x64 = x[:1].double().permute(0, 3, 1, 2)
-        y = (F.conv2d(F.pad(x64, (1, 1, 1, 1)), w.double(), b.double()).permute(0, 2, 3, 1) + x[:1].double())
-        ref = (F.relu(y) if relu else y).numpy()
-        err = np.abs(outs[True][:1].astype(np.float64) - ref)
-        assert (err <= 2e-2 + 1e-2 * np.abs(ref)).all() and err.mean() < 2e-3, err.max()
+        conv = F.conv2d(F.pad(x64, (1, 1, 1, 1)), w.double()).permute(0, 2, 3, 1).numpy()
+        A = F.conv2d(F.pad(x64.abs(), (1, 1, 1, 1)), w.double().abs()).permute(0, 2, 3, 1).numpy()
+        cc.check(outs[True][:1], conv, A, b.numpy(), K=9 * 64, order=cc.order_of(PINGPONG), relu=relu, r=x[:1].numpy(),
+                 what=f"pingpong b{N}_{H}x{W} relu={relu}")
     finally:
         for t in temps:
             ctx.free(t)

@@ -3,11 +3,11 @@
 Every wav2lip256 bottleneck geometry it supports (3x3 s1 with a residual on 8x8 and 4x4 maps, 3x3 s2 to 8x8 and 4x4, the
 k3 s2 ConvT on 4x4 and 8x8 grids, the 4x4 valid conv to 1x1 and the 1x1 GEMM on a 1x1 map) at B = 16, 3 and 1, through
 ltb_op_conv2d with the opt-in flag.  Inputs, outputs and residuals are channel slices whose neighbours hold sentinels that must
-keep their bits.  Bound per element: the GATHER-kind bound of test_gpu_w2l_layers.py (tensor-core accumulation over the K chain,
-fp32 epilogue adds, one fp16 rounding, and min(32, K / 128) fp32 adds of split-K partials).  Also: two launches are
+keep their bits.  Each output is held to conv_check.py with the gather rounding order (the split partials summed in fp32 with
+the bias and residual, one fp16 rounding): the bound of test_gpu_w2l_layers.py with the planned split count, and the rounding
+model.  Also: two launches are
 bit-identical, the planner routes the wav2lip256 bottleneck geometries here only when asked, and the wav2lip256 forward with
 LTB_CONV_SMALLMAP on and off agrees within the layers' bounds."""
-import math
 from types import SimpleNamespace
 
 import numpy as np
@@ -16,10 +16,11 @@ import torch
 import torch.nn.functional as F
 from conv_cases import bits, ctx, slice_buf
 
+import conv_check as cc
+
 pytestmark = pytest.mark.gpu
 
 SENT = -3.25
-U16, SUB16, V32, ULP32 = 2.0 ** -11, 2.0 ** -25, 2.0 ** -24, 2.0 ** -23
 
 # id: (IH, Cin, Cout, k, stride, pad, transposed, residual)
 CASES = {
@@ -91,21 +92,12 @@ def _launch(ctx, P, B, smallmap=True, plan_only=False, slices=True):
     return full[..., oc[1]:oc[1] + cout]
 
 
-def _check(P, got, ks):
+def _check(P, got, ks, what):
     K = 4 * P["cin"] if P["tr"] else P["cin"] * P["k"] ** 2
-    bb = P["b"][None, :, None, None]
-    pre = P["conv"] + bb
-    r = P["r"].double().permute(0, 3, 1, 2) if P["r"] is not None else torch.zeros_like(pre)
-    ref = torch.relu(pre + r)
-    A = P["A"]
-    bound = (18 * math.ceil(K / 16) * ULP32 * A + 3 * V32 * (A + bb.abs() + r.abs()) + U16 * ref.abs() + SUB16
-             + min(32, K // 128) * V32 * (A + bb.abs()))
     assert ks <= min(32, K // 128)
-    g = torch.from_numpy(got.astype(np.float64)).permute(0, 3, 1, 2)
-    assert torch.isfinite(g).all(), "unwritten / non-finite outputs"
-    ratio = ((g - ref).abs() / (1.25 * bound)).max().item()
-    assert ratio <= 1.0, f"err / bound {ratio:.3f}"
-    return ratio
+    nhwc = lambda t: t.permute(0, 2, 3, 1).numpy()
+    return cc.check(got, nhwc(P["conv"]), nhwc(P["A"]), P["b"].numpy(), K=K, order=cc.order_of(dict(kernel=4)), relu=True,
+                    r=None if P["r"] is None else P["r"].numpy(), ks=ks, what=what)
 
 
 @pytest.mark.parametrize("B", [16, 3, 1])
@@ -116,7 +108,7 @@ def test_smallmap_against_float64(ctx, name, B):
     assert v["kernel"] == 4 and v["bn"] == 128 and v["kb"] == 64, v
     assert v["taps"] == (9 if P["tr"] else P["k"] ** 2), v
     got = _launch(ctx, P, B, slices=(B != 1))
-    _check(P, got, v["ksplit"])
+    _check(P, got, v["ksplit"], f"smallmap {name} B={B}")
 
 
 @pytest.mark.parametrize("name", ["res3x3_8x8", "convT_8x8", "k4_valid"])

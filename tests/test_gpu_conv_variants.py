@@ -3,8 +3,8 @@
 conv_halo.cu builds conv_halo_wgmma_kernel<BN, NSUB, NACC, TAPS, RC, GRP> and conv_gather.cu conv_gather_wgmma_kernel<BN, KB, GRP>;
 which one runs is decided by the host planner from the shape (and, for the resident-weight halo variants, the SM count).  VARIANTS
 has one row per instance, keyed by its template arguments: an ltb_op_conv2d geometry that Ctx.conv_plan (ltb_op_conv2d_plan) must
-map to exactly that instance, then the op itself against float64 PyTorch on the same fp16 inputs and fp16-rounded weights
-(|err| <= 2e-2 + 1e-2 |ref|, mean < 2e-3).  Inputs, outputs and residuals are channel slices whose neighbours hold sentinels; every
+map to exactly that instance, then the op itself against float64 PyTorch on the same fp16 inputs and fp16 weights, held to
+conv_check.py: the hard error bound and the rounding model of the instance's kernel.  Inputs, outputs and residuals are channel slices whose neighbours hold sentinels; every
 byte outside the output slice must keep its bits and the inputs must not change.  Rows reach, where the instance admits them: a
 ragged last M tile or overhanging halo tiles, Cin that is not a multiple of 64 (zero-filled last K chunk), several N tiles (the
 resident variants need exactly one), more tiles than SMs (persistent halo CTAs run a second tile, the mbarrier phases wrap), and
@@ -24,6 +24,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 from kernel_instances import compiled_instances
+
+import conv_check as cc
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 H100_SMS = 132
@@ -203,25 +205,30 @@ def _pack_convT(w):
     return np.ascontiguousarray(rows), np.ascontiguousarray(view)
 
 
-def _reference(row, x, w, b):
-    """float64 NCHW result of the row's op.  x: (N, Cin, H, W); w: (Cout, Cin, k, k), ConvT (Cin, Cout, 3, 3)."""
-    if row["kind"] == "convT":
-        return F.conv_transpose2d(x, w, b, stride=2, padding=1, output_padding=1)
-    if row["kind"] == "up":
-        x = F.interpolate(x, scale_factor=2, mode="nearest")
-    p = row["pad"]
-    return F.conv2d(F.pad(x, (p, p, p, p)), w, b, stride=row["stride"])
+def _reference(row, x, w):
+    """float64 NHWC parts of the row's op on x (N, Cin, H, W) and w (Cout, Cin, k, k), ConvT (Cin, Cout, 3, 3): (conv without
+    bias, conv of the absolute values, the fused upsample's sum with its pre-summed fp16 weights or None)."""
+    def op(a, b):
+        if row["kind"] == "convT":
+            return F.conv_transpose2d(a, b, stride=2, padding=1, output_padding=1)
+        if row["kind"] == "up":
+            a = F.interpolate(a, scale_factor=2, mode="nearest")
+        p = row["pad"]
+        return F.conv2d(F.pad(a, (p, p, p, p)), b, stride=row["stride"])
+    nhwc = lambda t: t.permute(0, 2, 3, 1).numpy()
+    up = nhwc(cc.upsample_presummed(x, w.float().numpy())) if row["kind"] == "up" else None
+    return nhwc(op(x, w)), nhwc(op(x.abs(), w.abs())), up
 
 
-def _check_close(got, ref, what):
-    got = got.astype(np.float64)
-    assert np.isfinite(got).all(), f"{what}: {int((~np.isfinite(got)).sum())} unwritten / non-finite outputs, first at {np.argwhere(~np.isfinite(got))[0]}"
-    err = np.abs(got - ref)
-    tol = 2e-2 + 1e-2 * np.abs(ref)
-    bad = err > tol
-    assert not bad.any(), (f"{what}: {int(bad.sum())} of {bad.size} outside tolerance; max err {err.max():.4f} at "
-                           f"{np.unravel_index(err.argmax(), err.shape)} (got {got.flat[err.argmax()]:.4f}, want {ref.flat[err.argmax()]:.4f})")
-    assert err.mean() < 2e-3, f"{what}: mean err {err.mean():.5f}"
+def _chain_k(row):
+    return 4 * row["Cin"] if row["kind"] in ("convT", "up") else row["k"] ** 2 * row["Cin"]
+
+
+def _check_model(got, parts, b, r, relu, row, variant, what, ks=None):
+    """conv_check.check of the row's output: parts = (conv, A, conv_model) of _reference, b the bias per element."""
+    conv, A, up = parts
+    return cc.check(got, conv, A, b, K=_chain_k(row), order=cc.order_of(variant), relu=relu, r=r,
+                    ks=cc.ksplit_of(variant) if ks is None else ks, conv_model=up, upsample=up is not None, what=what)
 
 
 def _run_row(ctx, row, seed, relu, with_res):
@@ -241,8 +248,8 @@ def _run_row(ctx, row, seed, relu, with_res):
     w = w.half()
     b = torch.randn(nslot, Cout, generator=g) * 0.2
     x64 = x.double().permute(0, 3, 1, 2)
-    ref_shape = _reference(row, x64[:1, :, :, :], w[0].double(), b[0].double()).shape
-    OH, OW = ref_shape[2], ref_shape[3]
+    OH, OW = (2 * IH, 2 * IW) if kind in ("convT", "up") else ((IH + 2 * row["pad"] - k) // row["stride"] + 1,
+                                                               (IW + 2 * row["pad"] - k) // row["stride"] + 1)
     ICtot, OCtot, RCtot = Cin + 24, Cout + 16, Cout + 8
     xv, xt, xbuf = _slice_buf(ctx, x.numpy(), ICtot, 8, SENT_IN)
     ov, ot, obuf = _slice_buf(ctx, np.full((N, OH, OW, Cout), np.nan, np.float16), OCtot, 8, SENT_OUT)
@@ -291,13 +298,15 @@ def _run_row(ctx, row, seed, relu, with_res):
         assert np.array_equal(_bits(ctx.download(rt)), _bits(rbuf)), "the conv changed its residual buffer"
     got = full[..., 8:8 + Cout]
     slots = [table[n // gi] for n in range(N)] if gi else [0] * N
-    ref = np.empty(got.shape, np.float64)
+    # each group's float64 parts with its own slot's weights and bias
+    parts = [np.empty(got.shape, np.float64) for _ in range(3 if kind == "up" else 2)]
+    bias = np.empty((N, 1, 1, Cout), np.float64)
     for s in sorted(set(slots)):
         idx = [n for n in range(N) if slots[n] == s]
-        y = _reference(row, x64[idx], w[s].double(), b[s].double()).permute(0, 2, 3, 1)
-        if with_res:
-            y = y + r[idx].double()
-        ref[idx] = (F.relu(y) if relu else y).numpy()
+        for dst, src in zip(parts, _reference(row, x64[idx], w[s].double())):
+            dst[idx] = src
+        bias[idx] = b[s].double().numpy()
+    ref = (parts[0], parts[1], parts[2] if kind == "up" else None), bias, (r.numpy() if with_res else None)
 
     def ungrouped(grp, s):
         """The ungrouped op on group grp's images with slot s's weights, into a fresh output slice."""
@@ -329,9 +338,9 @@ def _assert_variant(variant, want, sms, what):
 
 
 def _check_row(ctx, sms, what, row, want, seed, relu, with_res):
-    (variant, got, ref, ungrouped, slots), temps = _run_row(ctx, row, seed, relu, with_res)
+    (variant, got, (parts, bias, r), ungrouped, slots), temps = _run_row(ctx, row, seed, relu, with_res)
     try:
-        _check_close(got, ref, f"{what} (planned {variant})")
+        _check_model(got, parts, bias, r, relu, row, variant, f"{what} (planned {variant})")
         _assert_variant(variant, want, sms, what)
         if ungrouped is not None:
             gi = row["gi"]

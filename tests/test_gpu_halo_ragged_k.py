@@ -12,7 +12,7 @@ output conv is checked against the separate head kernel by test_gpu_w2l_layers.p
 import numpy as np
 import pytest
 import torch
-from test_gpu_conv_variants import (H100_SMS, SENT_IN, SENT_OUT, H, _bits, _check_close, _conv, _convT, _expected, _gemm, _key_id,
+from test_gpu_conv_variants import (H100_SMS, SENT_IN, SENT_OUT, H, _bits, _check_model, _conv, _convT, _expected, _gemm, _key_id,
                                     _pack_convT, _reference, _shape_weight, _slice_buf, _up)
 
 CASES = [
@@ -126,10 +126,8 @@ def test_ragged_cin_is_bit_identical_to_zero_padded_cin(ctx, case):
     w = (torch.randn(*((Cin, Cout) if tr else (Cout, Cin)), k, k, generator=g) * (2.0 / (Cin * k * k)) ** 0.5).half()
     b = torch.randn(Cout, generator=g) * 0.2
     relu, with_res = case % 2 == 0, case % 3 != 2
-    y = _reference(row, x.double().permute(0, 3, 1, 2), w.double(), b.double()).permute(0, 2, 3, 1)
-    r = (torch.randn(*y.shape, generator=g) * 0.5).half() if with_res else None
-    if with_res:
-        y = y + r.double()
+    parts = _reference(row, x.double().permute(0, 3, 1, 2), w.double())
+    r = (torch.randn(*parts[0].shape, generator=g) * 0.5).half() if with_res else None
 
     variant, got = _run(ctx, row, x, w, b, r, relu)
     x_pad = torch.cat([x, torch.zeros(N, IH, IW, pad, dtype=x.dtype)], dim=-1)
@@ -138,7 +136,7 @@ def test_ragged_cin_is_bit_identical_to_zero_padded_cin(ctx, case):
 
     want = _expected(key)
     assert variant == want and variant_pad == want, f"planned {variant} (Cin {Cin}) and {variant_pad} (Cin {Cin + pad}), expected {want}"
-    _check_close(got, (torch.relu(y) if relu else y).numpy(), IDS[case])
+    _check_model(got, parts, b.double().numpy(), None if r is None else r.numpy(), relu, row, variant, IDS[case])
     diff = _bits(got) != _bits(got_pad)
     assert not diff.any(), (f"{IDS[case]}: {int(diff.sum())} outputs differ from the zero-padded Cin {Cin + pad}, first at "
                             f"{np.argwhere(diff)[0]}")
