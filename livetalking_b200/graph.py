@@ -6,7 +6,7 @@ memory a session allocates, captures the session's op sequence into one CUDA gra
 from __future__ import annotations
 
 import os
-from typing import Callable, List, Optional
+from typing import Callable, List, Optional, Tuple
 
 import numpy as np
 
@@ -190,6 +190,7 @@ class GraphSession:
         self.graph: Optional[Graph] = None
         self._owned: List[DevTensor] = []
         self._ctxs: List[Ctx] = []                       # contexts close() closes
+        self._paste: Optional[Tuple[Ctx, DevTensor, DevTensor]] = None
         self._borrowed = with_ctx and ctx is not None
         self.ctx = None
         if with_ctx:
@@ -200,6 +201,14 @@ class GraphSession:
         c = Ctx()
         self._ctxs.append(c)
         return c
+
+    def paste_ctx(self, pred_shape, pred_dtype, frame_shape) -> Tuple[Ctx, DevTensor, DevTensor]:
+        """(ctx, prediction scratch, uint8 output frame) for pasting one host prediction, made on first use.  The ctx is the session's
+        own (new_ctx), so a paste runs while the session's graph is in flight (the reference's process_frames thread)."""
+        if self._paste is None:
+            c = self.new_ctx()
+            self._paste = (c, c.alloc(pred_shape, pred_dtype), c.alloc(frame_shape, np.uint8))
+        return self._paste
 
     def alloc(self, shape, dtype=np.float16, zero: bool = False) -> DevTensor:
         t = self.ctx.alloc(shape, dtype, zero=zero)
@@ -228,7 +237,7 @@ class GraphSession:
             self.ctx.sync()
             for t in owned:
                 self.ctx.free(t)
-        ctxs, self._ctxs = self._ctxs, []
+        ctxs, self._ctxs, self._paste = self._ctxs, [], None
         for c in ctxs:
             c.close()
         self.ctx = None

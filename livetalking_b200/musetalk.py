@@ -7,6 +7,9 @@ device operators — tcgen05 implicit-GEMM convs / linears / attention GEMMs, Gr
 captures them ONCE into a CUDA graph per batch size and replays the graph per step.  Weights are taken from state_dicts
 with the diffusers key scheme (so a real ``unet.pth`` / ``sd-vae`` loads by name).
 
+``MuseTalkBatchSession`` runs G sessions' frames through one graph, each group's latents gathered from its own avatar before the
+launch (cross-session mode); ``MuseTalkSession`` is its one-group form bound to one avatar, one session's own stream.
+
 Load-time rewrites (exact up to fp16 rounding):
   * timestep is the constant 0 (musetalk_avatar.py:61): ``time_emb_proj(silu(time_embedding(t=0)))`` is folded into the
     bias of every ResnetBlock's conv1;
@@ -356,109 +359,6 @@ class MuseTalkAvatar:
         self.latents = ctx.upload(lat16)
 
 
-class MuseTalkSession(GraphSession):
-    """One avatar stream at a fixed batch size: the captured UNet + VAE-decode graph and the paste-back buffers."""
-
-    def __init__(self, model: MuseTalkModel, avatar: MuseTalkAvatar, batch: int, keep_taps: bool = False, ctx: Optional[Ctx] = None,
-                 paste_only: bool = False):
-        """ctx: the session's own stream + scratch (created here unless given).  Sessions never share a ctx: the reference
-        opens up to max_session of them concurrently (app.py:76-100), each driven by its own three threads, and capturing /
-        synchronising a stream another session is using would corrupt both.
-        paste_only: no network graph and no activation arena — only paste_pred() works (cross-session mode: the UNet / VAE pass of
-        this session's frames runs in a shared MuseTalkBatchSession)."""
-        super().__init__(ctx, with_ctx=not paste_only)
-        self.model, self.avatar, self.B = model, avatar, int(batch)
-        self._paste_ctx = None
-        if paste_only:
-            return
-        try:
-            ctx, B, hw = self.ctx, self.B, avatar.lat_hw
-            self.d_index = self.alloc((4,), np.int32, zero=True)
-            self.audio_in = self.alloc((B, KEY_PAD, model.ucfg.cross_attention_dim), np.float16, zero=True)
-            self.audio_pe = self.alloc((B * KEY_PAD, model.ucfg.cross_attention_dim), np.float16, zero=True)
-            self.latents16 = self.alloc((B, hw, hw, 16), np.float16, zero=True)
-            self.image_u8 = self.alloc((B, hw * 8, hw * 8, 3), np.uint8, zero=True)
-            self.frames_out = self.alloc((B, avatar.H, avatar.W, 3), np.uint8, zero=True)
-            self.taps = {} if keep_taps else None
-            self._audio_host = np.zeros((B, KEY_PAD, model.ucfg.cross_attention_dim), np.float16)
-
-            def emit(b: Builder):
-                ctx.gather_rows(avatar.latents, avatar.latents.shape[0], self.d_index, B, hw * hw * 16, self.latents16)
-                ctx.eltwise(self.audio_in, model.pe, self.audio_in.rows * self.audio_in.C, KEY_PAD * self.audio_in.C, 0, self.audio_pe)
-                self.pred16 = model.emit_unet(b, self.latents16, self.audio_pe, self.taps)
-                self.image16 = model.emit_vae_decode(b, self.pred16, self.image_u8, self.taps)
-
-            self.capture(emit)
-        except BaseException:
-            self.close()
-            raise
-
-    # ---- MuseReal.inference_batch (musetalk_avatar.py:130-152)
-    def infer_async(self, index: int, audio_feats: Optional[np.ndarray] = None):
-        if self.graph is None:
-            raise RuntimeError("MuseTalkSession: paste-only (or closed) session has no network graph")
-        if audio_feats is not None:
-            a = np.asarray(audio_feats)
-            if a.shape != (self.B, 50, self._audio_host.shape[2]):
-                raise ValueError(f"audio features must be ({self.B},50,{self._audio_host.shape[2]}), got {a.shape}")
-            self._audio_host[:, :50] = a.astype(np.float16)
-            self.ctx.h2d(self.audio_in, self._audio_host, sync=False)
-        self.ctx.set_i32(self.d_index, index)
-        self.graph.launch()
-
-    def infer(self, index: int, audio_feats: Optional[np.ndarray] = None, want_pred: bool = True):
-        with self.ctx.lock:       # h2d -> index -> graph -> d2h is one critical section (inference vs process_frames thread)
-            self.infer_async(index, audio_feats)
-            if want_pred:
-                return self.ctx.download(self.image_u8)          # uint8 (B,hw*8,hw*8,3) BGR, as vae.decode_latents returns
-            self.ctx.sync()
-            return None
-
-    # ---- MuseReal.paste_back_frame (musetalk_avatar.py:154-164)
-    def _paste_op(self, pred: DevTensor, slot0: int, index: int, explicit_idx: int, count: int):
-        self.ctx.mt_paste(_paste_op(self.avatar, pred, self.frames_out, slot0, index, explicit_idx, count))
-
-    def paste(self, slot: int, idx: int) -> np.ndarray:
-        if not (0 <= slot < self.B and 0 <= idx < self.avatar.n):
-            raise ValueError("paste: slot / idx out of range")
-        with self.ctx.lock:
-            self._paste_op(self.image_u8, slot, 0, idx, 1)
-            one = DevTensor(self.frames_out.ptr, (self.avatar.H, self.avatar.W, 3), np.uint8)
-            return self.ctx.download(one)
-
-    def paste_pred(self, pred_u8: np.ndarray, idx: int) -> np.ndarray:
-        """paste_back_frame for a host prediction (S,S,3) uint8 — the reference's exact argument.  Runs on its own small
-        ctx (stream + scratch prediction + output frame): process_frames calls it while inference_batch is in flight."""
-        S = self.avatar.lat_hw * 8
-        pred_u8 = np.ascontiguousarray(pred_u8, np.uint8)
-        if pred_u8.shape != (S, S, 3):
-            raise ValueError(f"paste_pred: prediction must be ({S},{S},3) uint8, got {pred_u8.shape}")
-        if not 0 <= idx < self.avatar.n:
-            raise ValueError("paste_pred: idx out of range")
-        if self._paste_ctx is None:
-            self._paste_ctx = self.new_ctx()
-            self._pred_scratch = self._paste_ctx.alloc((1, S, S, 3), np.uint8)
-            self._paste_out = self._paste_ctx.alloc((self.avatar.H, self.avatar.W, 3), np.uint8)
-        pc = self._paste_ctx
-        with pc.lock:
-            pc.h2d(self._pred_scratch, pred_u8, sync=False)
-            pc.mt_paste(_paste_op(self.avatar, self._pred_scratch, self._paste_out, 0, 0, idx, 1))
-            return pc.download(self._paste_out)
-
-    def paste_batch_async(self, index: int):
-        self._paste_op(self.image_u8, 0, index, -1, self.B)
-
-    def paste_batch(self, index: int, out: Optional[np.ndarray] = None) -> np.ndarray:
-        with self.ctx.lock:
-            self.paste_batch_async(index)
-            return self.ctx.download(self.frames_out, out)
-
-    def step_async(self, index: int):
-        """Everything resident (audio features already on the device): UNet + VAE decode + blend paste-back."""
-        self.infer_async(index, None)
-        self.paste_batch_async(index)
-
-
 class MuseTalkBatchSession(GraphSession):
     """Cross-session batching for MuseTalk (SURVEY 8(f) rank 1, the MuseTalk twin of ltb_w2l_infer_slots): up to G sessions x Bs
     frames run as ONE captured PE + UNet + VAE-decode graph of batch G*Bs.  A *group request* is (avatar, first frame index,
@@ -466,11 +366,18 @@ class MuseTalkBatchSession(GraphSession):
     graph, so any session may occupy any group of any round), its features occupy rows [g*Bs, (g+1)*Bs) of audio_in.
     The reference serves every session with its own B-frame forward (avatars/musetalk_avatar.py:130-152 under app.py:76-100's
     max_session connections); at batch 8 the UNet is launch-latency bound (64 M-tiles per layer), so four sessions per
-    launch cost far less than four launches.  `batch` / `infer_slots` make it a mux for plugin.batcher.CrossSessionBatcher."""
+    launch cost far less than four launches.  `batch` / `infer_slots` make it a mux for plugin.batcher.CrossSessionBatcher.
 
-    def __init__(self, model: MuseTalkModel, lat_hw: int, groups: int, frames_per_session: int, ctx: Optional[Ctx] = None):
+    keep_taps: `taps` holds the UNet's and the VAE decoder's intermediate activations (else None).
+    avatar: bind the session to this one avatar — every request must use it, and its output frames are allocated here.
+    ctx: the session's own stream + scratch (created here unless given).  Sessions never share a ctx: the reference opens up to
+    max_session of them concurrently (app.py:76-100), each driven by its own three threads, and capturing / synchronising a stream
+    another session is using would corrupt both."""
+
+    def __init__(self, model: MuseTalkModel, lat_hw: int, groups: int, frames_per_session: int, *, ctx: Optional[Ctx] = None,
+                 keep_taps: bool = False, avatar: Optional[MuseTalkAvatar] = None):
         super().__init__(ctx)
-        self.model, self.lat_hw, self.Bs, self.G = model, int(lat_hw), int(frames_per_session), int(groups)
+        self.model, self.lat_hw, self.Bs, self.G, self.avatar = model, int(lat_hw), int(frames_per_session), int(groups), avatar
         self.batch = self.G                                  # CrossSessionBatcher: requests per engine call
         self.B = B = self.G * self.Bs
         try:
@@ -484,12 +391,19 @@ class MuseTalkBatchSession(GraphSession):
             self.latents16_of = [DevTensor(self.latents16.ptr + g * Bs * hw * hw * 16 * 2, (Bs, hw, hw, 16)) for g in range(self.G)]
             self.image_u8 = self.alloc((B, hw * 8, hw * 8, 3), np.uint8, zero=True)
             self._frames_out: Dict[tuple, DevTensor] = {}
+            if avatar is not None:
+                if self.G != 1:
+                    raise ValueError("a session bound to an avatar has one group")
+                self.frames_out = self._out(0, avatar)
+                # the warm-up pass below runs on the avatar's frame-0 latents (d_index is 0), not on zeros
+                ctx.gather_rows(avatar.latents, avatar.latents.shape[0], self.d_index[0], Bs, hw * hw * 16, self.latents16_of[0])
+            self.taps = {} if keep_taps else None
             self._audio_host = np.zeros((B, KEY_PAD, cad), np.float16)
 
             def emit(b: Builder):
                 ctx.eltwise(self.audio_in, model.pe, self.audio_in.rows * self.audio_in.C, KEY_PAD * self.audio_in.C, 0, self.audio_pe)
-                self.pred16 = model.emit_unet(b, self.latents16, self.audio_pe, None)
-                self.image16 = model.emit_vae_decode(b, self.pred16, self.image_u8, None)
+                self.pred16 = model.emit_unet(b, self.latents16, self.audio_pe, self.taps)
+                self.image16 = model.emit_vae_decode(b, self.pred16, self.image_u8, self.taps)
 
             self.capture(emit)
         except BaseException:
@@ -502,9 +416,14 @@ class MuseTalkBatchSession(GraphSession):
         for r in requests:
             if r[0].lat_hw != self.lat_hw:
                 raise ValueError("avatar latent size does not match the batch session")
+            if self.avatar is not None and r[0] is not self.avatar:
+                raise ValueError("the session is bound to another avatar")
 
-    def infer_async(self, requests: Sequence[tuple]):
-        """requests[g] = (MuseTalkAvatar, first frame index, features (Bs,50,384) | None = resident in audio_in_of[g])."""
+    def _launch(self, requests: Sequence[tuple]):
+        """requests[g] = (MuseTalkAvatar, first frame index, features (Bs,50,384) | None = resident in audio_in_of[g]): stage the
+        features, gather every group's latents (set_i32 + gather_rows before the launch) and launch the graph."""
+        if self.graph is None:
+            raise RuntimeError(f"{type(self).__name__}: paste-only (or closed) session has no network graph")
         self._check(requests)
         ctx, Bs, row = self.ctx, self.Bs, self.lat_hw * self.lat_hw * 16
         stage = False
@@ -512,7 +431,7 @@ class MuseTalkBatchSession(GraphSession):
             if feats is not None:
                 a = np.asarray(feats)
                 if a.shape != (Bs, 50, self._audio_host.shape[2]):
-                    raise ValueError(f"group features must be ({Bs},50,{self._audio_host.shape[2]}), got {a.shape}")
+                    raise ValueError(f"audio features must be ({Bs},50,{self._audio_host.shape[2]}), got {a.shape}")
                 self._audio_host[g * Bs:(g + 1) * Bs, :50] = a.astype(np.float16)
                 stage = True
             ctx.set_i32(self.d_index[g], int(index))
@@ -521,17 +440,6 @@ class MuseTalkBatchSession(GraphSession):
             n = len(requests) * Bs
             ctx.h2d(DevTensor(self.audio_in.ptr, (n,) + self.audio_in.shape[1:]), self._audio_host[:n], sync=False)
         self.graph.launch()
-
-    def infer_groups(self, requests: Sequence[tuple]) -> List[np.ndarray]:
-        """-> per request its (Bs, S, S, 3) uint8 BGR predictions (what MuseReal.inference_batch returns for that session)."""
-        with self.ctx.lock:
-            self.infer_async(requests)
-            n = len(requests) * self.Bs
-            S = self.lat_hw * 8
-            pred = self.ctx.download(DevTensor(self.image_u8.ptr, (n, S, S, 3), np.uint8))
-        return [pred[g * self.Bs:(g + 1) * self.Bs] for g in range(len(requests))]
-
-    infer_slots = infer_groups
 
     def _out(self, g: int, av: MuseTalkAvatar) -> DevTensor:
         key = (g, av.H, av.W)
@@ -549,17 +457,93 @@ class MuseTalkBatchSession(GraphSession):
             outs.append(out)
         return outs
 
+    infer_async = _launch
+
+    def infer_groups(self, requests: Sequence[tuple]) -> List[np.ndarray]:
+        """-> per request its (Bs, S, S, 3) uint8 BGR predictions (what MuseReal.inference_batch returns for that session)."""
+        with self.ctx.lock:
+            self._launch(requests)
+            n = len(requests) * self.Bs
+            S = self.lat_hw * 8
+            pred = self.ctx.download(DevTensor(self.image_u8.ptr, (n, S, S, 3), np.uint8))
+        return [pred[g * self.Bs:(g + 1) * self.Bs] for g in range(len(requests))]
+
+    infer_slots = infer_groups
+
     def step_async(self, requests: Sequence[tuple]):
-        self.infer_async(requests)
+        self._launch(requests)
         self.paste_async(requests)
 
     def step(self, requests: Sequence[tuple]) -> List[np.ndarray]:
         """One batched round: returns, per session, its Bs composited frames (Bs, H, W, 3) uint8."""
         with self.ctx.lock:
-            self.infer_async(requests)
+            self._launch(requests)
             outs = [self.ctx.download(t, sync=False) for t in self.paste_async(requests)]
             self.ctx.sync()
             return outs
+
+
+class MuseTalkSession(MuseTalkBatchSession):
+    """One avatar stream at a fixed batch size: MuseTalkBatchSession with one group, bound to `avatar`."""
+
+    def __init__(self, model: MuseTalkModel, avatar: MuseTalkAvatar, batch: int, keep_taps: bool = False, ctx: Optional[Ctx] = None,
+                 paste_only: bool = False):
+        """paste_only: no ctx, network graph or activation arena — only paste_pred() works (cross-session mode: the UNet / VAE pass
+        of this session's frames runs in a shared MuseTalkBatchSession)."""
+        if paste_only:
+            GraphSession.__init__(self, ctx, with_ctx=False)
+            self.model, self.avatar, self.B = model, avatar, int(batch)
+            return
+        super().__init__(model, avatar.lat_hw, 1, batch, ctx=ctx, keep_taps=keep_taps, avatar=avatar)
+
+    # ---- MuseReal.inference_batch (musetalk_avatar.py:130-152)
+    def infer_async(self, index: int, audio_feats: Optional[np.ndarray] = None):
+        self._launch([(self.avatar, index, audio_feats)])
+
+    def infer(self, index: int, audio_feats: Optional[np.ndarray] = None, want_pred: bool = True):
+        with self.ctx.lock:       # h2d -> index -> graph -> d2h is one critical section (inference vs process_frames thread)
+            self.infer_async(index, audio_feats)
+            if want_pred:
+                return self.ctx.download(self.image_u8)          # uint8 (B,hw*8,hw*8,3) BGR, as vae.decode_latents returns
+            self.ctx.sync()
+            return None
+
+    # ---- MuseReal.paste_back_frame (musetalk_avatar.py:154-164)
+    def paste(self, slot: int, idx: int) -> np.ndarray:
+        if not (0 <= slot < self.B and 0 <= idx < self.avatar.n):
+            raise ValueError("paste: slot / idx out of range")
+        with self.ctx.lock:
+            self.ctx.mt_paste(_paste_op(self.avatar, self.image_u8, self.frames_out, slot, 0, idx, 1))
+            one = DevTensor(self.frames_out.ptr, (self.avatar.H, self.avatar.W, 3), np.uint8)
+            return self.ctx.download(one)
+
+    def paste_pred(self, pred_u8: np.ndarray, idx: int) -> np.ndarray:
+        """paste_back_frame for a host prediction (S,S,3) uint8 — the reference's exact argument, on the session's paste ctx."""
+        a = self.avatar
+        S = a.lat_hw * 8
+        pred_u8 = np.ascontiguousarray(pred_u8, np.uint8)
+        if pred_u8.shape != (S, S, 3):
+            raise ValueError(f"paste_pred: prediction must be ({S},{S},3) uint8, got {pred_u8.shape}")
+        if not 0 <= idx < a.n:
+            raise ValueError("paste_pred: idx out of range")
+        pc, pred, out = self.paste_ctx((1, S, S, 3), np.uint8, (a.H, a.W, 3))
+        with pc.lock:
+            pc.h2d(pred, pred_u8, sync=False)
+            pc.mt_paste(_paste_op(a, pred, out, 0, 0, idx, 1))
+            return pc.download(out)
+
+    def paste_batch_async(self, index: int):
+        self.paste_async([(self.avatar, index, None)])
+
+    def paste_batch(self, index: int, out: Optional[np.ndarray] = None) -> np.ndarray:
+        with self.ctx.lock:
+            self.paste_batch_async(index)
+            return self.ctx.download(self.frames_out, out)
+
+    def step_async(self, index: int):
+        """Everything resident (audio features already on the device): latent gather + UNet + VAE decode + blend paste-back."""
+        self.infer_async(index, None)
+        self.paste_batch_async(index)
 
 
 def _paste_op(a: MuseTalkAvatar, pred: DevTensor, out: DevTensor, slot0: int, index: int, explicit_idx: int, count: int) -> _capi.MtPasteOp:

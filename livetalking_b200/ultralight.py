@@ -10,7 +10,8 @@ straight into channel slices of the concat buffers.  One CUDA graph per (session
 
 Cross-session batching (``UltraLightBatchSession``): the network belongs to the avatar, so a batch of several sessions runs every
 layer as a *grouped* op — the weights of up to S avatars are stacked slot by slot in an ``UltraLightBank`` and image n of the
-batch reads slot ``group_slot[n // Bs]`` from a device table, so one captured graph serves any assignment of avatars to groups."""
+batch reads slot ``group_slot[n // Bs]`` from a device table, so one captured graph serves any assignment of avatars to groups.
+``UltraLightSession`` is its one-group form bound to one avatar: no bank, the avatar's own network on the ungrouped ops."""
 from __future__ import annotations
 
 from typing import Dict, List, Optional, Sequence
@@ -238,132 +239,58 @@ class _Grouping:
         return (self.table, self.images, int(np.prod(w.shape)), int(np.prod(b.shape)))
 
 
-class UltraLightSession(GraphSession):
-    """One avatar stream at a fixed batch size: captured prep + U-Net + head graph, paste-back buffers."""
-
-    def __init__(self, avatar: UltraLightAvatar, batch: int, keep_taps: bool = False, ctx: Optional[Ctx] = None, paste_only: bool = False):
-        """paste_only: no network graph and no activation arena — only paste_pred() works (cross-session mode: this session's
-        U-Net pass runs in a shared UltraLightBatchSession)."""
-        super().__init__(ctx, with_ctx=not paste_only)
-        self.avatar, self.B = avatar, int(batch)
-        self._paste_ctx = None
-        if paste_only:
-            return
-        try:
-            ctx, B = self.ctx, self.B
-            self.d_index = self.alloc((4,), np.int32, zero=True)
-            self.audio16 = self.alloc((B, 32, 32, 16), np.float16, zero=True)           # NHWC view of audiofeat.reshape(16, 32, 32)
-            self.img16 = self.alloc((B, FACE, FACE, 16), np.float16, zero=True)
-            self.pred = self.alloc((B, FACE, FACE, 3), np.float32, zero=True)
-            self.frames_out = self.alloc((B, avatar.H, avatar.W, 3), np.uint8, zero=True)
-            self.taps = {} if keep_taps else None
-
-            def emit(b: Builder):
-                ctx.ul_prep(avatar.faces, avatar.n, self.d_index, B, self.img16)
-                avatar.model.emit(b, self.img16, self.audio16, self.pred, self.taps)
-
-            self.capture(emit)
-        except BaseException:
-            self.close()
-            raise
-
-    # ---- LightReal.inference_batch (ultralight_avatar.py:141-169)
-    def infer_async(self, index: int, audio_feats: Optional[np.ndarray] = None):
-        """audio_feats: (B, 16, 1024) float (the HubertASR windows) or None when audio16 is already resident."""
-        if self.graph is None:
-            raise RuntimeError("UltraLightSession: paste-only (or closed) session has no network graph")
-        if audio_feats is not None:
-            a = np.asarray(audio_feats, np.float32)
-            if a.shape != (self.B, 16, 1024):
-                raise ValueError(f"audio features must be ({self.B},16,1024), got {a.shape}")
-            self.ctx.h2d(self.audio16, np.ascontiguousarray(a.transpose(0, 2, 1)).astype(np.float16), sync=False)
-        self.ctx.set_i32(self.d_index, index)
-        self.graph.launch()
-
-    def infer(self, index: int, audio_feats: Optional[np.ndarray] = None, want_pred: bool = True):
-        with self.ctx.lock:
-            self.infer_async(index, audio_feats)
-            if want_pred:
-                return self.ctx.download(self.pred)              # float32 (B,160,160,3) = pred * 255, as the reference returns
-            self.ctx.sync()
-            return None
-
-    # ---- LightReal.paste_back_frame (ultralight_avatar.py:171-184)
-    def paste_batch_async(self, index: int):
-        a = self.avatar
-        self.ctx.ul_paste(a.frames, a.faces, a.coords, self.pred, self.frames_out, a.n, a.H, a.W, index, -1, 0, self.B)
-
-    def paste_batch(self, index: int, out: Optional[np.ndarray] = None) -> np.ndarray:
-        with self.ctx.lock:
-            self.paste_batch_async(index)
-            return self.ctx.download(self.frames_out, out)
-
-    def infer_paste(self, index: int, audio_feats: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None) -> np.ndarray:
-        """inference_batch + B x paste_back_frame as one engine round: (B, H, W, 3) uint8 composited frames."""
-        with self.ctx.lock:
-            self.infer_async(index, audio_feats)
-            self.paste_batch_async(index)
-            return self.ctx.download(self.frames_out, out)
-
-    def paste_pred(self, pred_frame: np.ndarray, idx: int) -> np.ndarray:
-        """paste_back_frame for a host prediction (160,160,3) — the reference's exact argument; own small ctx (process_frames thread)."""
-        a = self.avatar
-        p = np.ascontiguousarray(pred_frame, np.float32)
-        if p.shape != (FACE, FACE, 3):
-            raise ValueError(f"paste_pred: prediction must be ({FACE},{FACE},3), got {p.shape}")
-        if not 0 <= idx < a.n:
-            raise ValueError("paste_pred: idx out of range")
-        if self._paste_ctx is None:
-            self._paste_ctx = self.new_ctx()
-            self._pred_scratch = self._paste_ctx.alloc((1, FACE, FACE, 3), np.float32)
-            self._paste_out = self._paste_ctx.alloc((a.H, a.W, 3), np.uint8)
-        pc = self._paste_ctx
-        with pc.lock:
-            pc.h2d(self._pred_scratch, p, sync=False)
-            pc.ul_paste(a.frames, a.faces, a.coords, self._pred_scratch, self._paste_out, a.n, a.H, a.W, 0, idx, 0, 1)
-            return pc.download(self._paste_out)
-
-    def step_async(self, index: int):
-        self.infer_async(index, None)
-        self.paste_batch_async(index)
-
-
 class UltraLightBatchSession(GraphSession):
     """Cross-session batching for UltraLight: up to G sessions x Bs frames run as ONE captured prep + U-Net + head graph of batch
     G*Bs.  A *group request* is (UltraLightAvatar, first frame index, HuBERT features (Bs, 16, 1024) or None = resident).  Each
     avatar brings its own network: the graph's ops are grouped, group g reads the weights of bank slot group_slot[g] and its crops
     from its own avatar (a per-group prep descriptor), both device tables written before every launch.  Groups beyond the
     requests of a call keep their last slot and a blank crop source; their output is discarded.  `batch` / `infer_slots` make it a
-    mux for plugin.batcher.CrossSessionBatcher; infer_groups returns composited frames, or float32 predictions with return_pred."""
+    mux for plugin.batcher.CrossSessionBatcher; infer_groups returns composited frames, or float32 predictions with return_pred.
+
+    avatar: bind the session to this one avatar (groups = 1).  There is no bank then: the graph runs the avatar's own network on
+    the ungrouped ops, its crops indexed by the d_index scalar, and its output frames are allocated here.
+    keep_taps: `taps` holds intermediate activations of the U-Net (else None)."""
 
     def __init__(self, template: UltraLightModel, groups: int, frames_per_session: int, slots: Optional[int] = None,
-                 return_pred: bool = False, ctx: Optional[Ctx] = None):
+                 return_pred: bool = False, *, ctx: Optional[Ctx] = None, keep_taps: bool = False,
+                 avatar: Optional[UltraLightAvatar] = None):
         super().__init__(ctx)
-        self.G, self.Bs, self.return_pred = int(groups), int(frames_per_session), bool(return_pred)
+        self.G, self.Bs, self.return_pred, self.avatar = int(groups), int(frames_per_session), bool(return_pred), avatar
         self.batch = self.G                                  # CrossSessionBatcher: requests per engine call
         self.B = B = self.G * self.Bs
         try:
             ctx = self.ctx
-            self.bank = UltraLightBank(ctx, template, slots if slots is not None else 2 * self.G, alloc=self.alloc)
-            if self.bank.slots < self.G:
-                raise ValueError(f"the bank needs at least {self.G} slots")
-            self.d_slot = self.alloc((self.G,), np.int32, zero=True)
-            self._slot_host = np.zeros(self.G, np.int32)
-            self._blank = self.alloc((1, CROP, CROP, 3), np.uint8, zero=True)      # crop source of the groups a call leaves empty
-            self._prep = [(self._blank, 1, 0)] * self.G
-            table = ul_prep_table(self._prep)
-            self.d_prep = self.alloc(table.shape, table.dtype)
-            ctx.h2d(self.d_prep, table)
-            self.audio16 = self.alloc((B, 32, 32, 16), np.float16, zero=True)
+            if avatar is not None:
+                if self.G != 1:
+                    raise ValueError("a session bound to an avatar has one group")
+                self.d_index = self.alloc((4,), np.int32, zero=True)
+            else:
+                self.bank = UltraLightBank(ctx, template, slots if slots is not None else 2 * self.G, alloc=self.alloc)
+                if self.bank.slots < self.G:
+                    raise ValueError(f"the bank needs at least {self.G} slots")
+                self.d_slot = self.alloc((self.G,), np.int32, zero=True)
+                self._slot_host = np.zeros(self.G, np.int32)
+                self._blank = self.alloc((1, CROP, CROP, 3), np.uint8, zero=True)      # crop source of the groups a call leaves empty
+                self._prep = [(self._blank, 1, 0)] * self.G
+                table = ul_prep_table(self._prep)
+                self.d_prep = self.alloc(table.shape, table.dtype)
+                ctx.h2d(self.d_prep, table)
+            self.audio16 = self.alloc((B, 32, 32, 16), np.float16, zero=True)           # NHWC view of audiofeat.reshape(16, 32, 32)
             self.img16 = self.alloc((B, FACE, FACE, 16), np.float16, zero=True)
             self.pred = self.alloc((B, FACE, FACE, 3), np.float32, zero=True)
-            self._audio_host = np.zeros((B, 1024, 16), np.float16)
             self._frames_out: Dict[tuple, DevTensor] = {}
-            grp = _Grouping(self.bank, self.d_slot, self.Bs)
+            if avatar is not None:
+                self.frames_out = self._out(0, avatar)
+            self.taps = {} if keep_taps else None
+            self._audio_host = np.zeros((B, 1024, 16), np.float16)
 
             def emit(b: Builder):
-                ctx.ul_prep_grouped(self.d_prep, self.Bs, B, self.img16)
-                template.emit(b, self.img16, self.audio16, self.pred, None, grp)
+                if avatar is not None:
+                    ctx.ul_prep(avatar.faces, avatar.n, self.d_index, B, self.img16)
+                    avatar.model.emit(b, self.img16, self.audio16, self.pred, self.taps)
+                else:
+                    ctx.ul_prep_grouped(self.d_prep, self.Bs, B, self.img16)
+                    template.emit(b, self.img16, self.audio16, self.pred, self.taps, _Grouping(self.bank, self.d_slot, self.Bs))
 
             self.capture(emit)
         except BaseException:
@@ -373,32 +300,42 @@ class UltraLightBatchSession(GraphSession):
     def _check(self, requests):
         if not 1 <= len(requests) <= self.G:
             raise ValueError(f"1..{self.G} group requests per call, got {len(requests)}")
+        if self.avatar is not None and requests[0][0] is not self.avatar:
+            raise ValueError("the session is bound to another avatar")
 
-    def infer_async(self, requests: Sequence[tuple]):
-        """requests[g] = (UltraLightAvatar, first frame index, features (Bs,16,1024) | None = resident in audio16 rows of group g)."""
+    def _launch(self, requests: Sequence[tuple]):
+        """requests[g] = (UltraLightAvatar, first frame index, features (Bs,16,1024) | None = resident in audio16 rows of group g):
+        stage the features, write the frame index (bound avatar) or the slot and prep tables, launch the graph."""
+        if self.graph is None:
+            raise RuntimeError(f"{type(self).__name__}: paste-only (or closed) session has no network graph")
         self._check(requests)
         ctx, Bs = self.ctx, self.Bs
-        keep: List[int] = []
         stage = False
         for g, (av, index, feats) in enumerate(requests):
-            s = self.bank.slot_of(av.model, keep)
-            keep.append(s)
-            self._slot_host[g] = s
-            self._prep[g] = (av.faces, av.n, int(index))
             if feats is not None:
                 a = np.asarray(feats, np.float32)
                 if a.shape != (Bs, 16, 1024):
-                    raise ValueError(f"group features must be ({Bs},16,1024), got {a.shape}")
+                    raise ValueError(f"audio features must be ({Bs},16,1024), got {a.shape}")
                 self._audio_host[g * Bs:(g + 1) * Bs] = a.transpose(0, 2, 1)
                 stage = True
-        for g in range(len(requests), self.G):
-            self._prep[g] = (self._blank, 1, 0)
-        ctx.h2d(self.d_slot, self._slot_host, sync=False)
-        ctx.h2d(self.d_prep, ul_prep_table(self._prep), sync=False)
         if stage:
-            n = len(requests) * Bs
-            ctx.h2d(self.audio16, self._audio_host[:n], sync=False)
+            ctx.h2d(self.audio16, self._audio_host[:len(requests) * Bs], sync=False)
+        if self.avatar is not None:
+            ctx.set_i32(self.d_index, int(requests[0][1]))
+        else:
+            keep: List[int] = []
+            for g, (av, index, _f) in enumerate(requests):
+                s = self.bank.slot_of(av.model, keep)
+                keep.append(s)
+                self._slot_host[g] = s
+                self._prep[g] = (av.faces, av.n, int(index))
+            for g in range(len(requests), self.G):
+                self._prep[g] = (self._blank, 1, 0)
+            ctx.h2d(self.d_slot, self._slot_host, sync=False)
+            ctx.h2d(self.d_prep, ul_prep_table(self._prep), sync=False)
         self.graph.launch()
+
+    infer_async = _launch
 
     def _out(self, g: int, av: UltraLightAvatar) -> DevTensor:
         key = (g, av.H, av.W)
@@ -417,14 +354,14 @@ class UltraLightBatchSession(GraphSession):
         return outs
 
     def step_async(self, requests: Sequence[tuple]):
-        self.infer_async(requests)
+        self._launch(requests)
         self.paste_async(requests)
 
     def infer_groups(self, requests: Sequence[tuple]) -> List[np.ndarray]:
         """-> per request its (Bs, H, W, 3) uint8 composited frames, or with return_pred its float32 (Bs, 160, 160, 3) predictions
         (what LightReal.inference_batch returns for that session)."""
         with self.ctx.lock:
-            self.infer_async(requests)
+            self._launch(requests)
             if self.return_pred:
                 n = len(requests) * self.Bs
                 pred = self.ctx.download(DevTensor(self.pred.ptr, (n, FACE, FACE, 3), np.float32))
@@ -434,6 +371,67 @@ class UltraLightBatchSession(GraphSession):
             return outs
 
     infer_slots = infer_groups
+
+
+class UltraLightSession(UltraLightBatchSession):
+    """One avatar stream at a fixed batch size: UltraLightBatchSession with one group, bound to `avatar` (its own network on the
+    ungrouped ops)."""
+
+    def __init__(self, avatar: UltraLightAvatar, batch: int, keep_taps: bool = False, ctx: Optional[Ctx] = None, paste_only: bool = False):
+        """paste_only: no ctx, network graph or activation arena — only paste_pred() works (cross-session mode: this session's
+        U-Net pass runs in a shared UltraLightBatchSession)."""
+        if paste_only:
+            GraphSession.__init__(self, ctx, with_ctx=False)
+            self.avatar, self.B = avatar, int(batch)
+            return
+        super().__init__(avatar.model, 1, batch, ctx=ctx, keep_taps=keep_taps, avatar=avatar)
+
+    # ---- LightReal.inference_batch (ultralight_avatar.py:141-169)
+    def infer_async(self, index: int, audio_feats: Optional[np.ndarray] = None):
+        """audio_feats: (B, 16, 1024) float (the HubertASR windows) or None when audio16 is already resident."""
+        self._launch([(self.avatar, index, audio_feats)])
+
+    def infer(self, index: int, audio_feats: Optional[np.ndarray] = None, want_pred: bool = True):
+        with self.ctx.lock:
+            self.infer_async(index, audio_feats)
+            if want_pred:
+                return self.ctx.download(self.pred)              # float32 (B,160,160,3) = pred * 255, as the reference returns
+            self.ctx.sync()
+            return None
+
+    # ---- LightReal.paste_back_frame (ultralight_avatar.py:171-184)
+    def paste_batch_async(self, index: int):
+        self.paste_async([(self.avatar, index, None)])
+
+    def paste_batch(self, index: int, out: Optional[np.ndarray] = None) -> np.ndarray:
+        with self.ctx.lock:
+            self.paste_batch_async(index)
+            return self.ctx.download(self.frames_out, out)
+
+    def infer_paste(self, index: int, audio_feats: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """inference_batch + B x paste_back_frame as one engine round: (B, H, W, 3) uint8 composited frames."""
+        with self.ctx.lock:
+            self.infer_async(index, audio_feats)
+            self.paste_batch_async(index)
+            return self.ctx.download(self.frames_out, out)
+
+    def paste_pred(self, pred_frame: np.ndarray, idx: int) -> np.ndarray:
+        """paste_back_frame for a host prediction (160,160,3) — the reference's exact argument, on the session's paste ctx."""
+        a = self.avatar
+        p = np.ascontiguousarray(pred_frame, np.float32)
+        if p.shape != (FACE, FACE, 3):
+            raise ValueError(f"paste_pred: prediction must be ({FACE},{FACE},3), got {p.shape}")
+        if not 0 <= idx < a.n:
+            raise ValueError("paste_pred: idx out of range")
+        pc, pred, out = self.paste_ctx((1, FACE, FACE, 3), np.float32, (a.H, a.W, 3))
+        with pc.lock:
+            pc.h2d(pred, p, sync=False)
+            pc.ul_paste(a.frames, a.faces, a.coords, pred, out, a.n, a.H, a.W, 0, idx, 0, 1)
+            return pc.download(out)
+
+    def step_async(self, index: int):
+        self.infer_async(index, None)
+        self.paste_batch_async(index)
 
 
 def unet_gflop_per_frame() -> float:
