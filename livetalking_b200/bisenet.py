@@ -28,19 +28,14 @@ from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 
-from .graph import GraphSession
-from .ops import ConvWeight, Ctx, DevTensor
+from .layerplan import Layer, LayerSession, Step, _f64, check_fp16_margin, fp16_weights
+from .ops import Ctx
 
 INPUT, S2D, IN_C = 512, 259, 16
 N_CLASSES, OUT_C = 19, 32
 BN_EPS = 1e-5
-FP16_LIMIT = 2.0 ** 14
 # (layer, blocks, cin, cout, stride, output map size) of Resnet18 at 512 x 512
 LAYERS = [("layer1", 2, 64, 64, 1, 128), ("layer2", 2, 64, 128, 2, 64), ("layer3", 2, 128, 256, 2, 32), ("layer4", 2, 256, 512, 2, 16)]
-
-
-def _f64(t) -> np.ndarray:
-    return t.detach().cpu().double().numpy() if hasattr(t, "detach") else np.asarray(t, np.float64)
 
 
 def _fold(sd, wk: str, bn: Optional[str]) -> Tuple[np.ndarray, np.ndarray]:
@@ -49,13 +44,6 @@ def _fold(sd, wk: str, bn: Optional[str]) -> Tuple[np.ndarray, np.ndarray]:
         return w, np.zeros(w.shape[0])
     s = _f64(sd[bn + ".weight"]) / np.sqrt(_f64(sd[bn + ".running_var"]) + BN_EPS)
     return w * s[:, None, None, None], _f64(sd[bn + ".bias"]) - _f64(sd[bn + ".running_mean"]) * s
-
-
-def _check(name: str, *arrs):
-    for a in arrs:
-        m = float(np.abs(a).max(initial=0.0))
-        if not m < FP16_LIMIT:
-            raise ValueError(f"BiSeNet {name}: largest folded value {m:g} leaves less than a 4x margin to the fp16 range")
 
 
 def s2d_stem(w7: np.ndarray) -> np.ndarray:
@@ -70,20 +58,6 @@ def s2d_stem(w7: np.ndarray) -> np.ndarray:
                     if 0 <= ky < 7 and 0 <= kx < 7:
                         w4[:, (by * 2 + bx) * 3: (by * 2 + bx) * 3 + 3, a, b] = w7[:, :, ky, kx]
     return w4
-
-
-class Layer:
-    """One planner conv: w the fp16-rounded kernel as float32 [cout, cin, k, k], b fp32 [cout]; src / dst / res: (buffer, c_off, C)
-    (res None: no residual).  up: nearest 2x upsample fused in front (ConvWeight.upconv)."""
-
-    def __init__(self, name, w, b, stride, relu, src, dst, res=None, up=False):
-        self.name, self.w, self.b, self.stride, self.relu = name, w, b, stride, relu
-        self.src, self.dst, self.res, self.up = src, dst, res, up
-        self.dev: Optional[ConvWeight] = None
-
-    @property
-    def pad(self) -> int:
-        return 0 if self.name == "stem" else self.w.shape[-1] // 2
 
 
 class Gate:
@@ -117,16 +91,16 @@ def plan(sd) -> Tuple[List[Layer], Dict[str, Gate], Dict[str, Tuple[int, int, in
     layers: List[Layer] = []
     bufs = {"in": (S2D, S2D, IN_C)}
 
-    def conv(name, wk, bn, stride, relu, src, dst, res=None, up=False, w64=None):
+    def conv(name, wk, bn, stride, relu, src, dst, res=None, up=False, w64=None, pad=None):
         w, b = _fold(sd, wk, bn)
         if w64 is not None:
             w = w64(w)
             b = np.concatenate([b, np.zeros(w.shape[0] - b.shape[0])])
-        _check(name, w, b)
-        layers.append(Layer(name, w.astype(np.float16).astype(np.float32), b.astype(np.float32), stride, relu, src, dst, res, up))
+        w, b = fp16_weights(f"BiSeNet {name}", w, b)
+        layers.append(Layer(name, "conv", w, b, stride, w.shape[-1] // 2 if pad is None else pad, relu, src, dst, res, up))
 
     bufs["stem"] = (256, 256, 64)
-    conv("stem", "cp.resnet.conv1.weight", "cp.resnet.bn1", 1, True, ("in", 0, IN_C), ("stem", 0, 64), w64=s2d_stem)
+    conv("stem", "cp.resnet.conv1.weight", "cp.resnet.bn1", 1, True, ("in", 0, IN_C), ("stem", 0, 64), w64=s2d_stem, pad=0)
     bufs["pool"] = (128, 128, 64)
     cur = ("pool", 0, 64)
     for name, nb, cin, cout, s, hw in LAYERS:
@@ -174,10 +148,10 @@ def plan(sd) -> Tuple[List[Layer], Dict[str, Gate], Dict[str, Tuple[int, int, in
 
     def gate(name, wk, bn, act, *second):
         w, b = _fold(sd, wk, bn)
-        _check(name, w, b)
+        check_fp16_margin(f"BiSeNet {name}", w, b)
         if second:
             w2 = _f64(sd[second[0]])
-            _check(name, w2)
+            check_fp16_margin(f"BiSeNet {name}", w2)
             gates[name] = Gate(name, w, None, Ctx.ACT_RELU, w2, None, act)
         else:
             gates[name] = Gate(name, w, b, act)
@@ -202,9 +176,7 @@ class BiSeNetNet:
         layers, gates, bufs = plan(sd)
         ctx = ctx or Ctx()
         for L in layers:
-            L.dev = ConvWeight(ctx, L.w, L.b)
-            if L.up:
-                L.dev.upconv(ctx)
+            L.upload(ctx)
         for g in gates.values():
             g.dev = tuple(None if a is None else ctx.upload(a) for a in (g.w1t, g.b1, g.w2t, g.b2))
         net = cls(ctx, layers, gates, bufs)
@@ -212,86 +184,37 @@ class BiSeNetNet:
         return net
 
 
-class BiSeNetParser(GraphSession):
-    """One captured graph for batches of N RGB crops of 512 x 512.  Every conv writes its own buffer (the layer tests read them)."""
+class BiSeNetParser(LayerSession):
+    """One captured graph for batches of N RGB crops of 512 x 512.  Every conv writes its own buffer (the layer tests read them);
+    labels: the u8 [N, 512, 512] label map the graph writes."""
 
     def __init__(self, net: BiSeNetNet, N: int, ctx: Optional[Ctx] = None):
-        super().__init__(ctx)
-        self.net, self.N = net, int(N)
-        try:
-            self._build()
-        except BaseException:
-            self.close()
-            raise
+        self.net, N = net, int(N)
+        bufs = {"rgb": ((N, INPUT, INPUT, 3), np.uint8), **{name: ((N,) + hwc, np.float16) for name, hwc in net.bufs.items()},
+                **{name: ((N, (g.w1t if g.w2t is None else g.w2t).shape[1]), np.float32) for name, g in net.gates.items()},
+                "labels": ((N, INPUT, INPUT), np.uint8)}
 
-    def _build(self):
-        N, net = self.N, self.net
-        self.rgb = self.alloc((N, INPUT, INPUT, 3), np.uint8, zero=True)
-        self.buf = {name: self.alloc((N, h, w, c), zero=True) for name, (h, w, c) in net.bufs.items()}
-        self.vec = {name: self.alloc((N, g.w2t.shape[1] if g.w2t is not None else g.w1t.shape[1]), np.float32, zero=True)
-                    for name, g in net.gates.items()}
-        self.labels = self.alloc((N, INPUT, INPUT), np.uint8, zero=True)
-        conv = {L.name: L for L in net.layers}
-        self.ops = [("prep", None)]
+        def gate(name, src):
+            g = net.gates[name]
+            return Step(name, run=lambda s, x, y: s.ctx.chan_gate(s.buf[src], s.N, g.dev[0], g.dev[1], g.act1, s.buf[name], g.dev[2],
+                                                                  g.dev[3], g.act2))
+
+        def scale_add(src, g, out, **y):            # out = src * gate g + (yvec: a gate vector, y: a map, neither: src)
+            return Step(out, run=lambda s, x_, y_: s.ctx.chan_scale_add(s.buf[src], s.N, s.buf[g], s.buf[out],
+                                                                         **{k: s.buf[v] for k, v in y.items()}))
+        before = {"cp.resnet.layer1.0.conv1": [Step("pool", src=("stem", 0, 64), dst=("pool", 0, 64),
+                                                    run=lambda s, x, y: s.ctx.maxpool3x3s2(x, s.N, 256, 256, y))],
+                  "arm32": [gate("avg", "cp.resnet.layer4.1")]}
+        after = {"arm32": [gate("att32", "arm32"), scale_add("arm32", "att32", "sum32", yvec="avg")],
+                 "arm16": [gate("att16", "arm16"), scale_add("arm16", "att16", "sum16", y="head32")],
+                 "ffm": [gate("attffm", "ffm"), scale_add("ffm", "attffm", "fuse")]}
+        steps = [Step("prep", src=("rgb", 0, 3), dst=("in", 0, IN_C), run=lambda s, x, y: s.ctx.bisenet_prep(x, s.N, y))]
         for L in net.layers:
-            if L.name == "cp.resnet.layer1.0.conv1":
-                self.ops.append(("pool", None))
-            if L.name == "arm32":
-                self.ops.append(("gate", ("avg", "cp.resnet.layer4.1")))
-            self.ops.append(("conv", L))
-            if L.name == "arm32":
-                self.ops += [("gate", ("att32", "arm32")), ("scale_add", ("arm32", "att32", "sum32", ("vec", "avg")))]
-            elif L.name == "arm16":
-                self.ops += [("gate", ("att16", "arm16")), ("scale_add", ("arm16", "att16", "sum16", ("map", "head32")))]
-            elif L.name == "ffm":
-                self.ops += [("gate", ("attffm", "ffm")), ("scale_add", ("ffm", "attffm", "fuse", ("self", None)))]
-        self.ops.append(("argmax", conv["classes"]))
-        self.ctx.sync()
-        with self.ctx.capture() as g:
-            for op in self.ops:
-                self._run(op)
-        self.graph = g.graph
-
-    def view(self, ref) -> DevTensor:
-        """(buffer, c_off, C) -> the channel-slice view."""
-        name, c_off, C = ref
-        t = self.buf[name]
-        n, h, w, pitch = t.shape
-        return DevTensor(t.ptr, (n, h, w, C), pitch=pitch, c_off=c_off)
-
-    def _conv_kw(self, L: Layer) -> dict:
-        x, y = self.view(L.src), self.view(L.dst)
-        kw = dict(N=self.N, IH=x.shape[1], IW=x.shape[2], OH=y.shape[1], OW=y.shape[2], stride=(L.stride, L.stride), pad=(L.pad, L.pad),
-                  relu=L.relu, upsample2x=L.up)
-        if L.res is not None:
-            kw["res"] = self.view(L.res)
-        return kw
-
-    def _run(self, op):
-        kind, a = op
-        ctx, N = self.ctx, self.N
-        if kind == "prep":
-            ctx.bisenet_prep(self.rgb, N, self.buf["in"])
-        elif kind == "pool":
-            ctx.maxpool3x3s2(self.buf["stem"], N, 256, 256, self.buf["pool"])
-        elif kind == "conv":
-            ctx.conv(self.view(a.src), a.dev, self.view(a.dst), **self._conv_kw(a))
-        elif kind == "gate":
-            g, src = self.net.gates[a[0]], a[1]
-            w1t, b1, w2t, b2 = g.dev
-            ctx.chan_gate(self.buf[src], N, w1t, b1, g.act1, self.vec[a[0]], w2t, b2, g.act2)
-        elif kind == "scale_add":
-            x, g, out, (ykind, y) = a
-            kw = {"yvec": self.vec[y]} if ykind == "vec" else ({"y": self.buf[y]} if ykind == "map" else {})
-            ctx.chan_scale_add(self.buf[x], N, self.vec[g], self.buf[out], **kw)
-        elif kind == "argmax":
-            ctx.bisenet_upsample_argmax(self.view(a.dst), N, N_CLASSES, self.labels)
-        else:
-            raise ValueError(kind)
-
-    def conv_variants(self) -> dict:
-        """name -> the kernel instance (Ctx.conv_plan) each planner conv runs in this graph."""
-        return {L.name: self.ctx.conv_plan(self.view(L.src), L.dev, self.view(L.dst), **self._conv_kw(L)) for L in self.net.layers}
+            steps += before.get(L.name, []) + [Step(L.name, L)] + after.get(L.name, [])
+        steps.append(Step("argmax", src=("logits", 0, OUT_C),
+                          run=lambda s, x, y: s.ctx.bisenet_upsample_argmax(x, s.N, N_CLASSES, s.buf["labels"])))
+        super().__init__(N, bufs, steps, ctx, zero=True)
+        self.labels = self.buf["labels"]
 
     def parse(self, rgb512_u8: np.ndarray) -> np.ndarray:
         """u8 RGB [n <= N, 512, 512, 3] (FaceParsing's PIL resize of each crop) -> u8 labels [n, 512, 512]."""
@@ -299,10 +222,4 @@ class BiSeNetParser(GraphSession):
         n = x.shape[0]
         if x.shape[1:] != (INPUT, INPUT, 3) or not 1 <= n <= self.N:
             raise ValueError(f"expected up to {self.N} RGB crops of 512x512x3, got {x.shape}")
-        if n < self.N:   # images are independent: pad with copies of the last crop
-            x = np.concatenate([x, np.repeat(x[-1:], self.N - n, 0)], 0)
-        with self.ctx.lock:
-            self.ctx.h2d(self.rgb, x)
-            self.graph.launch()
-            out = self.ctx.download(self.labels)
-        return out[:n]
+        return self.replay({"rgb": x}, ("labels",))[0]

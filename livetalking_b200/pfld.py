@@ -34,12 +34,12 @@ from typing import List, Optional, Tuple
 
 import numpy as np
 
-from .graph import GraphSession, _ceil16
-from .ops import ConvWeight, Ctx, DevTensor
+from .graph import _ceil16
+from .layerplan import Layer, LayerSession, Step, _f64, fp16_weights
+from .ops import Ctx
 
 INPUT, LANDMARKS, IN_C = 192, 110, 16
 BRANCHES, BN_EPS = 6, 1e-5
-FP16_LIMIT = 2.0 ** 14
 # GhostOneBottleneck(in, hidden, out, stride) of PFLD_GhostOne at width_factor 0.5 (pfld_mobileone.py:59-72)
 BOTTLENECKS = [("conv3_1", 32, 48, 40, 2), ("conv3_2", 40, 60, 40, 1), ("conv3_3", 40, 60, 40, 1),
                ("conv4_1", 40, 100, 48, 2), ("conv4_2", 48, 120, 48, 1), ("conv4_3", 48, 120, 48, 1),
@@ -72,10 +72,6 @@ def _blocks():
     return out
 
 
-def _f64(t) -> np.ndarray:
-    return t.detach().cpu().double().numpy() if hasattr(t, "detach") else np.asarray(t, np.float64)
-
-
 def fold_block(sd, p: str, cin: int, cout: int, k: int, groups: int) -> Tuple[np.ndarray, np.ndarray]:
     """MobileOneBlock._get_kernel_bias in float64 (or p.reparam_conv as stored) -> (kernel [cout, cin/groups, k, k], bias [cout])."""
     if p + ".reparam_conv.weight" in sd:
@@ -103,30 +99,6 @@ def fold_block(sd, p: str, cin: int, cout: int, k: int, groups: int) -> Tuple[np
     return kern, bias
 
 
-class Layer:
-    """One device op of the plan: kind 'conv' (planner) or 'dw' (dwconv3x3).  w: the padded kernel in PyTorch layout, fp16-rounded
-    values as float32 ([cout_p, cin_p, k, k], or [C_p, 1, 3, 3] for 'dw'); b: fp32 [cout_p].  src / dst: (buffer, c_off, C)."""
-
-    def __init__(self, name, kind, w, b, stride, relu, src, dst):
-        self.name, self.kind, self.w, self.b, self.stride, self.relu, self.src, self.dst = name, kind, w, b, stride, relu, src, dst
-        self.dev = None
-
-
-def _half(w64: np.ndarray, name: str) -> np.ndarray:
-    m = float(np.abs(w64).max()) if w64.size else 0.0
-    if not m < FP16_LIMIT:
-        raise ValueError(f"PFLD {name}: largest folded weight {m:g} leaves less than a 4x margin to the fp16 range")
-    return w64.astype(np.float16).astype(np.float32)          # one rounding float64 -> fp16
-
-
-def _bias(b64: np.ndarray, n: int, idx, name: str) -> np.ndarray:
-    if np.abs(b64).max(initial=0.0) >= FP16_LIMIT:
-        raise ValueError(f"PFLD {name}: a folded bias leaves less than a 4x margin to the fp16 range")
-    b = np.zeros(n, np.float32)
-    b[idx] = b64.astype(np.float32)
-    return b
-
-
 def plan(sd) -> Tuple[List[Layer], dict, list]:
     """Host-side plan from a PFLD_GhostOne state dict: (layers, buffers {name: (H, W, pitch)}, taps [(buffer, real channel list)] x 5).
     Buffer 'in' is the prepared crop [192, 192, 16], 'c7' conv7's output [12, 12, 16] which conv8 reads as [1, 1, 2304]."""
@@ -137,19 +109,19 @@ def plan(sd) -> Tuple[List[Layer], dict, list]:
 
     def dense(name, src, src_idx, dst, relu):
         _, cin, cout, k, s, g, _ = blocks[name]
-        w64, b64 = fold_block(sd, name, cin, cout, k, g)
+        w16, b32 = fp16_weights(f"PFLD {name}", *fold_block(sd, name, cin, cout, k, g))
         cin_p, cout_p = bufs[src][2], _ceil16(cout)
-        w = np.zeros((cout_p, cin_p, k, k), np.float32)
-        w[:cout, src_idx] = _half(w64, name)
-        layers.append(Layer(name, "conv", w, _bias(b64, cout_p, slice(0, cout), name), s, relu, (src, 0, cin_p), (dst, 0, cout_p)))
+        w, b = np.zeros((cout_p, cin_p, k, k), np.float32), np.zeros(cout_p, np.float32)
+        w[:cout, src_idx], b[:cout] = w16, b32
+        layers.append(Layer(name, "conv", w, b, s, k // 2, relu, (src, 0, cin_p), (dst, 0, cout_p)))
         return list(range(cout))
 
     def depthwise(name, buf, c_in, c_out, idx, C, relu):
         _, cin, cout, k, s, g, _ = blocks[name]
-        w64, b64 = fold_block(sd, name, cin, cout, k, g)
-        w = np.zeros((C, 1, 3, 3), np.float32)
-        w[idx] = _half(w64, name)
-        layers.append(Layer(name, "dw", w, _bias(b64, C, idx, name), s, relu, (buf[0], c_in, C), (buf[1], c_out, C)))
+        w16, b32 = fp16_weights(f"PFLD {name}", *fold_block(sd, name, cin, cout, k, g))
+        w, b = np.zeros((C, 1, 3, 3), np.float32), np.zeros(C, np.float32)
+        w[idx], b[idx] = w16, b32
+        layers.append(Layer(name, "dw", w, b, s, 1, relu, (buf[0], c_in, C), (buf[1], c_out, C)))
 
     H = INPUT // 2
     bufs["c1"] = (H, H, 32)
@@ -187,8 +159,8 @@ def plan(sd) -> Tuple[List[Layer], dict, list]:
     k8 = w8.shape[-1]
     assert w8.shape == (64, 16, H, H) and k8 == H, w8.shape
     bufs["x5"] = (1, 1, 64)
-    layers.append(Layer("conv8", "conv", _half(w8.transpose(0, 2, 3, 1).reshape(64, -1, 1, 1), "conv8"), np.zeros(64, np.float32), 1, True,
-                        ("c7", 0, H * H * 16), ("x5", 0, 64)))
+    w8, b8 = fp16_weights("PFLD conv8", w8.transpose(0, 2, 3, 1).reshape(64, -1, 1, 1), np.zeros(64))
+    layers.append(Layer("conv8", "conv", w8, b8, 1, 0, True, ("c7", 0, H * H * 16), ("x5", 0, 64)))
     taps.append(("x5", list(range(64))))
     return layers, bufs, taps
 
@@ -211,11 +183,7 @@ class PFLDNet:
             raise ValueError(f"PFLD: mean_face {mean.shape} / conv_out {wo.shape} do not match 110 landmarks over 256 features")
         ctx = ctx or Ctx()
         for L in layers:
-            if L.kind == "conv":
-                L.dev = ConvWeight(ctx, L.w, L.b)
-            else:
-                C = L.w.shape[0]
-                L.dev = (ctx.upload(np.ascontiguousarray(L.w.reshape(C, 9).T).astype(np.float16)), ctx.upload(L.b))
+            L.upload(ctx)
         wt = ctx.upload(np.ascontiguousarray(wo.T).astype(np.float32))
         bias = ctx.upload(_f64(sd["conv_out.bias"]).astype(np.float32))
         net = cls(ctx, layers, bufs, taps, wt, bias, ctx.upload(mean))
@@ -223,68 +191,20 @@ class PFLDNet:
         return net
 
 
-class PFLDLandmarker(GraphSession):
+class PFLDLandmarker(LayerSession):
     """One captured graph for batches of N crops of 192 x 192.  Every layer writes its own buffer (the layer tests read them)."""
 
     def __init__(self, net: PFLDNet, N: int, ctx: Optional[Ctx] = None):
-        super().__init__(ctx)
-        self.net, self.N = net, int(N)
-        try:
-            self._build()
-        except BaseException:
-            self.close()
-            raise
-
-    def _build(self):
-        N, net = self.N, self.net
-        self.crops = self.alloc((N, INPUT, INPUT, 3), np.uint8, zero=True)
-        self.crop_wh = self.alloc((N, 2), np.int32, zero=True)
-        self.buf = {name: self.alloc((N, h, w, c), zero=True) for name, (h, w, c) in net.bufs.items()}
-        self.out_f = self.alloc((N, 2 * LANDMARKS), np.float32, zero=True)
-        self.out_i = self.alloc((N, 2 * LANDMARKS), np.int32, zero=True)
-        self.ops = [("prep", None, self.crops, self.buf["in"])]
-        for L in net.layers:
-            self.ops.append((L.kind, L, self.view(L.src), self.view(L.dst)))
-        self.ops.append(("head", None, None, self.out_f))
-        self.ctx.sync()
-        with self.ctx.capture() as g:
-            for op in self.ops:
-                self._run(op)
-        self.graph = g.graph
-
-    def view(self, ref) -> DevTensor:
-        """(buffer, c_off, C) -> the channel-slice view; conv8's source is conv7's map seen as [N, 1, 1, 2304]."""
-        name, c_off, C = ref
-        t = self.buf[name]
-        n, h, w, pitch = t.shape
-        if C > pitch:
-            return DevTensor(t.ptr, (n, 1, 1, h * w * pitch))
-        return DevTensor(t.ptr, (n, h, w, C), pitch=pitch, c_off=c_off)
-
-    def _conv_kw(self, L: Layer, x: DevTensor, y: DevTensor) -> dict:
-        k = L.w.shape[-1]
-        return dict(N=self.N, IH=x.shape[1], IW=x.shape[2], OH=y.shape[1], OW=y.shape[2], stride=(L.stride, L.stride), pad=(k // 2, k // 2),
-                    relu=L.relu)
-
-    def _run(self, op):
-        kind, L, x, y = op
-        ctx = self.ctx
-        if kind == "prep":
-            ctx.pfld_prep(x, self.N, INPUT, INPUT, y)
-        elif kind == "conv":
-            ctx.conv(x, L.dev, y, **self._conv_kw(L, x, y))
-        elif kind == "dw":
-            ctx.dwconv3x3(x, self.N, x.shape[1], x.shape[2], L.dev[0], L.dev[1], L.stride, L.relu, y)
-        elif kind == "head":
-            taps = [self.buf[name] for name, _ in self.net.taps]
-            ctx.pfld_head(taps, [c for _, c in self.net.taps], self.N, self.net.wt, self.net.bias, self.net.mean, self.crop_wh, self.out_f,
-                          self.out_i)
-        else:
-            raise ValueError(kind)
-
-    def conv_variants(self) -> dict:
-        """name -> the kernel instance (Ctx.conv_plan) each planner conv runs in this graph."""
-        return {L.name: self.ctx.conv_plan(x, L.dev, y, **self._conv_kw(L, x, y)) for kind, L, x, y in self.ops if kind == "conv"}
+        self.net, N = net, int(N)
+        bufs = {"crops": ((N, INPUT, INPUT, 3), np.uint8), "crop_wh": ((N, 2), np.int32),
+                **{name: ((N,) + hwc, np.float16) for name, hwc in net.bufs.items()},
+                "out_f": ((N, 2 * LANDMARKS), np.float32), "out_i": ((N, 2 * LANDMARKS), np.int32)}
+        taps, chans = [name for name, _ in net.taps], [c for _, c in net.taps]
+        steps = [Step("prep", src=("crops", 0, 3), dst=("in", 0, IN_C), run=lambda s, x, y: s.ctx.pfld_prep(x, s.N, INPUT, INPUT, y)),
+                 *[Step(L.name, L) for L in net.layers],
+                 Step("head", run=lambda s, x, y: s.ctx.pfld_head([s.buf[t] for t in taps], chans, s.N, net.wt, net.bias, net.mean,
+                                                                  s.buf["crop_wh"], s.buf["out_f"], s.buf["out_i"]))]
+        super().__init__(N, bufs, steps, ctx, zero=True)
 
     def run(self, crops_u8: np.ndarray, crop_wh) -> Tuple[np.ndarray, np.ndarray]:
         """crops u8 BGR [n <= N, 192, 192, 3] (cv2.resize of the face crops), crop_wh [n, 2] = the crops' width and height before the
@@ -294,13 +214,5 @@ class PFLDLandmarker(GraphSession):
         n = crops_u8.shape[0]
         if crops_u8.shape[1:] != (INPUT, INPUT, 3) or not 1 <= n <= self.N or wh.shape[0] != n:
             raise ValueError(f"expected up to {self.N} crops of 192x192x3 and their sizes, got {crops_u8.shape} / {wh.shape}")
-        if n < self.N:   # images are independent: pad with copies of the last crop
-            crops_u8 = np.concatenate([crops_u8, np.repeat(crops_u8[-1:], self.N - n, 0)], 0)
-            wh = np.concatenate([wh, np.repeat(wh[-1:], self.N - n, 0)], 0)
-        with self.ctx.lock:
-            self.ctx.h2d(self.crops, crops_u8)
-            self.ctx.h2d(self.crop_wh, wh)
-            self.graph.launch()
-            of = self.ctx.download(self.out_f)
-            oi = self.ctx.download(self.out_i)
-        return of[:n].reshape(n, LANDMARKS, 2), oi[:n].reshape(n, LANDMARKS, 2)
+        of, oi = self.replay({"crops": crops_u8, "crop_wh": wh}, ("out_f", "out_i"))
+        return of.reshape(n, LANDMARKS, 2), oi.reshape(n, LANDMARKS, 2)

@@ -27,8 +27,9 @@ from typing import List, Optional, Tuple
 
 import numpy as np
 
-from .graph import GraphSession, _np
-from .ops import ConvWeight, Ctx, DevTensor
+from .graph import _np
+from .layerplan import Layer, LayerSession, Step
+from .ops import Ctx
 
 IN_C = 16            # channels of the prepared image (both conv kernels need Cin >= 16)
 HEAD_C = 16          # fused conf + loc head outputs, zero-padded (the gather kernel needs Cout % 16 == 0)
@@ -75,9 +76,9 @@ def gflop_per_frame(H: int, W: int) -> float:
 
 
 class S3FDNet:
-    """Device-resident S3FD weights: trunk convs, L2Norm scales and the six fused heads."""
+    """Device-resident S3FD weights: the trunk convs and the six fused heads as Layers, and the L2Norm scales."""
 
-    def __init__(self, ctx: Ctx, convs: dict, norms: dict, heads: list):
+    def __init__(self, ctx: Ctx, convs: List[Layer], norms: dict, heads: List[Layer]):
         self.ctx, self.convs, self.norms, self.heads = ctx, convs, norms, heads
 
     @classmethod
@@ -87,21 +88,37 @@ class S3FDNet:
         if missing:
             raise KeyError(f"S3FD state dict lacks {len(missing)} keys, e.g. {missing[:3]}")
         ctx = ctx or Ctx()
-        convs = {}
+        convs, src = [], "in"
         for e in TRUNK:
             if e == "pool":
+                src += "_pool"
                 continue
-            name = e[0]
-            convs[name] = ConvWeight(ctx, _np(sd[name + ".weight"]), _np(sd[name + ".bias"]), pad_cin=IN_C if name == "conv1_1" else None)
-        norms = {src: ctx.upload(_np(sd[src + "_norm.weight"]).astype(np.float32)) for src, _, normed, _ in LEVELS if normed}
+            name, _, _, _, s, p = e
+            convs.append(_layer(name, _np(sd[name + ".weight"]), _np(sd[name + ".bias"]), s, p, True, src, name))
+            src = name
         heads = []
         for src, _, normed, _ in LEVELS:
             pre = _head_name(src, normed)
             w = np.concatenate([_np(sd[pre + "_mbox_conf.weight"]), _np(sd[pre + "_mbox_loc.weight"])], 0)
             b = np.concatenate([_np(sd[pre + "_mbox_conf.bias"]), _np(sd[pre + "_mbox_loc.bias"])], 0)
-            heads.append(ConvWeight(ctx, w, b, pad_cout=HEAD_C))
+            heads.append(_layer(pre + "_mbox", w, b, 1, 1, False, pre, pre + "_mbox"))
+        for L in convs:
+            L.upload(ctx)
+        norms = {src: ctx.upload(_np(sd[src + "_norm.weight"]).astype(np.float32)) for src, _, normed, _ in LEVELS if normed}
+        for L in heads:
+            L.upload(ctx)
         ctx.sync()
         return cls(ctx, convs, norms, heads)
+
+
+def _layer(name, w, b, stride, pad, relu, src, dst) -> Layer:
+    """A trunk conv or head, zero-padded to at least IN_C inputs (conv1_1) and HEAD_C outputs (the heads), rounded to fp16 once."""
+    cout, cin = max(w.shape[0], HEAD_C), max(w.shape[1], IN_C)
+    wp = np.zeros((cout, cin) + w.shape[2:], np.float32)
+    wp[:w.shape[0], :w.shape[1]] = w
+    bp = np.zeros(cout, np.float32)
+    bp[:b.shape[0]] = b
+    return Layer(name, "conv", wp.astype(np.float16).astype(np.float32), bp, stride, pad, relu, (src, 0, cin), (dst, 0, cout))
 
 
 def _expected_keys():
@@ -111,102 +128,52 @@ def _expected_keys():
     return keys
 
 
-class S3FDDetector(GraphSession):
+class S3FDDetector(LayerSession):
     """One captured graph for batches of N frames of H x W.  keep_layers: every op writes its own buffer (the layer tests read
-    them back); otherwise the trunk ping-pongs between two buffers and only the six level features have their own."""
+    them back); otherwise the trunk ping-pongs between two arenas, only the six level features have their own buffers and
+    L2Norm runs in place on them."""
 
     def __init__(self, net: S3FDNet, N: int, H: int, W: int, keep_layers: bool = False, ctx: Optional[Ctx] = None):
         if H < 32 or W < 32:
             raise ValueError(f"S3FD needs frames of at least 32 x 32, got {H} x {W}")
-        super().__init__(ctx)
-        self.net, self.N, self.H, self.W = net, int(N), int(H), int(W)
-        try:
-            self._build(keep_layers)
-        except BaseException:
-            self.close()
-            raise
-
-    def _build(self, keep: bool):
-        N, H, W = self.N, self.H, self.W
-        self.frames = self.alloc((N, H, W, 3), np.uint8)
-        x0 = self.alloc((N, H, W, IN_C))
-        self.ops: List[tuple] = [("prep", "prep", self.frames, x0, {})]
+        self.net, self.H, self.W = net, int(H), int(W)
+        N, H, W = int(N), self.H, self.W
+        bufs = {"frames": ((N, H, W, 3), np.uint8), "in": ((N, H, W, IN_C), np.float16)}
+        steps = [Step("prep", src=("frames", 0, 3), dst=("in", 0, IN_C), run=lambda s, x, y: s.ctx.s3fd_prep(x, s.N, s.H, s.W, y))]
         feats = {src for src, _, _, _ in LEVELS}
-        # pass 1: shapes, so that the ping-pong buffers can be sized
-        plan, h, w, c = [], H, W, IN_C
+        arenas, nxt, convs, cur, h, w, c = {}, 0, iter(net.convs), "in", H, W, IN_C
         for e in TRUNK:
             if e == "pool":
-                plan.append(("pool", plan[-1][1] + "_pool", (N, h // 2, w // 2, c), dict(N=N, H=h, W=w)))
-                h, w = h // 2, w // 2
-                continue
-            name, _, cout, k, s, p = e
-            oh, ow = _out_dim(h, k, s, p), _out_dim(w, k, s, p)
-            plan.append(("conv", name, (N, oh, ow, cout), dict(N=N, IH=h, IW=w, OH=oh, OW=ow, stride=(s, s), pad=(p, p), relu=True)))
-            h, w, c = oh, ow, cout
-        pp = []
-        if not keep:
-            big = max(int(np.prod(shape)) for kind, name, shape, _ in plan if name not in feats)
-            pp = [self.alloc((big,)), self.alloc((big,))]
-        cur, nxt, fmap = x0, 0, {}
-        for kind, name, shape, kw in plan:
-            if keep or name in feats:
-                out = self.alloc(shape)
+                name, h, w = cur + "_pool", h // 2, w // 2
+                steps.append(Step(name, src=(cur, 0, c), dst=(name, 0, c),
+                                  run=lambda s, x, y: s.ctx.maxpool2x2(x, s.N, x.shape[1], x.shape[2], y)))
             else:
-                if cur.ptr == pp[nxt].ptr:
+                L = next(convs)
+                name, c = L.name, L.w.shape[0]
+                h, w = _out_dim(h, L.w.shape[-1], L.stride, L.pad), _out_dim(w, L.w.shape[-1], L.stride, L.pad)
+                steps.append(Step(name, L))
+            bufs[name] = ((N, h, w, c), np.float16)
+            if not keep_layers and name not in feats:     # the next arena that does not hold the input
+                if arenas.get(cur) == nxt:
                     nxt ^= 1
-                out = DevTensor(pp[nxt].ptr, shape)
-                nxt ^= 1
-            self.ops.append((kind, name, cur, out, kw))
-            if name in feats:
-                fmap[name] = out
-            cur = out
-        self.heads = []
-        for lv, (src, _, normed, _) in enumerate(LEVELS):
-            f = fmap[src]
-            n_, fh, fw, fc = f.shape
-            if normed:
-                g = self.alloc(f.shape) if keep else f          # in place: the pool has already read f
-                self.ops.append(("l2norm", src + "_norm", f, g, dict(npix=n_ * fh * fw, w=self.net.norms[src])))
-                f = g
-            hd = self.alloc((N, fh, fw, HEAD_C))
-            self.ops.append(("head", _head_name(src, normed) + "_mbox", f, hd,
-                             dict(N=N, IH=fh, IW=fw, OH=fh, OW=fw, stride=(1, 1), pad=(1, 1), relu=False, level=lv)))
-            self.heads.append(hd)
-        self.out_i = self.alloc((N, 6), np.int32)
-        self.out_s = self.alloc((N,), np.float32)
-        self.ops.append(("select", "select", None, self.out_i, {}))
-        self.ctx.sync()
-        with self.ctx.capture() as g:
-            for op in self.ops:
-                self._run(op)
-        self.graph = g.graph
-
-    def _weights(self, kind: str, name: str, kw: dict) -> ConvWeight:
-        return self.net.heads[kw["level"]] if kind == "head" else self.net.convs[name]
-
-    def _conv_kw(self, kw: dict) -> dict:
-        return {k: v for k, v in kw.items() if k != "level"}
-
-    def _run(self, op):
-        kind, name, x, y, kw = op
-        ctx = self.ctx
-        if kind == "prep":
-            ctx.s3fd_prep(self.frames, self.N, self.H, self.W, y)
-        elif kind in ("conv", "head"):
-            ctx.conv(x, self._weights(kind, name, kw), y, **self._conv_kw(kw))
-        elif kind == "pool":
-            ctx.maxpool2x2(x, kw["N"], kw["H"], kw["W"], y)
-        elif kind == "l2norm":
-            ctx.l2norm(x, kw["npix"], kw["w"], L2_EPS, y)
-        elif kind == "select":
-            ctx.s3fd_select(self.heads, self.N, THRESH, self.out_i, self.out_s)
-        else:
-            raise ValueError(kind)
-
-    def conv_variants(self) -> dict:
-        """name -> the kernel instance (Ctx.conv_plan) each conv and head runs in this graph."""
-        return {name: self.ctx.conv_plan(x, self._weights(kind, name, kw), y, **self._conv_kw(kw))
-                for kind, name, x, y, kw in self.ops if kind in ("conv", "head")}
+                arenas[name], nxt = nxt, nxt ^ 1
+            cur = name
+        for (src, _, normed, _), L in zip(LEVELS, net.heads):
+            shape = bufs[src][0]
+            f = (src, 0, shape[3])
+            if normed:                                      # in place unless keep_layers: the pool has already read f
+                if keep_layers:
+                    bufs[L.src[0]] = bufs[src]
+                steps.append(Step(L.src[0], src=f, dst=L.src if keep_layers else f,
+                                  run=lambda s, x, y, g=net.norms[src]: s.ctx.l2norm(x, x.rows, g, L2_EPS, y)))
+            bufs[L.name] = (shape[:3] + (HEAD_C,), np.float16)
+            steps.append(Step(L.name, L, src=None if keep_layers else f))
+        bufs["out_i"], bufs["out_s"] = ((N, 6), np.int32), ((N,), np.float32)
+        heads = [L.name for L in net.heads]
+        steps.append(Step("select", run=lambda s, x, y: s.ctx.s3fd_select([s.buf[n] for n in heads], s.N, THRESH, s.buf["out_i"],
+                                                                            s.buf["out_s"])))
+        super().__init__(N, bufs, steps, ctx, arenas=arenas)
+        self.heads = [self.buf[n] for n in heads]
 
     def run_raw(self, frames_u8: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
         """frames u8 BGR [n <= N, H, W, 3] -> (int32 [n, 6] = found, x1, y1, x2, y2, anchor; float32 [n] winning score)."""
@@ -214,14 +181,7 @@ class S3FDDetector(GraphSession):
         n = frames_u8.shape[0]
         if frames_u8.shape[1:] != (self.H, self.W, 3) or not 1 <= n <= self.N:
             raise ValueError(f"expected up to {self.N} frames of {self.H}x{self.W}x3, got {frames_u8.shape}")
-        if n < self.N:   # images are independent: pad with copies of the last frame
-            frames_u8 = np.concatenate([frames_u8, np.repeat(frames_u8[-1:], self.N - n, 0)], 0)
-        with self.ctx.lock:
-            self.ctx.h2d(self.frames, frames_u8)
-            self.graph.launch()
-            oi = self.ctx.download(self.out_i)
-            os_ = self.ctx.download(self.out_s)
-        return oi[:n], os_[:n]
+        return tuple(self.replay({"frames": frames_u8}, ("out_i", "out_s")))
 
     def detect(self, frames_u8: np.ndarray) -> List[Optional[Tuple[int, int, int, int]]]:
         oi, _ = self.run_raw(frames_u8)

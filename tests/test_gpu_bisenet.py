@@ -4,7 +4,7 @@ pinned to the unmodified reference by tests/test_bisenet_oracle.py).  Everything
 * bisenet_prep and maxpool3x3s2 bit-exact against numpy.
 * chan_gate and chan_scale_add against float64 within derived bounds (fp32 sums of ceil(HW / T) + T terms, FMA chains of the
   mat-vec length, one fp16 rounding for chan_scale_add).
-* Every planner conv against float64 on its own fp16 GPU input with the per-element bound of tests/test_gpu_pfld.py (plus the
+* Every planner conv against float64 on its own fp16 GPU input with the per-element bound of tests/layer_bound.py (plus the
   residual, and for the fused nearest-2x convs one fp16 rounding of the summed sub-pixel weights).  Padded channels are exactly 0,
   every activation stays below 2^14, and the test asserts which kernel each conv ran.
 * bisenet_upsample_argmax on its own fp16 logits: labels equal the float64 arg-max wherever the top-2 margin exceeds twice the fp32
@@ -26,16 +26,13 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from conv_check import SAFETY, SUB16, U16, V32
+from layer_bound import conv_bound
 from oracle import bisenet_ref as R
 from oracle import pfld_ref
 
 pytestmark = pytest.mark.gpu
 
-SAFETY = 1.25
-U16 = 2.0 ** -11
-SUB16 = 2.0 ** -25
-V32 = 2.0 ** -24
-ULP32 = 2.0 ** -23
 # largest |logit| error of the fp16 network against the float64 oracle, end to end at B = 16 and 5 on the synthetic weights
 # (measured on an H100 80GB HBM3: 4.9e-3 at B = 16, 6.2e-3 at B = 5); T_LABEL = 4x that
 LOGIT_ERR = 6.5e-3
@@ -176,31 +173,15 @@ def test_every_conv_against_float64(net, N):
     variants = p.conv_variants()
     ctx, bad, report = p.ctx, [], []
     imgs = [0, N - 1]
-    for L in net.layers:
+    for L in [st.layer for st in p.steps if st.layer]:
         xb = ctx.download(p.buf[L.src[0]])[imgs][..., L.src[1]:L.src[1] + L.src[2]]
         yfull = ctx.download(p.buf[L.dst[0]])[imgs]
         assert np.isfinite(yfull).all(), L.name
         got = _nchw(yfull[..., L.dst[1]:L.dst[1] + L.dst[2]])
-        x = _nchw(xb)
-        if L.up:
-            x = F.interpolate(x, scale_factor=2, mode="nearest")
         w = torch.from_numpy(L.w).to("cuda", torch.float64)
-        bb = torch.from_numpy(L.b).to("cuda", torch.float64)[None, :, None, None]
-        conv = F.conv2d(x, w, stride=L.stride, padding=L.pad)
-        A = F.conv2d(x.abs(), w.abs(), stride=L.stride, padding=L.pad)
-        pre = conv + bb
-        extra = torch.zeros_like(A)
-        if L.res is not None:
-            # the epilogue may round conv + bias to fp16 before it adds the residual: one more fp16 rounding of that sum
-            r = _nchw(ctx.download(p.buf[L.res[0]])[imgs][..., L.res[1]:L.res[1] + L.res[2]])
-            extra = r.abs() + (U16 / V32) * pre.abs()
-            pre = pre + r
-        ref = torch.relu(pre) if L.relu else pre
-        K = w.shape[1] * w.shape[2] * w.shape[3]
-        acc = 18 * math.ceil(K / 16) * ULP32 * A + (3 + min(32, K // 128)) * V32 * (A + bb.abs() + extra)
-        if L.up:
-            acc = acc + U16 * A                                    # the summed sub-pixel weights are rounded to fp16 once
-        bound = SAFETY * (acc + U16 * ref.abs() + SUB16)
+        b = torch.from_numpy(L.b).to("cuda", torch.float64)
+        r = None if L.res is None else _nchw(ctx.download(p.buf[L.res[0]])[imgs][..., L.res[1]:L.res[1] + L.res[2]])
+        ref, bound = conv_bound(_nchw(xb), w, b, L.stride, L.pad, L.relu, r=r, up=L.up)
         ratio = ((got - ref).abs() / bound).max().item()
         real = np.abs(L.w).reshape(L.w.shape[0], -1).max(1) > 0
         if (~real).any():

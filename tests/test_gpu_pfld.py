@@ -3,7 +3,7 @@ to the unmodified reference by tests/test_pfld_oracle.py).
 
 * pfld_prep bit-exact against numpy's fp16(fp32(v) / 255).
 * Every conv (planner) and depthwise layer, conv8 as a 2304-wide GEMM included, against float64 computed from that layer's own fp16
-  GPU input and the padded fp16 weights, with the per-element bound of tests/test_gpu_s3fd.py (A = sum |w||x|, u = 2^-11,
+  GPU input and the padded fp16 weights, with the per-element bound of tests/layer_bound.py (A = sum |w||x|, u = 2^-11,
   v = 2^-24, K the accumulation length): 1.25 (18 ceil(K/16) 2^-23 A + 3 v (A + |b|) + u |ref| + 2^-25 + min(32, K/128) v (A + |b|)).
   For the depthwise kernel (an fp32 FMA chain of 9 taps) the same formula is a loose bound.  Every padded channel must be exactly 0,
   every activation below 2^14 (a 4x margin to the fp16 range), and the test asserts which planner kernel each conv ran.
@@ -26,17 +26,13 @@ import cv2
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
+from conv_check import SAFETY, V32
+from layer_bound import conv_bound
 from oracle import pfld_ref as R
 
 pytestmark = pytest.mark.gpu
 
-SAFETY = 1.25
-U16 = 2.0 ** -11
-SUB16 = 2.0 ** -25
-V32 = 2.0 ** -24
-ULP32 = 2.0 ** -23
 TOL_NORM = 2e-4          # end to end, fp16 network vs float64 oracle, in units of the crop size (4x the largest error measured)
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 GATHER, HALO = 0, 1
@@ -95,19 +91,8 @@ def _nchw(a):
     return torch.from_numpy(np.asarray(a, np.float32)).permute(0, 3, 1, 2).to("cuda", torch.float64)
 
 
-def _bound(x, w, b, stride, pad, groups, relu):
-    conv = F.conv2d(x, w, stride=stride, padding=pad, groups=groups)
-    A = F.conv2d(x.abs(), w.abs(), stride=stride, padding=pad, groups=groups)
-    bb = b[None, :, None, None]
-    pre = conv + bb
-    ref = torch.relu(pre) if relu else pre
-    K = w.shape[1] * w.shape[2] * w.shape[3]
-    acc = 18 * math.ceil(K / 16) * ULP32 * A + 3 * V32 * (A + bb.abs()) + min(32, K // 128) * V32 * (A + bb.abs())
-    return ref, SAFETY * (acc + U16 * ref.abs() + SUB16)
-
-
 @pytest.mark.parametrize("N", [16, 5])
-def test_every_layer_against_float64(net, N):
+def test_every_step_against_float64(net, N):
     from livetalking_b200.pfld import PFLDLandmarker
     lm = PFLDLandmarker(net, N)
     crops = _crops(N, 11 + N)
@@ -115,9 +100,7 @@ def test_every_layer_against_float64(net, N):
     variants = lm.conv_variants()
     ctx, bad, report = lm.ctx, [], []
     imgs = [0, N - 1]
-    for kind, L, x, y in lm.ops:
-        if kind in ("prep", "head"):
-            continue
+    for L in [st.layer for st in lm.steps if st.layer]:
         xb = ctx.download(lm.buf[L.src[0]])[imgs]
         yb = ctx.download(lm.buf[L.dst[0]])[imgs]
         assert np.isfinite(yb).all(), L.name
@@ -128,13 +111,12 @@ def test_every_layer_against_float64(net, N):
         got = _nchw(yb[..., L.dst[1]:L.dst[1] + L.dst[2]])
         w = torch.from_numpy(L.w).to("cuda", torch.float64)
         b = torch.from_numpy(L.b).to("cuda", torch.float64)
-        k = w.shape[-1]
-        ref, bound = _bound(xin, w, b, L.stride, k // 2, L.w.shape[0] if kind == "dw" else 1, L.relu)
+        ref, bound = conv_bound(xin, w, b, L.stride, L.pad, L.relu, groups=L.w.shape[0] if L.kind == "dw" else 1)
         ratio = ((got - ref).abs() / bound).max().item()
         real = np.abs(L.w).reshape(L.w.shape[0], -1).max(1) > 0
         assert torch.all(got[:, torch.from_numpy(~real).cuda()] == 0), f"{L.name}: a padded channel is not zero"
         amax = got.abs().max().item()
-        report.append((L.name, kind, variants.get(L.name), ratio, amax))
+        report.append((L.name, L.kind, variants.get(L.name), ratio, amax))
         if ratio > 1.0:
             bad.append((L.name, ratio))
         assert amax < 2.0 ** 14, f"{L.name}: largest activation {amax}"

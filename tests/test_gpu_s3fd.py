@@ -17,7 +17,6 @@
   the softmax being at most 1/4 on each of the two logits), boxes within 1 px of the oracle's decode of that anchor.
 * generate_avatar on a generated video (img_size 256, the engine's wav2lip256 face size): coords.pkl and face PNGs equal to the host path driven by the oracle's detections, and
   the wav2lip plugin loading the result from the directory and from avatar.ltbav."""
-import math
 import os
 import pickle
 import zlib
@@ -27,15 +26,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from conv_check import SAFETY, SUB16, U16, V32
+from layer_bound import conv_bound
 from oracle import s3fd_ref as R
 
 pytestmark = pytest.mark.gpu
-
-SAFETY = 1.25
-U16 = 2.0 ** -11
-SUB16 = 2.0 ** -25
-V32 = 2.0 ** -24
-ULP32 = 2.0 ** -23
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -85,17 +80,6 @@ def test_prep_and_maxpool_bit_exact():
     ctx.close()
 
 
-def _conv_bound(x, w, b, stride, pad, relu):
-    conv = F.conv2d(x, w, stride=stride, padding=pad)
-    A = F.conv2d(x.abs(), w.abs(), stride=stride, padding=pad)
-    bb = b[None, :, None, None]
-    pre = conv + bb
-    ref = torch.relu(pre) if relu else pre
-    K = w.shape[1] * w.shape[2] * w.shape[3]
-    acc = 18 * math.ceil(K / 16) * ULP32 * A + 3 * V32 * (A + bb.abs()) + min(32, K // 128) * V32 * (A + bb.abs())
-    return ref, SAFETY * (acc + U16 * ref.abs() + SUB16)
-
-
 HALO, GATHER = 1, 0
 _TRUNK_3X3 = ["conv1_1", "conv1_2", "conv2_1", "conv2_2", "conv3_1", "conv3_2", "conv3_3", "conv4_1", "conv4_2", "conv4_3", "conv5_1",
               "conv5_2", "conv5_3"]
@@ -118,7 +102,7 @@ def _images(ctx, t, imgs):
 
 
 @pytest.mark.parametrize("run", list(LAYER_RUNS))
-def test_every_layer_against_float64(net, sd, run):
+def test_every_step_against_float64(net, sd, run):
     from livetalking_b200.s3fd import S3FDDetector, LEVELS
     N, H, W, imgs, halo = LAYER_RUNS[run]
     frames = R.synth_frames(([35, 50, 0, 45] * 4)[:N], H, W, seed=11)
@@ -127,11 +111,13 @@ def test_every_layer_against_float64(net, sd, run):
     variants = det.conv_variants()
     ctx, bad, report = det.ctx, [], []
     head_src = {f"{s}_norm_mbox" if n else f"{s}_mbox": lv for lv, (s, _, n, _) in enumerate(LEVELS)}
-    for kind, name, x, y, kw in det.ops:
-        if kind in ("prep", "select"):
+    for st in det.steps:
+        name = st.name
+        if name in ("prep", "select"):
             continue
-        xin = _images(ctx, x, imgs)
-        got = _images(ctx, y, imgs)
+        kind = "head" if name in head_src else "conv" if st.layer else "pool" if name.endswith("_pool") else "l2norm"
+        xin = _images(ctx, det.view(st.src), imgs)
+        got = _images(ctx, det.view(st.dst), imgs)
         assert torch.isfinite(got).all(), name
         if kind == "pool":
             assert torch.equal(got, F.max_pool2d(xin, 2, 2)), name
@@ -148,13 +134,13 @@ def test_every_layer_against_float64(net, sd, run):
             if name == "conv1_1":
                 xin = xin[:, :3]
             w16 = w.half().double()
-            ref, bound = _conv_bound(xin, w16, sd[name + ".bias"].to("cuda", torch.float64), e[4], e[5], True)
+            ref, bound = conv_bound(xin, w16, sd[name + ".bias"].to("cuda", torch.float64), e[4], e[5], True)
         else:
             lv = head_src[name]
             pre = name[:-5]
             w = torch.cat([sd[pre + "_mbox_conf.weight"], sd[pre + "_mbox_loc.weight"]]).to("cuda", torch.float64).half().double()
             b = torch.cat([sd[pre + "_mbox_conf.bias"], sd[pre + "_mbox_loc.bias"]]).to("cuda", torch.float64)
-            ref, bound = _conv_bound(xin, w, b, 1, 1, False)
+            ref, bound = conv_bound(xin, w, b, 1, 1, False)
             assert torch.all(got[:, w.shape[0]:] == 0), f"{name}: padded head channels not zero"
             got = got[:, :w.shape[0]]
         ratio = ((got - ref).abs() / bound).max().item()

@@ -172,6 +172,9 @@ def _weights(name):
     if name == "s3fd":
         from oracle import s3fd_ref as R
         return R.synth_state_dict(0)
+    if name == "bisenet":
+        from oracle import bisenet_ref as R
+        return R.synth_state_dict(0)
     from oracle import pfld_ref as R
     return R.synth_state_dict(0), R.read_mean_face(os.path.join(GOLDEN, "pfld_mean_face.txt"))
 
@@ -277,8 +280,15 @@ def _case_pfld(mctx):
     return lambda ctx: PFLDLandmarker(net, 2, ctx=ctx), [], lambda s: s.run(_u8(2, 192, 192, 3), [[100, 100], [120, 90]])
 
 
+def _case_bisenet(mctx):
+    from livetalking_b200.bisenet import BiSeNetNet, BiSeNetParser
+    net = BiSeNetNet.from_state_dict(_weights("bisenet"), mctx)
+    return lambda ctx: BiSeNetParser(net, 2, ctx=ctx), [], lambda s: s.parse(_u8(2, 512, 512, 3))
+
+
 CASES = {f.__name__[len("_case_"):]: f for f in (_case_ultralight, _case_ultralight_batch, _case_hubert, _case_hubert_batch,
-                                                   _case_musetalk, _case_musetalk_batch, _case_whisper, _case_s3fd, _case_pfld)}
+                                                   _case_musetalk, _case_musetalk_batch, _case_whisper, _case_s3fd, _case_pfld,
+                                                   _case_bisenet)}
 PASTE_ONLY = {"ultralight_paste_only": _case_ultralight_paste_only, "musetalk_paste_only": _case_musetalk_paste_only}
 
 
@@ -334,6 +344,23 @@ def test_a_session_constructor_that_raises_releases_its_allocations(monkeypatch,
     with pytest.raises(RuntimeError):
         UltraLightSession(av, 2, ctx=ctx)
     assert ctx.live == models and set(before) <= set(ctx.live) and not ctx.closed
+
+
+def test_a_layer_plan_that_reads_an_overwritten_arena_buffer_raises():
+    """Buffers of one arena share memory: a step that reads one after another of them was written is refused at construction,
+    before anything is allocated."""
+    from livetalking_b200.layerplan import LayerSession, Step
+    ctx = _RecordingCtx()
+    bufs = {name: ((1, 4, 4, 16), np.float16) for name in ("in", "a", "b", "c")}
+    copy = lambda s, x, y: s.ctx.copy_channels(x, y)                # noqa: E731
+    ok = [Step("a", src=("in", 0, 16), dst=("a", 0, 16), run=copy), Step("b", src=("a", 0, 16), dst=("b", 0, 16), run=copy)]
+    LayerSession(1, bufs, ok, ctx, arenas={"a": 0, "b": 0}).close()
+    assert ctx.live == {}
+    bad = ok + [Step("c", src=("a", 0, 16), dst=("c", 0, 16), run=copy)]
+    with pytest.raises(ValueError, match="reads a after b"):
+        LayerSession(1, bufs, bad, ctx, arenas={"a": 0, "b": 0})
+    assert ctx.live == {} and not ctx.closed
+    LayerSession(1, bufs, bad, ctx, arenas={"a": 0, "b": 1}).close()
 
 
 # ---------------------------------------------------------------------------------------------------------------- GPU

@@ -12,7 +12,6 @@ import argparse
 import json
 import os
 import shutil
-import subprocess
 import sys
 import tempfile
 import time
@@ -20,22 +19,12 @@ import time
 import numpy as np
 import torch
 
+from gpu_bench import events_ms, gpu_info
+
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from oracle import bisenet_ref as R  # noqa: E402
 from oracle import pfld_ref, s3fd_ref  # noqa: E402
-
-
-def _events(fn, iters):
-    fn()
-    torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    a.record()
-    for _ in range(iters):
-        fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) / iters
 
 
 def main():
@@ -44,21 +33,15 @@ def main():
     args = ap.parse_args()
     from livetalking_b200 import engine
     from livetalking_b200.bisenet import BiSeNetNet, BiSeNetParser, gflop_per_frame
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    card = ", ".join(gpu_info())
     engine.set_device(0)
     sd = R.synth_state_dict(0)
     net = BiSeNetNet.from_state_dict(sd)
     B = 16
     p = BiSeNetParser(net, B)
     crops = np.ascontiguousarray(pfld_ref.synth_video_frames(B, 512, 512, seed=1)[..., ::-1])
-    p.ctx.h2d(p.rgb, crops)
-    p.graph.launch()
-    p.ctx.sync()
-    t0 = time.perf_counter()
-    for _ in range(args.iters):
-        p.graph.launch()
-    p.ctx.sync()
-    graph_ms = (time.perf_counter() - t0) / args.iters * 1e3
+    p.ctx.h2d(p.buf["rgb"], crops)
+    graph_ms = events_ms(p.graph.launch, args.iters, warmup=1, stream=torch.cuda.ExternalStream(p.ctx.cuda_stream))
     t0 = time.perf_counter()
     for _ in range(10):
         p.parse(crops)
@@ -84,9 +67,9 @@ def main():
                 return R.upsample(R.forward(fw, xd)).argmax(1)
         return run
     it = max(3, args.iters // 10)
-    eager32 = _events(run_dtype(torch.float32, x32), it)
-    eager16 = _events(run_dtype(torch.float16, x32), it)
-    eager1 = _events(run_dtype(torch.float32, x32[:1]), it)
+    eager32 = events_ms(run_dtype(torch.float32, x32), it, warmup=1)
+    eager16 = events_ms(run_dtype(torch.float16, x32), it, warmup=1)
+    eager1 = events_ms(run_dtype(torch.float32, x32[:1]), it, warmup=1)
 
     from livetalking_b200.plugin import musetalk_face_parsing as mfp
     from livetalking_b200.plugin import musetalk_genavatar as G

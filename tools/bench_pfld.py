@@ -16,32 +16,16 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
 
 import numpy as np
 
+from gpu_bench import events_ms, gpu_info
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-
-
-def _gpu_info():
-    out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
-                         timeout=30).stdout.strip().splitlines()[0]
-    name, pl = [s.strip() for s in out.split(",")]
-    return name, pl
-
-
-def _events_ms(torch, stream, fn, iters):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(stream)
-    for _ in range(iters):
-        fn()
-    e1.record(stream)
-    e1.synchronize()
-    return e0.elapsed_time(e1) / iters
 
 
 def main():
@@ -65,25 +49,17 @@ def main():
     lm = PFLDLandmarker(net, N)
     crops = R.synth_video_frames(N, 192, 192, seed=1)
     lm.run(crops, np.full((N, 2), 200, np.int32))         # uploads the crops; the timed replays reuse them
-    stream = torch.cuda.ExternalStream(lm.ctx.cuda_stream)
-    for _ in range(5):
-        lm.graph.launch()
-    lm.ctx.sync()
-    ms = _events_ms(torch, stream, lm.graph.launch, a.iters)
+    ms = events_ms(lm.graph.launch, a.iters, warmup=5, stream=torch.cuda.ExternalStream(lm.ctx.cuda_stream))
 
     torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
     x = R.prep(crops).cuda()
     sd32 = {k: (v.cuda().float() if v.is_floating_point() else v) for k, v in sd.items()}
     sd16 = {k: (v.cuda().half() if v.is_floating_point() else v) for k, v in sd.items()}
-    cur = torch.cuda.current_stream()
     res = {}
     with torch.no_grad():
         for name, fn in (("fp32", lambda: R.forward_train(sd32, x)), ("fp16", lambda: R.forward_train(sd16, x.half())),
                          ("fp32_b1", lambda: R.forward_train(sd32, x[:1]))):
-            for _ in range(3):
-                fn()
-            torch.cuda.synchronize()
-            res[name] = _events_ms(torch, cur, fn, max(5, a.iters // 5))
+            res[name] = events_ms(fn, max(5, a.iters // 5), warmup=3)
 
     tmp = tempfile.mkdtemp(prefix="bench_pfld_")
     nfr = int(round(a.video_seconds * 25))
@@ -101,7 +77,7 @@ def main():
     G.generate_avatar(vid, "bench", save_path=os.path.join(tmp, "avatars"), detector=R.ReplayDetector(R.face_records(boxes)),
                       make_landmarker=lambda n: PFLDLandmarker(net, n), timings=split)
     total = time.perf_counter() - t0
-    name, pl = _gpu_info()
+    name, pl = gpu_info()
     lm.close()
     gf = gflop_per_frame() * N
     print(json.dumps({

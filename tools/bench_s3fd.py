@@ -15,38 +15,16 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
 
-import numpy as np
+from gpu_bench import events_ms, gpu_info
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 PEAK_TFLOPS = 989.0
-
-
-def _gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
-                             timeout=30).stdout.strip().splitlines()[0]
-        name, pl = [s.strip() for s in out.split(",")]
-        return name, pl
-    except Exception:
-        import torch
-        return torch.cuda.get_device_name(0), "unknown"
-
-
-def _events_ms(torch, stream, fn, iters):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(stream)
-    for _ in range(iters):
-        fn()
-    e1.record(stream)
-    e1.synchronize()
-    return e0.elapsed_time(e1) / iters
 
 
 def main():
@@ -71,11 +49,7 @@ def main():
     det = S3FDDetector(net, N, H, W)
     frames = R.synth_frames([35 + (i % 3) * 5 for i in range(N)], H, W, seed=1)
     det.run_raw(frames)                                   # uploads the frames; the timed replays reuse them
-    stream = torch.cuda.ExternalStream(det.ctx.cuda_stream)
-    for _ in range(3):
-        det.graph.launch()
-    det.ctx.sync()
-    ms = _events_ms(torch, stream, det.graph.launch, a.iters)
+    ms = events_ms(det.graph.launch, a.iters, warmup=3, stream=torch.cuda.ExternalStream(det.ctx.cuda_stream))
     gflop = gflop_per_frame(H, W) * N
     tflops = gflop / ms                                  # GFLOP per ms = TFLOP/s
 
@@ -84,7 +58,6 @@ def main():
     x = R.prep(frames, "cuda")
     sd_h = {k: v.cuda().half() for k, v in sd.items()}
     x_h = x.half().contiguous(memory_format=torch.channels_last)
-    cur = torch.cuda.current_stream()
     with torch.no_grad():
         def eager32():
             R.select(R.forward(sd, x))
@@ -93,10 +66,7 @@ def main():
             R.select(R.forward(sd_h, x_h))
         res = {}
         for name, fn in (("fp32", eager32), ("fp16_channels_last", eager16)):
-            for _ in range(2):
-                fn()
-            torch.cuda.synchronize()
-            res[name] = _events_ms(torch, cur, fn, max(3, a.iters // 4))
+            res[name] = events_ms(fn, max(3, a.iters // 4), warmup=2)
 
     tmp = tempfile.mkdtemp(prefix="bench_s3fd_")
     nfr = int(round(a.video_seconds * 25))
@@ -115,7 +85,7 @@ def main():
     split = {}
     G.generate_avatar(vid, "bench", save_path=os.path.join(tmp, "avatars"), face_det_batch_size=N, weights_path=wpath, timings=split)
     total = time.perf_counter() - t0
-    name, pl = _gpu_info()
+    name, pl = gpu_info()
     det.close()
     print(json.dumps({
         "gpu": name, "power_limit": pl, "batch": N, "height": H, "width": W,
